@@ -26,6 +26,11 @@ One JSON line on stdout (rank 0).  Keys beyond the base contract:
   e2e                 same metric through the host-buffer C-ABI entry point a deployment
                       calls (pinned host inputs in, pinned host outputs out, H2D + D2H inside
                       the timed region)
+
+--dump-outputs DIR writes what the timed path returned in its last timed step as DIR/<name>.npy
+(float32).  Inputs are seeded, so two builds run with the same arguments can be compared array
+for array.  An output larger than DUMP_MAX_ELEMS values is stored as a fixed sample: the values
+at DUMP_MAX_ELEMS flat indices drawn once from a seeded generator (sorted), the same for every run.
 """
 import argparse
 import json
@@ -46,10 +51,7 @@ V = D * HO * WO
 FLOPS_PER_FRAME = 521856.0 * V                       # SURVEY.md 8(d)
 IO_BYTES_PER_FRAME = 2 * 32 * H * W * 4 + 5.25e6 + 33 * V * 4
 KITTI_WORKLOAD = 'dfm_r34_1x8_kitti-3d-3class D=112 384x1248 batch=1'
-# dram__bytes_read.sum + dram__bytes_write.sum of one launch of the dominant kernel, from the
-# committed `ncu --set full` capture (profiles/): kitti: conv_tc 32->32 full resolution
-NCU_TRAFFIC = {'kitti': (973.0e6, 'profiles/r02_ncu_conv_tc_dominant_final.csv '
-                                  '(587.1 MB read + 386.0 MB written per launch)')}
+DUMP_MAX_ELEMS = 1 << 21   # per dumped array: 8 MB of float32, at most six arrays a workload
 WAYMO = {
     'waymo_mv': dict(T=1, agg='mean', neck='OutdoorImVoxelNeck', flops=3.212e12,
                      name='multiview-dfm_r101_dcn_2x16_waymoD5 (5 views, 832x1248 input) '
@@ -66,7 +68,8 @@ def peaks():
         j = json.load(open(p))
         return dict(bf16=j.get('bf16_tflops_sustained', j.get('bf16_tflops')),
                     hbm=j.get('hbm_gbs'), src='measured')
-    return dict(bf16=1400.0, hbm=6650.0, src='fallback')  # B200_PROFILING.md
+    # NVIDIA H100 SXM data sheet (700 W): dense BF16 tensor, HBM3 bandwidth
+    return dict(bf16=989.0, hbm=3350.0, src='H100 SXM data sheet')
 
 
 class ClockSampler:
@@ -243,7 +246,7 @@ def _setup_dist():
     world = int(os.environ.get('WORLD_SIZE', '1'))
     local = int(os.environ.get('LOCAL_RANK', '0'))
     if not torch.cuda.is_available():
-        raise SystemExit('bench.py needs a B200: there is no CPU path (use --impl reference)')
+        raise SystemExit('bench.py needs an H100: there is no CPU path (use --impl reference)')
     torch.cuda.set_device(local)
     if world > 1:
         # NCCL's INFO lines (if the caller set NCCL_DEBUG) must not interleave with the one
@@ -309,7 +312,7 @@ def run_kitti(args):
     capi.lib()
 
     # two different pairs per rank so consecutive steps never re-read the same inputs;
-    # the per-step working set (~7 GB of activations) is far larger than the 126 MB L2
+    # the per-step working set (~7 GB of activations) is far larger than the 50 MB L2
     pairs = []
     for i in range(2):
         cur, prev, metas, params = syn.make_kitti_pair(100 + 2 * rank + i, H, W, D,
@@ -326,14 +329,21 @@ def run_kitti(args):
     head.depth_samples = _depths(cfg, 1)
     head.downsample_factor = 4
 
+    last = {}
+
     def step(i):
         cur, prev, metas, _, _ = pairs[i % 2]
         cost, stereo, mono = model(cur, prev, metas)
-        return head(cost)
+        vol, sm, preds = head(cost)
+        last.update(cost=cost, stereo_feat=stereo, mono_feat=mono, depth_preds=preds)
+        last.update({k: v for k, v in (('depth_volume', vol), ('depth_softmax', sm)) if v is not None})
+        return vol, sm, preds
 
     ms_total, prof, clocks, launches, tc_launches, barrier = _timed_loop(
         step, args, world, rank, local, capi)
     fps = world * args.steps / (ms_total * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
 
     # ---- e2e: DfM.simple_test's hot-path segment through the host-buffer C-ABI call -------
     # pinned host (cur, prev, sem) in -> voxel features + depth_preds out (what the BEV stage
@@ -419,11 +429,10 @@ def run_kitti(args):
         ach = per_launch_flops / per_launch_s / 1e12
         roof = dict(bound='tensor', kernel=dom_key, achieved=round(ach, 2), peak=pk['bf16'],
                     unit='TFLOP/s', frac=round(ach / pk['bf16'], 4),
-                    traffic=NCU_TRAFFIC['kitti'][0], traffic_source=NCU_TRAFFIC['kitti'][1],
-                    algorithmic_bytes=2 * V * 32 * 4,
+                    traffic=None, algorithmic_bytes=2 * V * 32 * 4,
                     executed_bf16_tflops=round(3 * ach, 1),
                     executed_frac_of_peak=round(3 * ach / pk['bf16'], 4),
-                    peak_source=pk['src'] + ' bf16 dense (sustained)',
+                    peak_source=pk['src'] + ' bf16 dense',
                     launches_per_step=r['launches'] / args.steps,
                     ms_per_launch=round(per_launch_s * 1e3, 4),
                     note='achieved = algorithmic fp32 conv FLOPs (2*V*27*Cin*Cout); the kernel '
@@ -475,7 +484,7 @@ def run_kitti(args):
         scaling='weak', vs_baseline=None, dtype='f32 (bf16x2 split operands, fp32 accumulate)',
         data='synthetic',
         config=dict(workload=KITTI_WORKLOAD, pairs_per_step=world, planes=D, feature_hw=[H, W],
-                    l2='per-step working set ~7 GB >> 126 MB L2; two input pairs alternate',
+                    l2='per-step working set ~7 GB >> 50 MB L2; two input pairs alternate',
                     multi_gpu='replicas: one independent pair per rank, no data-path collective',
                     outputs='cost + stereo_feat + mono_feat + DepthHead(volume, softmax, preds)'),
         clocks=clocks,
@@ -536,13 +545,19 @@ def run_waymo(args):
         temporal_aggregate, valid_sample, neck_3d = spec['agg'], True, neck
     host = Host()
 
+    last = {}
+
     def step(i):
         feats, meta, _ = samples[i % 2]
-        return host.feature_transformation(feats[None], [meta], nv, t)[0]
+        bev = host.feature_transformation(feats[None], [meta], nv, t)[0]
+        last.update(bev=bev)
+        return bev
 
     ms_total, prof, clocks, launches, tc_launches, barrier = _timed_loop(
         step, args, world, rank, local, capi)
     sps = world * args.steps / (ms_total * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
 
     # ---- e2e: pinned host features in, pinned host BEV out --------------------------------
     # every step copies its sample H2D (166 / 83 MB) and its BEV map D2H (67.6 MB) inside the timed
@@ -609,7 +624,7 @@ def run_waymo(args):
                 achieved=round(ach, 2), peak=pk['bf16'], unit='TFLOP/s',
                 frac=round(ach / pk['bf16'], 4), traffic=None,
                 executed_bf16_tflops=round(3 * ach, 1),
-                peak_source=pk['src'] + ' bf16 dense (sustained)',
+                peak_source=pk['src'] + ' bf16 dense',
                 ms_per_step=round(neck_ms, 3), share_of_step=round(neck_ms * args.steps / ms_total, 4),
                 note='algorithmic fp32 conv FLOPs of the neck (SURVEY.md 8d) / summed conv time')
     roof_lift = dict(bound='hbm', kernel='lift (NCHW->NHWC staging of the 2-D features + lift_cl_kernel, channels-last volume out)',
@@ -636,7 +651,7 @@ def run_waymo(args):
         data='synthetic',
         config=dict(workload=spec['name'], samples_per_step=world, frames=t, views=nv,
                     n_voxels=syn.WAYMO_N_VOXELS, frame_unit='one multi-view sample',
-                    l2='volume 0.2-0.4 GB and 0.4-1.5 GB of activations per layer >> 126 MB L2; '
+                    l2='volume 0.2-0.4 GB and 0.4-1.5 GB of activations per layer >> 50 MB L2; '
                        'two input samples alternate',
                     multi_gpu='replicas: one independent sample per rank'),
         clocks=clocks,
@@ -654,6 +669,19 @@ def run_waymo(args):
     print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes each tensor as out_dir/<name>.npy (float32): whole when it has at most
+    DUMP_MAX_ELEMS values, else the values at a fixed seeded sample of flat indices."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in sorted(arrays.items()):
+        a = t.detach().float().cpu().numpy().reshape(-1)
+        if a.size > DUMP_MAX_ELEMS:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_MAX_ELEMS, replace=False))
+            a = a[idx]
+        np.save(os.path.join(out_dir, name + '.npy'), np.ascontiguousarray(a, dtype=np.float32))
 
 
 def _depths(cfg, ds):
@@ -675,6 +703,8 @@ def main():
     ap.add_argument('--workload', default='kitti', choices=['kitti'] + sorted(WAYMO))
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-gpu-eager', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == 'reference':

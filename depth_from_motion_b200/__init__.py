@@ -1,4 +1,4 @@
-"""depth_from_motion_b200 -- B200-native DfM plane-sweep cost-volume path.
+"""depth_from_motion_b200 -- H100-native (sm_90a) DfM plane-sweep cost-volume path.
 
 Host-side mirror of the reference's plugin interface (registry + module
 classes) over the C-ABI CUDA library ``libdfm_b200.so`` (``include/dfm_b200.h``).

@@ -1,4 +1,4 @@
-"""In-tree build of the C-ABI CUDA library (nvcc, sm_100a only)."""
+"""In-tree build of the C-ABI CUDA library (nvcc, sm_90a only)."""
 import os
 import shutil
 import subprocess
@@ -9,7 +9,7 @@ SRC = os.path.join(HERE, 'csrc', 'dfm_b200.cu')
 OUT = os.path.join(HERE, 'libdfm_b200.so')
 DEPS = [os.path.join(HERE, 'csrc', f) for f in
         ('dfm_b200.cu', 'common.cuh', 'simt_kernels.cuh', 'conv_tc.cuh', 'conv_tc_neck.cuh',
-         'neck_api.inc', 'frustum_api.inc', 'frustum_kernels.cuh', 'pipeline_api.inc', 'bev_api.inc', 'tail_kernels.cuh', 'voxel_sample_api.inc', 'stereo_tail_api.inc', 'logits_tc.cuh')] + [os.path.join(HERE, '..', 'include', 'dfm_b200.h')]
+         'neck_api.inc', 'frustum_api.inc', 'frustum_kernels.cuh', 'pipeline_api.inc', 'bev_api.inc', 'tail_kernels.cuh', 'voxel_sample_api.inc', 'stereo_tail_api.inc', 'logits_tc.cuh', 'wgmma.cuh')] + [os.path.join(HERE, '..', 'include', 'dfm_b200.h')]
 
 
 def nvcc_path():
@@ -26,7 +26,7 @@ def up_to_date():
 def build(force=False, verbose=False):
     if up_to_date() and not force:
         return OUT
-    cmd = [nvcc_path(), '-gencode', 'arch=compute_100a,code=sm_100a', '-O3',
+    cmd = [nvcc_path(), '-gencode', 'arch=compute_90a,code=sm_90a', '-O3',
            '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC', '-shared',
            '-o', OUT, SRC]
     if verbose:

@@ -2,7 +2,7 @@
 
 The library is built in-tree by ``__graft_entry__.build()`` /
 ``depth_from_motion_b200/build.py`` as ``depth_from_motion_b200/libdfm_b200.so``.
-There is no fallback: if the library is missing, or no sm_100 GPU is visible
+There is no fallback: if the library is missing, or no sm_90 GPU is visible
 when a compute entry point is called, the caller gets a ``RuntimeError``.
 """
 import ctypes
@@ -126,7 +126,7 @@ def lib():
     if not library_built():
         raise RuntimeError(
             f'{LIB_PATH} is missing: run `python -c "import __graft_entry__ as g; '
-            'g.build()"` (nvcc, sm_100a). There is no CPU/PyTorch fallback.')
+            'g.build()"` (nvcc, sm_90a). There is no CPU/PyTorch fallback.')
     L = ctypes.CDLL(LIB_PATH)
     fp, vp, ip = POINTER(c_float), c_void_p, POINTER(c_int)
     L.dfm_last_error.restype = c_char_p

@@ -1,4 +1,4 @@
-// Shared device/host definitions for the DfM B200 library.
+// Shared device/host definitions for the DfM library.
 #pragma once
 #include <cuda_runtime.h>
 

@@ -1,4 +1,4 @@
-// tcgen05 tensor-core implicit-GEMM 3x3x3 convolution (stride 1, pad 1) for sm_100a.
+// wgmma tensor-core implicit-GEMM 3x3x3 convolution (stride 1, pad 1) for sm_90a.
 //
 // Formulation (see DESIGN.md "conv_tc"):
 //   * activations are channels-last fp32 in HBM; a persistent CTA owns an 8x16 (x,y)
@@ -6,33 +6,29 @@
 //     gather a 10x18 halo brick, apply the fused input transform (GroupNorm /
 //     BatchNorm affine, ReLU, residual add -- or the plane-sweep warp for the first
 //     layer), split every value into bf16 hi + bf16 lo and store both in shared
-//     memory in the UMMA K-major *no-swizzle* core-matrix layout
+//     memory in the K-major *no-swizzle* core-matrix layout
 //     [chunk of 8 channels][brick row][16 B].  In that layout a 3x3 in-plane tap is
 //     just a 16-byte-granular shift of the descriptor start address and the 8-row
-//     group stride (SBO) is the brick row pitch, so ONE brick serves all 9 taps
-//     (validated on hardware by tests/probe/probe_umma.cu).
+//     group stride (SBO) is the brick row pitch, so ONE brick serves all 9 taps.
 //   * the three dz taps are folded into the N dimension: one MMA of input plane z
 //     against the weight image rows [kz=2 | kz=1 | kz=0] accumulates into the three
-//     TMEM accumulator slots of output planes z-1, z, z+1 at once (N = 3*NCTA).
-//     Each input plane is therefore read from HBM/L2 once per tile, and the MMA runs
-//     at N = 96 where the SS-mode smem operand read stops being the bound
-//     (tests/probe/probe_mma_rate.cu: cycles/MMA = max(N/2, 32+N/4, 47)).
+//     accumulator blocks of output planes z-1, z, z+1 at once (N = 3*NCTA), so each
+//     input plane is read from HBM/L2 once per tile.
 //   * fp32 parity: x*w is evaluated as x_hi*w_hi + x_lo*w_hi + x_hi*w_lo on the bf16
-//     tensor pipe with fp32 accumulation in TMEM (~2^-17 relative), because a single
+//     tensor pipe with fp32 accumulation (~2^-17 relative), because a single
 //     TF32/bf16 pass does not hold the 1e-3 end-to-end tolerance through 22 layers.
 //   * weights (hi+lo images of all 27 taps, <= 110.6 KB) stay resident in shared
 //     memory for the life of the CTA; layers with Cin*Cout > 1024 are split over
 //     output-channel groups of NCTA = 1024/Cin handled by different CTAs.
-//   * warp roles: warps 0-3 epilogue (TMEM -> registers -> global, GroupNorm sums), warps 4-11
-//     loaders (two groups filling alternate stages), warp 12 issues every tcgen05.mma /
-//     tcgen05.commit from warp-uniform code; smem stages and TMEM slots are handed over with
-//     mbarriers.  Accumulators are only ever accumulated into: the epilogue re-zeroes a slot
-//     after draining it.
+//   * warp roles: warps 0-7 are two consumer warpgroups (64 accumulator rows each) that issue
+//     wgmma.mma_async into register accumulators and store the finished planes (GroupNorm sums
+//     on the way); warps 8-15 are loaders (two groups filling alternate stages).  Shared-memory
+//     stages are handed over with mbarriers.
 //   * modes: stride 1 (TC_S1), stride 2 (TC_S2, x/y parity sub-bricks) and the stride-2
 //     transposed conv (TC_T, 4 (px,py) parity classes per output plane); the work of a launch
 //     is cut "stream-K" style into equal contiguous (tile column, plane) ranges per CTA.
 //   * diagnosis: DFM_TC_ROLE_CYCLES=1 prints per-role busy / wait cycles of every launch,
-//     DFM_TC_DEBUG=<bits> disables roles (1 loaders, 2 epilogue, 8 proxy fence, 16 the
+//     DFM_TC_DEBUG=<bits> disables loader work (1 everything, 8 proxy fence, 16 the
 //     loaders' global loads, 32 the loaders' shared-memory stores).
 #pragma once
 #include <cuda.h>
@@ -40,10 +36,12 @@
 
 #include <algorithm>
 #include <cstdlib>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
 #include "simt_kernels.cuh"
+#include "wgmma.cuh"
 
 namespace dfm {
 
@@ -64,13 +62,20 @@ inline float bf16_bits_to_float(uint16_t b) {
   return f;
 }
 
+inline int tc_sm_count() {
+  int& cached = per_device<int, 1>();
+  if (!cached) cudaDeviceGetAttribute(&cached, cudaDevAttrMultiProcessorCount, cur_device());
+  return cached;
+}
+
 // ----------------------------------------------------------------------------------
 // modes and compile-time geometry
 // ----------------------------------------------------------------------------------
 enum { TC_S1 = 0, TC_S2 = 1, TC_T = 2 };
 constexpr int TC_BX = 8, TC_BY = 16;  // M tile: 8 (x) * 16 (y) = 128 accumulator rows
-constexpr int TC_LOAD_THREADS = 320;  // 2 groups x 5 warps: 15 warps per CTA = 4,4,4,3 per scheduler, still 128 registers/thread
-constexpr int TC_THREADS = 128 + TC_LOAD_THREADS + 32;  // epilogue | loaders | MMA issuer
+constexpr int TC_MMA_THREADS = 256;   // two warpgroups: MMA issue + epilogue, 64 rows each
+constexpr int TC_LOAD_THREADS = 256;  // 2 groups x 4 warps
+constexpr int TC_THREADS = TC_MMA_THREADS + TC_LOAD_THREADS;  // 16 warps: 128 registers/thread
 constexpr int TC_MAXOPS = 9, TC_MAXBLK = 48;
 constexpr int TC_ZERO_TAP = 255;  // TcBlk::tap of an all-zero padding block
 
@@ -79,7 +84,7 @@ struct TcMode;
 template <>
 struct TcMode<TC_S1> {  // out(x,y,z) <- in(x+dx-1, y+dy-1, z+dz-1)
   static constexpr int PXB = 10, PYB = 18, PITCH = 10, ROWS = 186, CG = 32, NSTAGE = 4;
-  static constexpr int SLOT_BLOCKS = 1, NSLOT = 16;
+  static constexpr int SLOT_BLOCKS = 1;
   __host__ __device__ static int zo_of(int zi, int dz) { return zi + dz; }
   __host__ __device__ static int zi_first(int zo) { return zo - 1; }
   __host__ __device__ static int zi_last(int zo) { return zo + 1; }
@@ -88,7 +93,7 @@ struct TcMode<TC_S1> {  // out(x,y,z) <- in(x+dx-1, y+dy-1, z+dz-1)
 template <>
 struct TcMode<TC_S2> {  // out(x,y,z) <- in(2x+dx-1, 2y+dy-1, 2z+dz-1); x/y parity arrays
   static constexpr int PXB = 17, PYB = 33, PITCH = 9, ROWS = 620, CG = 16, NSTAGE = 3;
-  static constexpr int SLOT_BLOCKS = 1, NSLOT = 16;
+  static constexpr int SLOT_BLOCKS = 1;
   __host__ __device__ static int zo_of(int zi, int dz) { return (zi >> 1) + dz; }
   __host__ __device__ static int zi_first(int zo) { return 2 * zo - 1; }
   __host__ __device__ static int zi_last(int zo) { return 2 * zo + 1; }
@@ -97,7 +102,7 @@ struct TcMode<TC_S2> {  // out(x,y,z) <- in(2x+dx-1, 2y+dy-1, 2z+dz-1); x/y pari
 template <>
 struct TcMode<TC_T> {  // ConvTranspose3d(k3,s2,p1,op1): out(2m+p) <- in(m + s), 8 parity classes
   static constexpr int PXB = 9, PYB = 17, PITCH = 9, ROWS = 154, CG = 32, NSTAGE = 4;
-  static constexpr int SLOT_BLOCKS = 4, NSLOT = 8;  // 4 (px,py) classes per output plane
+  static constexpr int SLOT_BLOCKS = 4;  // 4 (px,py) classes per output plane
   __host__ __device__ static int zo_of(int zi, int dz) { return 2 * zi + dz; }
   __host__ __device__ static int zi_first(int zo) { return zo >> 1; }
   __host__ __device__ static int zi_last(int zo) { return (zo + 1) >> 1; }
@@ -120,7 +125,8 @@ inline bool tc_supported(int Cin, int Cout, int /*transposed*/) {
 inline bool tc_geom_supported(const ConvGeom& g) { return tc_mode_of(g) >= 0; }
 
 // One MMA "op" = one A view (tap shift of the brick) against a weight image whose
-// NCTA-row blocks land in consecutive accumulator column blocks.
+// NCTA-row blocks land in consecutive accumulator column blocks.  The host lays the weight
+// images out from this op list; the kernel issues the same sequence from compile-time constants.
 struct TcOp {
   uint32_t a_off;   // byte offset of the A view inside a stage (hi array)
   uint32_t b_off;   // byte offset of this op's weight image (hi half) in smem
@@ -212,9 +218,9 @@ inline void tc_build_program(int ptype, int Cin, int ncta, uint32_t* w_cursor, T
                                (uint8_t)(real ? kz * 9 + ky * 3 + kx : TC_ZERO_TAP), 0});
         }
       }
-      // The x-only and y-only shifts touch two classes per plane: instead of three N = 2*NCTA
-      // MMAs (each costs the ~47-cycle issue floor) keep the all-zero blocks between the first
-      // and the last real one, so that one N = 10*NCTA MMA spans the three planes.  The
+      // The x-only and y-only shifts touch two classes per plane: instead of three small
+      // N = 2*NCTA MMAs keep the all-zero blocks between the first and the last real one, so that
+      // one N = 10*NCTA MMA spans the three planes (the kernel's MMA sequence stays static).  The
       // diagonal shift touches one class per plane; padding it would not fit in shared memory
       // next to four stages, so it stays three small MMAs.
       if (sh == 3) {
@@ -294,10 +300,11 @@ struct TcWeights {
   }
   bool build(const float* packed, int cin, int cout, int m, std::string* err) {
     static const bool no_ks1 = getenv("DFM_NO_KSLICE") != nullptr;
-    // stride 1, 64 -> 64: four output-channel groups would each re-load the input and issue
-    // N = 48 MMAs (47-cycle issue floor for 48 columns); four input-channel slices issue
-    // N = 192 MMAs (96 cycles for 192 columns) on a quarter of the input each
-    static const bool ks1 = getenv("DFM_KSLICE_S1") != nullptr;  // opt-in until validated on GPU
+    // stride 1, 64 -> 64: four output-channel groups each re-load the input and issue N = 48
+    // MMAs; four input-channel slices would issue N = 192 MMAs on a quarter of the input each
+    // (opt-in: not measured on H100; the 64 -> 64 stride-1 layers of the backbone run on the
+    // K-outer kernel of conv_tc_neck.cuh)
+    static const bool ks1 = getenv("DFM_KSLICE_S1") != nullptr;
     if (m == TC_S1) return build_mode<TC_S1>(packed, cin, cout, err,
                                              cin == 64 && cout == 64 && !no_ks1 && ks1);
     if (m == TC_S2) {
@@ -368,68 +375,6 @@ __device__ __forceinline__ void desc_add(uint64_t& d, uint32_t inc16) {
 __device__ __forceinline__ uint64_t pack64(uint32_t lo, uint32_t hi) {
   return ((uint64_t)hi << 32) | lo;
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem, uint64_t ad, uint64_t bd,
-                                          uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem),
-      "l"(ad), "l"(bd), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// K-major, no-swizzle smem matrix descriptor (LBO: K core-matrix stride, SBO: 8-row group stride)
-__device__ __forceinline__ uint64_t umma_desc(uint32_t addr, uint32_t lbo, uint32_t sbo) {
-  return (uint64_t)((addr >> 4) & 0x3FFF) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) |
-         ((uint64_t)((sbo >> 4) & 0x3FFF) << 32) | ((uint64_t)1 << 46);
-}
-__device__ __forceinline__ uint32_t idesc_bf16(int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((128u >> 4) << 24);
-}
-
-template <int NC>
-__device__ __forceinline__ void tmem_ld(uint32_t taddr, uint32_t* r);
-template <>
-__device__ __forceinline__ void tmem_ld<32>(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,"
-      "%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]),
-        "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-        "=r"(r[31])
-      : "r"(taddr));
-}
-template <>
-__device__ __forceinline__ void tmem_ld<16>(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]),
-        "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-
-// zero NC accumulator columns of this warp's 32 TMEM lanes
-template <int NC>
-__device__ __forceinline__ void tmem_zero(uint32_t taddr) {
-#pragma unroll
-  for (int c = 0; c < NC; c += 16) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1};\n" ::"r"(taddr + c),
-        "r"(0u)
-        : "memory");
-  }
-}
-
 __device__ __forceinline__ void split_store(const float v[8], uint8_t* hi_dst, uint8_t* lo_dst) {
   uint32_t h[4], l[4];
 #pragma unroll
@@ -580,7 +525,8 @@ struct WarpLoader8 {
 // cp.async.bulk.tensor: per (hi|lo, x/y parity class) ONE dense box of 9 x 17 positions x 2
 // chunks, and out-of-range halo positions arrive as zeros.  No loader warp touches the data: the fused GroupNorm /
 // ReLU / residual transform and the bf16 split happened once, in the producer pass.
-// (tests/probe/probe_tma.cu pins the box / stride / zero-fill / byte-count semantics.)
+// (The box / zero-fill / byte-count semantics are pinned by the GPU parity tests of the backbone,
+// whose stride-2 hourglass.conv1 runs on this loader at full size and on ragged fixtures.)
 // ----------------------------------------------------------------------------------
 struct TmaLoader8 {
   static constexpr bool kTma = true;
@@ -610,7 +556,7 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
 // written in the pre-split layout of a stride-2 consumer: x / y PARITY-PLANAR,
 //   [plane z][hi|lo][y parity][x parity][8-channel chunk][H/2][W/2] x 16 bytes,
 // so every parity class of a stride-2 brick is a DENSE 2-D box for TMA (a strided box --
-// elementStrides 2 -- moves one 16-byte element per request and ran at ~2.5 cycles per element).
+// elementStrides 2 -- moves one 16-byte element per request).
 // A warp transforms a run of 64 consecutive x of one row (coalesced 32-byte reads), stages the
 // split values in shared memory and writes 512-byte runs per (hi|lo, x parity, chunk).
 constexpr int PS_XRUN = 64, PS_WARPS = 4, PS_SEG = 33;  // 33: shared-memory segment pitch
@@ -658,7 +604,7 @@ inline bool presplit_launch(const Src& s, int C, int Z, int H, int W, uint4* out
   if ((H | W) & 1) return false;
   const size_t smem = presplit_smem_bytes(C);
   const long long nruns = (long long)Z * H * ((W + PS_XRUN - 1) / PS_XRUN);
-  const int blocks = (int)std::min<long long>((nruns + PS_WARPS - 1) / PS_WARPS, 148LL * 12);
+  const int blocks = (int)std::min<long long>((nruns + PS_WARPS - 1) / PS_WARPS, 12LL * tc_sm_count());
   auto go = [&](auto kern, auto ld) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) !=
         cudaSuccess)
@@ -726,9 +672,8 @@ struct TcParams {
   float zw;
   long long slice_stride;  // K-slice variant: elements between the slices' partial outputs
   int store1;  // epilogue stores only output channel 0, densely ([V] floats): the Cout=1 conv
-  int dbg;  // diagnosis only (DFM_TC_DEBUG): 1 loaders skip work, 2 epilogue skips, 4 no MMA,
-            // 8 loaders skip the proxy fence
-  TcProgram prog[2];
+  int dbg;  // diagnosis only (DFM_TC_DEBUG): 1 loaders skip work, 8 loaders skip the proxy
+            // fence, 16 / 32 loaders skip their global loads / shared-memory stores
 };
 
 struct TcItem {
@@ -770,6 +715,27 @@ __device__ __forceinline__ bool tc_walk_next(const TcParams& p, TcWalk& w, TcIte
   return true;
 }
 
+// Accumulator window of the consumer warpgroups: the output planes that the current input plane
+// zi feeds, kept in registers.  Plane j of the window is output plane base(zi) + j; every block of
+// NCTA columns of a plane is one (px,py) class of the transposed conv (one block otherwise).
+template <int MODE>
+struct TcWin;
+template <>
+struct TcWin<TC_S1> {  // zi feeds zi-1 (kz=2), zi (kz=1), zi+1 (kz=0)
+  static constexpr int NPL = 3;
+  __device__ static int base(int zi) { return zi - 1; }
+};
+template <>
+struct TcWin<TC_S2> {  // zi = 2q feeds q (kz=1); zi = 2q+1 feeds q (kz=2), q+1 (kz=0)
+  static constexpr int NPL = 2;
+  __device__ static int base(int zi) { return zi >> 1; }
+};
+template <>
+struct TcWin<TC_T> {  // zi feeds 2zi-1 (kz=0), 2zi (kz=1), 2zi+1 (kz=2)
+  static constexpr int NPL = 3;
+  __device__ static int base(int zi) { return 2 * zi - 1; }
+};
+
 // ----------------------------------------------------------------------------------
 // the kernel
 // ----------------------------------------------------------------------------------
@@ -777,6 +743,7 @@ template <int MODE, int CIN, int NCTA, class Loader>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ TcParams p,
                                                                  const __grid_constant__ Loader ld) {
   using M = TcMode<MODE>;
+  using Win = TcWin<MODE>;
   constexpr bool TMA = Loader::kTma;
   static_assert(!TMA || MODE == TC_S2, "the TMA loader serves the stride-2 brick only");
   constexpr int CG = M::CG < CIN ? M::CG : CIN;  // channels per stage
@@ -792,55 +759,45 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   constexpr uint32_t A_HL = TMA ? 4 * TMA_S2_CLSR * 16 : NCH * M::ROWS * 16;  // hi -> lo offset
   constexpr uint32_t STAGE_BYTES = 2 * A_HL;
   constexpr uint32_t B_SBO = 128;
-  constexpr int SLOT_COLS = M::SLOT_BLOCKS * NCTA;
   // K-slice variant (stride 1 / 2, instantiated with CIN = 16 = the channels this CTA group loads,
   // NCTA = all output channels): every slice stores its partial sums; kslice_reduce_kernel adds
   // them in slice order (deterministic) and takes the GroupNorm statistics on the way
   constexpr bool KSLICE = CIN == 16;
-  constexpr int TC_NSLOT = M::NSLOT * SLOT_COLS > 512 ? 512 / SLOT_COLS : M::NSLOT;
-  constexpr uint32_t TMEM_COLS = TC_NSLOT * SLOT_COLS;  // 256 / 512
   constexpr int NPOS = M::PXB * M::PYB;
   // two loader groups (even / odd loader warps) fill alternate stages: while one group
   // waits for its global loads the other transforms and stores -> two stages in flight
   constexpr int LGROUPS = 2;
   constexpr int LG_THREADS = TC_LOAD_THREADS / LGROUPS;
   constexpr int NITEM = (NPOS * NCH + LG_THREADS - 1) / LG_THREADS;
+  constexpr int PCOLS = M::SLOT_BLOCKS * NCTA;        // accumulator columns per output plane
+  constexpr int NACC = Win::NPL * PCOLS / 2;          // accumulator registers per thread
 
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* w_s = smem;
   uint8_t* a_s = smem + p.w_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(a_s + M::NSTAGE * STAGE_BYTES);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * M::NSTAGE + 2 * M::NSLOT + 1);
 
-  const long long t_kernel0 = clock64();
   const int tid = threadIdx.x, lane = tid & 31;
   // shfl broadcast: tells the compiler the warp index is warp-uniform, so the role
-  // branches below are convergent and the MMA warp can use the uniform datapath
+  // branches below are convergent
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
   const uint32_t bar0 = smem_u32(bars);
   auto full_a = [&](int s) { return bar0 + 8u * s; };
   auto empty_a = [&](int s) { return bar0 + 8u * (M::NSTAGE + s); };
-  auto full_acc = [&](int s) { return bar0 + 8u * (2 * M::NSTAGE + s); };
-  auto empty_acc = [&](int s) { return bar0 + 8u * (2 * M::NSTAGE + TC_NSLOT + s); };
-  constexpr int MMA_WARP = TC_THREADS / 32 - 1;
+  const uint32_t w_bar = bar0 + 8u * (2 * M::NSTAGE);
+  constexpr int LOAD_WARP0 = TC_MMA_THREADS / 32;
 
-  const uint32_t w_bar = bar0 + 8u * (2 * M::NSTAGE + 2 * TC_NSLOT);
   if (tid == 0) {
     for (int s = 0; s < M::NSTAGE; ++s) {
       // one arrival per loader warp of the group; TMA: the issuing thread's expect_tx arrival
       mbar_init(full_a(s), TMA ? 1 : LG_THREADS / 32);
-      mbar_init(empty_a(s), 1);
-    }
-    for (int s = 0; s < TC_NSLOT; ++s) {
-      mbar_init(full_acc(s), 1);
-      mbar_init(empty_acc(s), 4);
+      mbar_init(empty_a(s), TC_MMA_THREADS / 32);  // one arrival per consumer warp
     }
     mbar_init(w_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     // Resident weights of this CTA's output-channel group: bulk async copies (TMA engine)
-    // that land while TMEM is being allocated / zeroed and the loaders fill the first
-    // stages; only the MMA issuer waits for them.  (A thread-copy loop here cost every
-    // launch ~10 us of serialised load latency.)
+    // that land while the loaders fill the first stages; only the consumers wait for them.
+    // (A thread-copy loop here cost every launch ~10 us of serialised load latency.)
     const int split = blockIdx.x % p.nsplit;
     const uint8_t* src = p.wimg + (size_t)split * p.w_bytes;
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(w_bar),
@@ -855,30 +812,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
           : "memory");
     }
   }
-  if (warp == MMA_WARP) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(tmem_slot)),
-                 "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  // Accumulators are always accumulated into (no "overwrite" MMA, which would force the
-  // dz-merged MMA to be split at the plane that starts a new accumulator): the epilogue
-  // re-zeroes a slot right after draining it, and all slots start at zero.
-  if (warp < 4) {
-    for (uint32_t c = 0; c < TMEM_COLS; c += 64)
-      tmem_zero<64>(tmem_base + ((uint32_t)(warp * 32) << 16) + c);
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 
   if constexpr (TMA) {
-    if (warp == 4 && lane == 0) {
+    if (warp == LOAD_WARP0 && lane == 0) {
       // ============================ TMA producer (one thread) ============================
       constexpr uint32_t STAGE_TX = 8u * 2u * TMA_S2_CLS * 16u;  // 8 boxes of 2 x 153 x 16 bytes
       uint32_t stage_ctr = 0;
@@ -916,15 +853,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
       }
     }
   }
-  if (TMA && warp >= 4 && warp < MMA_WARP) {
-    // (the loader warps have nothing to do: warp 4's lane 0 issued the TMA boxes above)
-  } else if (warp >= 4 && warp < MMA_WARP) {
+  if (TMA && warp >= LOAD_WARP0) {
+    // (the loader warps have nothing to do: the first loader warp's lane 0 issued the TMA boxes)
+  } else if (warp >= LOAD_WARP0) {
     // ============================ loaders ============================
-    const int lgrp = (warp - 4) & (LGROUPS - 1);
-    const int lt = ((warp - 4) / LGROUPS) * 32 + lane;  // thread index inside the group
+    const int lw = warp - LOAD_WARP0;
+    const int lgrp = lw & (LGROUPS - 1);
+    const int lt = (lw / LGROUPS) * 32 + lane;  // thread index inside the group
     const int chunk = lt % NCH;
     uint32_t stage_ctr = 0;
-    const bool timed = p.role_cycles != nullptr && tid == 128;
+    const bool timed = p.role_cycles != nullptr && lw == 0 && lane == 0;
     unsigned long long t_wait_e = 0;
     const long long t_begin = clock64();
     TcWalk walk = tc_walk_begin(p);
@@ -1000,446 +938,270 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
       rc[3] = (unsigned long long)(clock64() - t_begin);
       rc[4] = t_wait_e;
     }
-  } else if (warp == MMA_WARP) {
-    // ============================ MMA issuer ============================
-    // One thread issues every MMA, so its scalar overhead per MMA must stay far below
-    // the ~47-56 cycles an MMA occupies the tensor pipe: descriptors are split into a
-    // constant high word and a low word that only needs integer adds, per-plane slot
-    // state is hoisted out of the op loop.  The whole warp executes the (warp-uniform)
-    // control flow so the compiler keeps descriptors in uniform registers; only the
-    // tcgen05 instructions themselves are predicated on lane 0.
-    {
-      const bool timed = p.role_cycles != nullptr;
-      const bool issuer = lane == 0;
-      unsigned long long t_wait_a = 0, t_wait_acc = 0;
-      const long long t_begin = clock64();
-      mbar_wait(w_bar, 0u, p.err);  // weight image has landed
-      const uint32_t w_base = smem_u32(w_s), a_base = smem_u32(a_s);
-      const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);  // provably uniform
-      constexpr uint32_t A_LBO16 = A_LBO >> 4, A_HL16 = A_HL >> 4;
-      const uint32_t a_desc_hi = (A_SBO >> 4) | (1u << 14);  // SBO | version
-      const uint32_t b_desc_hi = (B_SBO >> 4) | (1u << 14);
-      const uint32_t w_hi16 = p.w_hi_bytes >> 4;
-      uint32_t stage_ctr = 0, plane_ctr = 0;  // plane_ctr: running index of output planes
-      TcWalk walk = tc_walk_begin(p);
-      TcItem it;
-      while (tc_walk_next(p, walk, it)) {
-        const int zi0 = max(M::zi_first(it.z_lo), 0);
-        const int zi1 = min(M::zi_last(it.z_hi - 1), p.Di - 1);
-        const uint32_t plane_base = plane_ctr;  // slot of output plane zo: (base + zo - z_lo) % NSLOT
-        for (int zi = zi0; zi <= zi1; ++zi) {
-          const TcProgram& pr = p.prog[M::ptype(zi)];
-          // per-plane state of the (up to) three output planes this input plane feeds
-          uint32_t vmask = 0, fmask = 0, colbase[3];
-#pragma unroll
-          for (int dz = -1; dz <= 1; ++dz) {
-            const int zo = M::zo_of(zi, dz);
-            const uint32_t j = plane_base + (uint32_t)(zo - it.z_lo);
-            colbase[dz + 1] = (j % TC_NSLOT) * SLOT_COLS;
-            if (zo >= it.z_lo && zo < it.z_hi) {
-              vmask |= 1u << (dz + 1);
-              if (zi == max(M::zi_first(zo), zi0)) {
-                fmask |= 1u << (dz + 1);
-                // a slot that starts with this input plane must have been drained
-                mbar_wait_timed(empty_acc(j % TC_NSLOT), ((j / TC_NSLOT) & 1) ^ 1, p.err,
-                                t_wait_acc, timed);
-              }
-            }
-          }
-          const bool regular = (vmask & pr.need) == pr.need;
-          // bit k: the slot ring wraps between the planes dz = k-1 and dz = k
-          const uint32_t wrapmask = (colbase[1] != colbase[0] + SLOT_COLS ? 1u : 0u) |
-                                    (colbase[2] != colbase[1] + SLOT_COLS ? 2u : 0u);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-          for (int cg = 0; cg < NCG; ++cg, ++stage_ctr) {
-            const int s = stage_ctr % M::NSTAGE;
-            mbar_wait_timed(full_a(s), (stage_ctr / M::NSTAGE) & 1, p.err, t_wait_a, timed);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t a_lo_stage =
-                (((a_base + s * STAGE_BYTES) >> 4) & 0x3FFF) | (A_LBO16 << 16);
-            bool done = false;
-            if constexpr (MODE == TC_S1) {
-              // Stride-1 issue sequence: the live output planes form one contiguous range
-              // of the three dz slots, cut only where the accumulator ring wraps.  Per piece
-              // a rolled loop over the 9 taps with persistent descriptors whose low words
-              // are bumped by uniform adds (the issuing warp is serial in scalar work +
-              // ~47 cycles per tcgen05.mma issue, so scalar work per MMA must be ~1 op).
-              constexpr uint32_t B_LBO16 = 3 * NCTA;               // weight image rows
-              constexpr uint32_t TAP16 = (CIN / 8) * B_LBO16;      // one tap, 16-byte units
-              constexpr int NKS = CG / 16;
-              const uint32_t b_lo0 = ((w_base >> 4) & 0x3FFF) + (uint32_t)(cg * NCH) * B_LBO16 +
-                                     (B_LBO16 << 16);
-              // first / one-past-last live plane index (0..3) of this input plane
-              const int pa = (vmask & 1u) ? 0 : (vmask & 2u) ? 1 : 2;
-              const int pb = (vmask & 4u) ? 3 : (vmask & 2u) ? 2 : 1;
-              int first = pa;
-              while (first < pb) {
-                int last = first + 1;  // exclusive
-                while (last < pb && !((wrapmask >> (last - 1)) & 1u)) ++last;
-                const uint32_t cb0 = first == 0 ? colbase[0] : first == 1 ? colbase[1] : colbase[2];
-                const uint32_t d0 = tmem_u + cb0;
-                const uint32_t idesc = idesc_bf16((last - first) * NCTA);
-                uint64_t da[NKS][2], db[NKS][2];
-#pragma unroll
-                for (int ks = 0; ks < NKS; ++ks) {
-                  da[ks][0] = pack64(a_lo_stage + 2 * ks * A_LBO16, a_desc_hi);
-                  da[ks][1] = pack64(a_lo_stage + 2 * ks * A_LBO16 + A_HL16, a_desc_hi);
-                  const uint32_t bl = b_lo0 + 2 * ks * B_LBO16 + (uint32_t)first * NCTA;
-                  db[ks][0] = pack64(bl, b_desc_hi);
-                  db[ks][1] = pack64(bl + w_hi16, b_desc_hi);
-                }
-#pragma unroll 1
-                for (int tap = 0; tap < 9; ++tap) {
-                  if (elect_one()) {
-#pragma unroll
-                    for (int ks = 0; ks < NKS; ++ks) {
-                      umma_bf16(d0, da[ks][0], db[ks][0], idesc, 1u);
-                      umma_bf16(d0, da[ks][1], db[ks][0], idesc, 1u);
-                      umma_bf16(d0, da[ks][0], db[ks][1], idesc, 1u);
-                    }
-                  }
-                  const uint32_t ainc = (tap == 2 || tap == 5) ? (uint32_t)(M::PITCH - 2) : 1u;
-#pragma unroll
-                  for (int ks = 0; ks < NKS; ++ks) {
-                    desc_add(da[ks][0], ainc);
-                    desc_add(da[ks][1], ainc);
-                    desc_add(db[ks][0], TAP16);
-                    desc_add(db[ks][1], TAP16);
-                  }
-                }
-                first = last;
-              }
-              done = true;
-            }
-            if constexpr (MODE == TC_S2) {
-              // Stride-2 issue sequence (one K step per 16-channel stage).  Even input planes
-              // feed one output plane (kz = 1); odd planes feed two (kz = 2 -> zo, kz = 0 ->
-              // zo + 1) with one N = 2*NCTA MMA when their slots are contiguous.
-              constexpr uint32_t KCH16 = CIN / 8;
-              const uint32_t odd = (uint32_t)zi & 1u;
-              const uint32_t nimg = odd ? 2u : 1u;                 // blocks per weight image
-              const uint32_t b_lbo16 = nimg * NCTA;
-              const uint32_t tap16 = KCH16 * b_lbo16;
-              const uint32_t b_lo0 = ((w_base >> 4) & 0x3FFF) + (odd ? 9u * KCH16 * NCTA : 0u) +
-                                     (uint32_t)(cg * NCH) * b_lbo16 + (b_lbo16 << 16);
-              auto run = [&](uint32_t col, uint32_t brow16, uint32_t nblk) {
-                const uint32_t d0 = tmem_u + col;
-                const uint32_t idesc = idesc_bf16((int)(nblk * NCTA));
-                uint64_t dbh = pack64(b_lo0 + brow16, b_desc_hi);
-                uint64_t dbl = pack64(b_lo0 + brow16 + w_hi16, b_desc_hi);
-#pragma unroll
-                for (int tap = 0; tap < 9; ++tap) {
-                  const int dy = tap / 3, dx = tap % 3;
-                  const uint32_t a16 = (uint32_t)(((dx & 1) * 2 + (dy & 1)) * S2_CLS16 +
-                                                  (dy >> 1) * M::PITCH + (dx >> 1));
-                  const uint64_t dah = pack64(a_lo_stage + a16, a_desc_hi);
-                  const uint64_t dal = pack64(a_lo_stage + a16 + A_HL16, a_desc_hi);
-                  if (elect_one()) {
-                    umma_bf16(d0, dah, dbh, idesc, 1u);
-                    umma_bf16(d0, dal, dbh, idesc, 1u);
-                    umma_bf16(d0, dah, dbl, idesc, 1u);
-                  }
-                  desc_add(dbh, tap16);
-                  desc_add(dbl, tap16);
-                }
-              };
-              if (!odd) {
-                if (vmask & 2u) run(colbase[1], 0u, 1u);
-              } else if ((vmask & 6u) == 6u && !(wrapmask & 2u)) {
-                run(colbase[1], 0u, 2u);
-              } else {
-                if (vmask & 2u) run(colbase[1], 0u, 1u);
-                if (vmask & 4u) run(colbase[2], NCTA, 1u);
-              }
-              done = true;
-            }
-            if constexpr (MODE == TC_T) {
-              // Transposed-conv issue sequence for a plane whose three output planes are all
-              // live: the op list of tc_build_program<TC_T> is static -- shift (0,0): one run
-              // of 12 blocks from lin 0; x-only / y-only shifts: one (zero-padded) run of 10
-              // blocks from lin 1 / lin 2; diagonal shift: single blocks at lin 2, 6, 10 --
-              // so everything but the slot-ring wrap position is a compile-time constant.
-              // (The table-driven path below costs ~35 scalar instructions per MMA and shares
-              // its issue slots with three other warps; it only serves the boundary planes.)
-              if (regular) {
-                constexpr uint32_t SB = M::SLOT_BLOCKS;
-                constexpr uint32_t KCH16 = CIN / 8;
-                constexpr uint32_t NB[4] = {12u, 10u, 10u, 3u};      // blocks per weight image
-                constexpr uint32_t LIN0[4] = {0u, 1u, 2u, 2u};
-                // lin index at which the accumulator slot ring wraps (16: not inside the window)
-                const uint32_t cut = (wrapmask & 1u) ? SB : (wrapmask & 2u) ? 2u * SB : 16u;
-                auto col_of = [&](uint32_t lin) {
-                  const uint32_t pl = lin / SB;
-                  const uint32_t cb = pl == 0u ? colbase[0] : pl == 1u ? colbase[1] : colbase[2];
-                  return cb + (lin % SB) * NCTA;
-                };
-                auto mma3 = [&](uint32_t lin, uint64_t dah, uint64_t dal, uint32_t blo,
-                                uint32_t nblk) {
-                  const uint32_t idesc = idesc_bf16((int)(nblk * NCTA));
-                  const uint32_t d0 = tmem_u + col_of(lin);
-                  const uint64_t dbh = pack64(blo, b_desc_hi);
-                  const uint64_t dbl = pack64(blo + w_hi16, b_desc_hi);
-                  if (elect_one()) {
-                    umma_bf16(d0, dah, dbh, idesc, 1u);
-                    umma_bf16(d0, dal, dbh, idesc, 1u);
-                    umma_bf16(d0, dah, dbl, idesc, 1u);
-                  }
-                };
-                uint32_t b_img16 = (w_base >> 4) & 0x3FFF;  // start of this shift's weight image
-#pragma unroll
-                for (int sh = 0; sh < 4; ++sh) {
-                  const uint32_t b_lbo16 = NB[sh] * NCTA;
-                  const uint32_t a16 = (uint32_t)((sh >> 1) * M::PITCH + (sh & 1));
-#pragma unroll
-                  for (int ks = 0; ks < CG / 16; ++ks) {
-                    const uint32_t alo = a_lo_stage + a16 + 2 * ks * A_LBO16;
-                    const uint64_t dah = pack64(alo, a_desc_hi);
-                    const uint64_t dal = pack64(alo + A_HL16, a_desc_hi);
-                    const uint32_t blo = b_img16 + (uint32_t)(cg * NCH + 2 * ks) * b_lbo16 +
-                                         (b_lbo16 << 16);
-                    if (sh == 3) {
-#pragma unroll
-                      for (uint32_t k = 0; k < 3; ++k)
-                        mma3(LIN0[3] + k * SB, dah, dal, blo + k * NCTA, 1u);
-                    } else {
-                      const uint32_t lin0 = LIN0[sh], end = LIN0[sh] + NB[sh];
-                      const uint32_t c = min(max(cut, lin0), end);
-                      if (c > lin0) mma3(lin0, dah, dal, blo, c - lin0);
-                      if (end > c) mma3(c, dah, dal, blo + (c - lin0) * NCTA, end - c);
-                    }
-                  }
-                  b_img16 += KCH16 * b_lbo16;
-                }
-                done = true;
-              }
-            }
-            if (!done) {
-#pragma unroll 1
-            for (int o = 0; o < pr.nops; ++o) {
-              const TcOp op = pr.ops[o];
-              const uint32_t a_lo_op = a_lo_stage + (op.a_off >> 4);
-              const uint32_t b_lbo16 = op.b_lbo >> 4;
-              const uint32_t b_lo_op = (((w_base + op.b_off) >> 4) & 0x3FFF) +
-                                       (uint32_t)(cg * NCH) * b_lbo16 + (b_lbo16 << 16);
-              const uint32_t fm = 0u;  // accumulators are pre-zeroed: always accumulate
-              auto issue = [&](uint32_t col0, uint32_t blk_rel, uint32_t nblk, uint32_t fresh) {
-                const uint32_t idesc = idesc_bf16((int)(nblk * NCTA));
-                const uint32_t d_tmem = tmem_u + col0;
-                const uint32_t b_lo_run = b_lo_op + blk_rel * NCTA;
-#pragma unroll
-                for (int ks = 0; ks < M::CG / 16; ++ks) {
-                  const uint64_t dah = pack64(a_lo_op + 2 * ks * A_LBO16, a_desc_hi);
-                  const uint64_t dal = pack64(a_lo_op + 2 * ks * A_LBO16 + A_HL16, a_desc_hi);
-                  const uint64_t dbh = pack64(b_lo_run + 2 * ks * b_lbo16, b_desc_hi);
-                  const uint64_t dbl = pack64(b_lo_run + 2 * ks * b_lbo16 + w_hi16, b_desc_hi);
-                  if (elect_one()) {
-                    umma_bf16(d_tmem, dah, dbh, idesc, (fresh && ks == 0) ? 0u : 1u);
-                    umma_bf16(d_tmem, dal, dbh, idesc, 1u);
-                    umma_bf16(d_tmem, dah, dbl, idesc, 1u);
-                  }
-                }
-              };
-              if (regular && fm == 0) {
-                // fast path: the host-precomputed runs, split only where the slot ring wraps
-                constexpr uint32_t SB = M::SLOT_BLOCKS;
-                for (uint32_t r = 0; r < op.nruns; ++r) {
-                  const uint32_t rc = op.runs[r];
-                  const uint32_t nblk = rc & 15u, bs = (rc >> 4) & 63u, lin0 = (rc >> 10) & 15u;
-                  uint32_t a = lin0;
-                  const uint32_t end = lin0 + nblk;
-                  while (a < end) {
-                    const uint32_t pl = a / SB;
-                    uint32_t b = end;
-                    if (pl == 0u) {
-                      if (wrapmask & 1u) b = min(b, SB);
-                      else if (wrapmask & 2u) b = min(b, 2u * SB);
-                    } else if (pl == 1u) {
-                      if (wrapmask & 2u) b = min(b, 2u * SB);
-                    }
-                    const uint32_t cbase = pl == 0u ? colbase[0] : pl == 1u ? colbase[1] : colbase[2];
-                    issue(cbase + (a % SB) * NCTA, bs + (a - lin0), b - a, 0u);
-                    a = b;
-                  }
-                }
-              } else {
-                int b = op.blk0;
-                while (b < op.blk1) {
-                  const TcBlk bk = pr.blks[b];
-                  const uint32_t bit = 1u << (bk.dz + 1);
-                  if (!(vmask & bit)) {
-                    ++b;
-                    continue;
-                  }
-                  const uint32_t fresh = fm & bit;
-                  const uint32_t col0 = colbase[bk.dz + 1] + bk.colblk * NCTA;
-                  int e = b + 1;
-                  while (e < op.blk1 && (e - b) * NCTA < 256) {
-                    const TcBlk bn = pr.blks[e];
-                    const uint32_t bitn = 1u << (bn.dz + 1);
-                    if (!(vmask & bitn) || ((fm & bitn) != 0) != (fresh != 0) ||
-                        colbase[bn.dz + 1] + bn.colblk * NCTA != col0 + (uint32_t)(e - b) * NCTA)
-                      break;
-                    ++e;
-                  }
-                  issue(col0, (uint32_t)(b - op.blk0), (uint32_t)(e - b), fresh);
-                  b = e;
-                }
-              }
-            }
-            }
-            if (elect_one()) umma_commit(empty_a(s));  // stage refillable once these MMAs retire
-            __syncwarp();
-          }
-          // output planes whose last contribution was this input plane
-#pragma unroll
-          for (int dz = -1; dz <= 1; ++dz) {
-            const int zo = M::zo_of(zi, dz);
-            if ((vmask >> (dz + 1)) & 1u) {
-              if (zi == min(M::zi_last(zo), zi1)) {
-                const uint32_t j = plane_base + (uint32_t)(zo - it.z_lo);
-                if (elect_one()) umma_commit(full_acc(j % TC_NSLOT));
-              }
-            }
-          }
-        }
-        plane_ctr += it.z_hi - it.z_lo;
-      }
-      if (timed && issuer) {
-        unsigned long long* rc = p.role_cycles + (size_t)blockIdx.x * 8;
-        rc[0] = (unsigned long long)(clock64() - t_begin);
-        rc[7] = (unsigned long long)(t_begin - t_kernel0);
-        rc[1] = t_wait_a;
-        rc[2] = t_wait_acc;
-      }
-    }
-    __syncwarp();
   } else {
-    // ============================ epilogue (warps 0-3) ============================
-    uint32_t plane_ctr = 0;
-    const int m = warp * 32 + lane;  // accumulator row == TMEM lane
+    // ======================= consumers: two MMA + epilogue warpgroups =======================
+    // Warpgroup wg owns accumulator rows [64*wg, 64*wg + 64) of the 128-row tile, i.e. tile
+    // rows y = 8*wg .. 8*wg + 7 (8 brick rows further into every A view).  Its accumulators are
+    // the window of output planes the current input plane feeds (TcWin): all window planes are
+    // computed for every input plane, planes outside the item's range are simply never stored,
+    // so the MMA sequence of a plane type is static.  A plane leaves the window (is stored,
+    // then its registers are reused) once the last input plane that feeds it is done.
+    const int wg = warp >> 2, wq = warp & 3;
     const bool timed = p.role_cycles != nullptr && tid == 0;
-    unsigned long long t_wait_f = 0;
+    unsigned long long t_wait_a = 0;
     const long long t_begin = clock64();
-    constexpr int EW = NCTA > 32 ? 32 : NCTA;   // accumulator columns drained per step
-    constexpr int NSUB = NCTA / EW;
-    constexpr int NST = KSLICE ? 1 : NCTA;      // the K-slice variant keeps no statistics
+    mbar_wait(w_bar, 0u, p.err);  // weight image has landed
+    const uint32_t w_base = smem_u32(w_s), a_base = smem_u32(a_s);
+    constexpr uint32_t A_LBO16 = A_LBO >> 4, A_HL16 = A_HL >> 4;
+    const uint32_t a_desc_hi = A_SBO >> 4;
+    const uint32_t b_desc_hi = B_SBO >> 4;
+    const uint32_t w_hi16 = p.w_hi_bytes >> 4;
+    const uint32_t a_wg16 = (uint32_t)wg * 8u * (A_SBO >> 4);  // this warpgroup's first A row
+
+    float acc[NACC];
+#pragma unroll
+    for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+    constexpr int NST = KSLICE ? 1 : NCTA / 4;  // channels of this thread (the K-slice variant keeps no statistics)
     float ssum[NST], ssq[NST];
 #pragma unroll
     for (int i = 0; i < NST; ++i) ssum[i] = ssq[i] = 0.f;
-    int cur_split = -1;
-    auto flush_stats = [&]() {
-      if (KSLICE || !p.stats || cur_split < 0) return;
+
+    // rows of this thread: tile (x, y) = (lane / 4, 8*wg + 2*wq + r), r = 0, 1
+    const int xr = lane >> 2, cq = lane & 3;
+    auto flush_stats = [&](int split) {
+      if (KSLICE || !p.stats) return;
 #pragma unroll
-      for (int i = 0; i < NST; ++i) {
-        double a = ssum[i], b = ssq[i];
+      for (int k = 0; k < NST; ++k) {
+        double a = ssum[k], b = ssq[k];
 #pragma unroll
-        for (int o = 16; o; o >>= 1) {
+        for (int o = 4; o < 32; o <<= 1) {
           a += __shfl_xor_sync(0xffffffffu, a, o);
           b += __shfl_xor_sync(0xffffffffu, b, o);
         }
-        if (lane == 0) {
-          atomicAdd(p.stats + 2 * (cur_split * NCTA + i), a);
-          atomicAdd(p.stats + 2 * (cur_split * NCTA + i) + 1, b);
+        if (lane < 4) {
+          const int ch = split * NCTA + 8 * (k >> 1) + 2 * lane + (k & 1);
+          atomicAdd(p.stats + 2 * ch, a);
+          atomicAdd(p.stats + 2 * ch + 1, b);
         }
-        ssum[i] = ssq[i] = 0.f;
+        ssum[k] = ssq[k] = 0.f;
       }
     };
+    // store window plane J (output plane zo) if the item owns it
+    auto emit = [&](const TcItem& it, auto jc, int zo) {
+      constexpr int J = decltype(jc)::value;
+      if (zo < it.z_lo || zo >= it.z_hi) return;
+#pragma unroll
+      for (int cb = 0; cb < M::SLOT_BLOCKS; ++cb) {
+        const float* r = acc + (J * PCOLS + cb * NCTA) / 2;
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const int mx = it.x0 + xr, my = it.y0 + 8 * wg + 2 * wq + rr;
+          if (mx >= p.Mx || my >= p.My) continue;
+          int xo = mx, yo = my;
+          if (MODE == TC_T) {  // class order (0,0), (1,0), (1,1), (0,1)
+            xo = 2 * mx + ((cb == 1 || cb == 2) ? 1 : 0);
+            yo = 2 * my + (cb >= 2 ? 1 : 0);
+          }
+          const long long vox = ((long long)zo * p.Ho + yo) * p.Wo + xo;
+          if (p.store1) {
+            if (cq == 0) p.out[vox] = r[2 * rr];
+            continue;
+          }
+          const int ch_base = (KSLICE ? 0 : it.split * NCTA) + 2 * cq;
+          const float wz = (zo >= p.zw_lo && zo < p.zw_hi) ? p.zw : 1.f;
+#pragma unroll
+          for (int j = 0; j < NCTA / 8; ++j) {
+            float v0 = r[4 * j + 2 * rr], v1 = r[4 * j + 2 * rr + 1];
+            const int ch = ch_base + 8 * j;
+            if (p.addend) {
+              const int cls = zo == 0 ? 0 : (zo == p.Do - 1 ? 2 : 1);
+              const float2 a2 = __ldg(reinterpret_cast<const float2*>(
+                  p.addend + (((long long)cls * p.Ho + yo) * p.Wo + xo) * p.Cout + ch));
+              v0 += a2.x;
+              v1 += a2.y;
+            }
+            // (K-slice variant: p.out is the scratch, every slice stores its partial sums)
+            *reinterpret_cast<float2*>(p.out + (KSLICE ? it.split * p.slice_stride : 0) +
+                                       vox * p.Cout + ch) = make_float2(v0, v1);
+            if constexpr (!KSLICE) {
+              if (p.stats) {
+                ssum[2 * j] = fmaf(wz, v0, ssum[2 * j]);
+                ssq[2 * j] = fmaf(wz * v0, v0, ssq[2 * j]);
+                ssum[2 * j + 1] = fmaf(wz, v1, ssum[2 * j + 1]);
+                ssq[2 * j + 1] = fmaf(wz * v1, v1, ssq[2 * j + 1]);
+              }
+            }
+          }
+        }
+      }
+    };
+    // drop the first SH planes of the window, open SH empty ones at its end
+    auto shift = [&](auto shc) {
+      constexpr int SH = decltype(shc)::value * PCOLS / 2;
+#pragma unroll
+      for (int i = 0; i < NACC; ++i) acc[i] = i + SH < NACC ? acc[i + SH] : 0.f;
+    };
+
+    uint32_t stage_ctr = 0;
     TcWalk walk = tc_walk_begin(p);
     TcItem it;
     while (tc_walk_next(p, walk, it)) {
-      cur_split = it.split;
-      const int mx = it.x0 + (m & 7), my = it.y0 + (m >> 3);
-      const bool ok = mx < p.Mx && my < p.My;
-      for (int zo = it.z_lo; zo < it.z_hi; ++zo, ++plane_ctr) {
-        const int slot = plane_ctr % TC_NSLOT;
-        mbar_wait_timed(full_acc(slot), (plane_ctr / TC_NSLOT) & 1, p.err, t_wait_f, timed);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (p.dbg & 2) {
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+      const int zi0 = max(M::zi_first(it.z_lo), 0);
+      const int zi1 = min(M::zi_last(it.z_hi - 1), p.Di - 1);
+      for (int zi = zi0; zi <= zi1; ++zi) {
+#pragma unroll 1
+        for (int cg = 0; cg < NCG; ++cg, ++stage_ctr) {
+          const int s = stage_ctr % M::NSTAGE;
+          mbar_wait_timed(full_a(s), (stage_ctr / M::NSTAGE) & 1, p.err, t_wait_a, timed);
           __syncwarp();
-          if (lane == 0) mbar_arrive(empty_acc(slot));
-          continue;
-        }
+          const uint32_t a_lo_stage =
+              ((((a_base + s * STAGE_BYTES) >> 4) & 0x3FFF) + a_wg16) | (A_LBO16 << 16);
+          wgmma_fence();
+          if constexpr (MODE == TC_S1) {
+            // one N = 3*NCTA MMA per (tap, K step, operand term): weight rows [kz=2|kz=1|kz=0]
+            // land in window planes zi-1, zi, zi+1; a 3x3 in-plane tap is a shift of the A view
+            constexpr uint32_t B_LBO16 = 3 * NCTA;               // weight image rows
+            constexpr uint32_t TAP16 = (CIN / 8) * B_LBO16;      // one tap, 16-byte units
+            constexpr int NKS = CG / 16;
+            const uint32_t b_lo0 = ((w_base >> 4) & 0x3FFF) + (uint32_t)(cg * NCH) * B_LBO16 +
+                                   (B_LBO16 << 16);
+            uint64_t da[NKS][2], db[NKS][2];
 #pragma unroll
-        for (int cb = 0; cb < M::SLOT_BLOCKS; ++cb) {
-#pragma unroll
-        for (int sub = 0; sub < NSUB; ++sub) {
-          uint32_t r[EW];
-          const uint32_t tcol = tmem_base + ((uint32_t)(warp * 32) << 16) + slot * SLOT_COLS +
-                                cb * NCTA + sub * EW;
-          tmem_ld<EW>(tcol, r);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          tmem_zero<EW>(tcol);
-          if (cb == M::SLOT_BLOCKS - 1 && sub == NSUB - 1) {
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(empty_acc(slot));
-          }
-          if (ok) {
-            int xo = mx, yo = my;
-            if (MODE == TC_T) {  // class order (0,0), (1,0), (1,1), (0,1)
-              xo = 2 * mx + ((cb == 1 || cb == 2) ? 1 : 0);
-              yo = 2 * my + (cb >= 2 ? 1 : 0);
+            for (int ks = 0; ks < NKS; ++ks) {
+              da[ks][0] = pack64(a_lo_stage + 2 * ks * A_LBO16, a_desc_hi);
+              da[ks][1] = pack64(a_lo_stage + 2 * ks * A_LBO16 + A_HL16, a_desc_hi);
+              const uint32_t bl = b_lo0 + 2 * ks * B_LBO16;
+              db[ks][0] = pack64(bl, b_desc_hi);
+              db[ks][1] = pack64(bl + w_hi16, b_desc_hi);
             }
-            const int ch0 = (KSLICE ? 0 : it.split * NCTA) + sub * EW;  // first output channel
-            if (p.addend) {
-              const int cls = zo == 0 ? 0 : (zo == p.Do - 1 ? 2 : 1);
-              const float4* ad = reinterpret_cast<const float4*>(
-                  p.addend + (((long long)cls * p.Ho + yo) * p.Wo + xo) * p.Cout + ch0);
+#pragma unroll 1
+            for (int tap = 0; tap < 9; ++tap) {
 #pragma unroll
-              for (int q = 0; q < EW / 4; ++q) {
-                const float4 a4 = __ldg(ad + q);
-                r[4 * q] = __float_as_uint(__uint_as_float(r[4 * q]) + a4.x);
-                r[4 * q + 1] = __float_as_uint(__uint_as_float(r[4 * q + 1]) + a4.y);
-                r[4 * q + 2] = __float_as_uint(__uint_as_float(r[4 * q + 2]) + a4.z);
-                r[4 * q + 3] = __float_as_uint(__uint_as_float(r[4 * q + 3]) + a4.w);
+              for (int ks = 0; ks < NKS; ++ks) {
+                wgmma_bf16<3 * NCTA>(acc, da[ks][0], db[ks][0]);
+                wgmma_bf16<3 * NCTA>(acc, da[ks][1], db[ks][0]);
+                wgmma_bf16<3 * NCTA>(acc, da[ks][0], db[ks][1]);
+              }
+              const uint32_t ainc = (tap == 2 || tap == 5) ? (uint32_t)(M::PITCH - 2) : 1u;
+#pragma unroll
+              for (int ks = 0; ks < NKS; ++ks) {
+                desc_add(da[ks][0], ainc);
+                desc_add(da[ks][1], ainc);
+                desc_add(db[ks][0], TAP16);
+                desc_add(db[ks][1], TAP16);
               }
             }
-            if (p.store1) {
-              p.out[((long long)zo * p.Ho + yo) * p.Wo + xo] = __uint_as_float(r[0]);
-            } else {
-              // (K-slice variant: p.out is the scratch, every slice stores its partial sums)
-              float4* dst = reinterpret_cast<float4*>(
-                  p.out + (KSLICE ? it.split * p.slice_stride : 0) +
-                  (((long long)zo * p.Ho + yo) * p.Wo + xo) * p.Cout + ch0);
+          }
+          if constexpr (MODE == TC_S2) {
+            // one K step per 16-channel stage.  Even input planes feed window plane 0 (kz = 1);
+            // odd planes feed planes 0 and 1 (kz = 2, kz = 0) with one N = 2*NCTA MMA.
+            constexpr uint32_t KCH16 = CIN / 8;
+            const uint32_t odd = (uint32_t)zi & 1u;
+            auto run = [&](auto nbc) {
+              constexpr uint32_t NB = decltype(nbc)::value;
+              constexpr uint32_t b_lbo16 = NB * NCTA;
+              constexpr uint32_t tap16 = KCH16 * b_lbo16;
+              const uint32_t b_lo0 = ((w_base >> 4) & 0x3FFF) + (NB == 2 ? 9u * KCH16 * NCTA : 0u) +
+                                     (uint32_t)(cg * NCH) * b_lbo16 + (b_lbo16 << 16);
+              uint64_t dbh = pack64(b_lo0, b_desc_hi);
+              uint64_t dbl = pack64(b_lo0 + w_hi16, b_desc_hi);
 #pragma unroll
-              for (int q = 0; q < EW / 4; ++q)
-                dst[q] = make_float4(__uint_as_float(r[4 * q]), __uint_as_float(r[4 * q + 1]),
-                                     __uint_as_float(r[4 * q + 2]), __uint_as_float(r[4 * q + 3]));
-            }
-            if constexpr (!KSLICE) {
-              if (p.stats) {
-                const float wz = (zo >= p.zw_lo && zo < p.zw_hi) ? p.zw : 1.f;
+              for (int tap = 0; tap < 9; ++tap) {
+                const int dy = tap / 3, dx = tap % 3;
+                const uint32_t a16 = (uint32_t)(((dx & 1) * 2 + (dy & 1)) * S2_CLS16 +
+                                                (dy >> 1) * M::PITCH + (dx >> 1));
+                const uint64_t dah = pack64(a_lo_stage + a16, a_desc_hi);
+                const uint64_t dal = pack64(a_lo_stage + a16 + A_HL16, a_desc_hi);
+                wgmma_bf16<NB * NCTA>(acc, dah, dbh);
+                wgmma_bf16<NB * NCTA>(acc, dal, dbh);
+                wgmma_bf16<NB * NCTA>(acc, dah, dbl);
+                desc_add(dbh, tap16);
+                desc_add(dbl, tap16);
+              }
+            };
+            if (odd) run(std::integral_constant<uint32_t, 2>());
+            else run(std::integral_constant<uint32_t, 1>());
+          }
+          if constexpr (MODE == TC_T) {
+            // the op list of tc_build_program<TC_T>: shift (0,0) one run of 12 class blocks from
+            // block 0; x-only / y-only shifts one (zero-padded) run of 10 blocks from block 1 /
+            // block 2; diagonal shift single blocks 2, 6, 10
+            constexpr uint32_t KCH16 = CIN / 8;
+            constexpr uint32_t NB[4] = {12u, 10u, 10u, 3u};      // blocks per weight image
+            constexpr uint32_t LIN0[4] = {0u, 1u, 2u, 2u};
+            uint32_t b_img16 = (w_base >> 4) & 0x3FFF;  // start of this shift's weight image
 #pragma unroll
-                for (int i = 0; i < EW; ++i) {
-                  const float v = __uint_as_float(r[i]);
-                  ssum[sub * EW + i] = fmaf(wz, v, ssum[sub * EW + i]);
-                  ssq[sub * EW + i] = fmaf(wz * v, v, ssq[sub * EW + i]);
+            for (int sh = 0; sh < 4; ++sh) {
+              const uint32_t b_lbo16 = NB[sh] * NCTA;
+              const uint32_t a16 = (uint32_t)((sh >> 1) * M::PITCH + (sh & 1));
+#pragma unroll
+              for (int ks = 0; ks < CG / 16; ++ks) {
+                const uint32_t alo = a_lo_stage + a16 + 2 * ks * A_LBO16;
+                const uint64_t dah = pack64(alo, a_desc_hi);
+                const uint64_t dal = pack64(alo + A_HL16, a_desc_hi);
+                const uint32_t blo = b_img16 + (uint32_t)(cg * NCH + 2 * ks) * b_lbo16 +
+                                     (b_lbo16 << 16);
+                auto mma3 = [&](float* d, uint32_t bl, auto nc) {
+                  constexpr int N = decltype(nc)::value;
+                  const uint64_t dbh = pack64(bl, b_desc_hi);
+                  const uint64_t dbl = pack64(bl + w_hi16, b_desc_hi);
+                  wgmma_bf16<N>(d, dah, dbh);
+                  wgmma_bf16<N>(d, dal, dbh);
+                  wgmma_bf16<N>(d, dah, dbl);
+                };
+                if (sh == 0) {
+                  mma3(acc, blo, std::integral_constant<int, 12 * NCTA>());
+                } else if (sh == 1) {
+                  mma3(acc + NCTA / 2, blo, std::integral_constant<int, 10 * NCTA>());
+                } else if (sh == 2) {
+                  mma3(acc + NCTA, blo, std::integral_constant<int, 10 * NCTA>());
+                } else {
+#pragma unroll
+                  for (uint32_t k = 0; k < 3; ++k)
+                    mma3(acc + (LIN0[3] + k * 4) * (NCTA / 2), blo + k * NCTA,
+                         std::integral_constant<int, NCTA>());
                 }
               }
+              b_img16 += KCH16 * b_lbo16;
             }
           }
+          wgmma_commit();
+          wgmma_wait<0>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_a(s));  // stage refillable: its MMAs have retired
         }
+        // planes whose last contribution was this input plane leave the window
+        if constexpr (MODE == TC_S1) {
+          emit(it, std::integral_constant<int, 0>(), zi - 1);
+          shift(std::integral_constant<int, 1>());
+        } else if constexpr (MODE == TC_S2) {
+          if (zi & 1) {
+            emit(it, std::integral_constant<int, 0>(), zi >> 1);
+            shift(std::integral_constant<int, 1>());
+          }
+        } else {
+          emit(it, std::integral_constant<int, 0>(), 2 * zi - 1);
+          emit(it, std::integral_constant<int, 1>(), 2 * zi);
+          shift(std::integral_constant<int, 2>());
         }
       }
+      // the planes still open after the item's last input plane
+      const int zb = Win::base(zi1 + 1);
+      emit(it, std::integral_constant<int, 0>(), zb);
+      emit(it, std::integral_constant<int, 1>(), zb + 1);
+      if constexpr (Win::NPL > 2) emit(it, std::integral_constant<int, 2>(), zb + 2);
+#pragma unroll
+      for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
       // a CTA keeps one output-channel group, so one flush per item keeps the fp32
-      // partial sums short (<= planes-per-item * classes values per thread)
-      flush_stats();
+      // partial sums short (<= planes-per-item * classes * 2 values per thread)
+      flush_stats(it.split);
     }
     if (timed) {
       unsigned long long* rc = p.role_cycles + (size_t)blockIdx.x * 8;
-      rc[5] = (unsigned long long)(clock64() - t_begin);
-      rc[6] = t_wait_f;
+      rc[0] = (unsigned long long)(clock64() - t_begin);
+      rc[1] = t_wait_a;
     }
   }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == MMA_WARP)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(TMEM_COLS));
 }
 
 // ----------------------------------------------------------------------------------
@@ -1478,11 +1240,6 @@ inline int tc_consume_error() {
   const int h = *reinterpret_cast<volatile int*>(f.host);
   if (h) *reinterpret_cast<volatile int*>(f.host) = 0;
   return h;
-}
-inline int tc_sm_count() {
-  int& cached = per_device<int, 1>();
-  if (!cached) cudaDeviceGetAttribute(&cached, cudaDevAttrMultiProcessorCount, cur_device());
-  return cached;
 }
 
 // out[v][c] = sum over slices (in slice order) of part[s][v][c], C = 64; optional per-channel
@@ -1553,8 +1310,7 @@ bool tc_launch(const Loader& ld, const TcWeights& w, float* out, double* stats,
   constexpr int CG = M::CG < CIN ? M::CG : CIN;
   constexpr size_t STAGE_BYTES = Loader::kTma ? (size_t)2 * 4 * TMA_S2_CLSR * 16
                                               : (size_t)2 * (CG / 8) * M::ROWS * 16;
-  const size_t smem = w.image_bytes + M::NSTAGE * STAGE_BYTES +
-                      (2 * M::NSTAGE + 2 * M::NSLOT) * 8 + 16;
+  const size_t smem = w.image_bytes + M::NSTAGE * STAGE_BYTES + (2 * M::NSTAGE + 1) * 8;
   auto kern = conv_tc_kernel<MODE, CIN, NCTA, Loader>;
   struct AttrTag { size_t v = 0; };
   static AttrTag attr_dev[kMaxDevices];  // per kernel instantiation and device
@@ -1589,8 +1345,6 @@ bool tc_launch(const Loader& ld, const TcWeights& w, float* out, double* stats,
   p.nsplit = w.nsplit;
   p.w_bytes = w.image_bytes;
   p.w_hi_bytes = w.hi_bytes;
-  p.prog[0] = w.prog[0];
-  p.prog[1] = w.prog[1];
   p.z_unit = MODE == TC_T ? 2 : 1;
   const long long cols = (long long)p.tiles_x * p.tiles_y;
   const long long units = cols * (g.Do / p.z_unit);
@@ -1618,10 +1372,9 @@ bool tc_launch(const Loader& ld, const TcWeights& w, float* out, double* stats,
     for (int b = 0; b < grid; ++b)
       for (int k = 0; k < 8; ++k) a[k] += (double)h[(size_t)b * 8 + k] / grid;
     fprintf(stderr,
-            "[tc mode=%d cin=%d ncta=%d grid=%d cols=%lld Do=%d] mma: total %.0f wait_full_a %.0f "
-            "wait_empty_acc %.0f | load: total %.0f wait_empty_a %.0f | epi: total %.0f "
-            "wait_full_acc %.0f | prologue %.0f\n",
-            MODE, CIN, NCTA, grid, cols, g.Do, a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7]);
+            "[tc mode=%d cin=%d ncta=%d grid=%d cols=%lld Do=%d] mma+epilogue: total %.0f "
+            "wait_full_a %.0f | load: total %.0f wait_empty_a %.0f\n",
+            MODE, CIN, NCTA, grid, cols, g.Do, a[0], a[1], a[3], a[4]);
   }
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
@@ -1664,7 +1417,7 @@ bool tc_dispatch(const Loader& ld, const TcWeights& w, float* out, double* stats
                      : tc_launch<TC_S1, 16, 64, Loader>(ld, w, part, nullptr, g, st, err, o2);
     }
     if (!launched) return false;
-    const int blocks = (int)std::min<long long>(148 * 8, (V + 15) / 16);
+    const int blocks = (int)std::min<long long>(8LL * tc_sm_count(), (V + 15) / 16);
     kslice_reduce_kernel<<<blocks, 256, 0, st>>>(part, w.nsplit, V, (long long)g.Ho * g.Wo, out,
                                                  stats, opt.zw_lo, opt.zw_hi, opt.zw);
     if (cudaGetLastError() != cudaSuccess) {

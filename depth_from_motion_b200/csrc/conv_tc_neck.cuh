@@ -1,21 +1,23 @@
-// tcgen05 3x3x3 conv for the BEV necks (DfMNeck / OutdoorImVoxelNeck, SURVEY.md 8a row a7):
+// wgmma 3x3x3 conv for the BEV necks (DfMNeck / OutdoorImVoxelNeck, SURVEY.md 8a row a7):
 // 64..256 channels on a [Nx=220][Ny=300][Nz<=12] voxel grid, strides (1,1,1) / (1,1,2),
 // pads (1,1,1) / (1,1,0).
 //
 // Same operand formulation as conv_tc.cuh (bf16 hi/lo split, K-major no-swizzle bricks, one
 // brick serves the 9 in-plane taps, kz folded into N), but the loop nest is K-outer because
 // the weights (27*Cin*Cout*4 B, up to 7 MB) cannot stay resident:
-//   * a CTA owns a 16 (x) x 8 (y) tile and ALL (<= 12) output planes of the short z axis;
-//     their accumulators (32 output channels each) live in TMEM for the whole item;
+//   * a CTA owns a 16 (x) x 8 (y) tile and a window of output planes of the short z axis
+//     (as many as NK_ACC_COLS accumulator columns hold; taller volumes are cut into windows
+//     whose halo planes are real data); the accumulators live in the registers of the two
+//     consumer warpgroups for the whole item;
 //   * for each 32-channel input group: copy that group's 110.6 KB weight image to shared
 //     memory, then march the input planes through the usual loader -> MMA pipeline;
-//   * after the last group the epilogue drains the planes (raw conv output; BatchNorm/ReLU
+//   * after the last group the consumers store the planes (raw conv output; BatchNorm/ReLU
 //     are applied by the consumer's load, like everywhere else).
 // "Windowed" use (neck_tc_conv_dhw): the same kernel runs the 64-channel stride-1 layers of the
-// plane-sweep volume [D][H][W][C] -- tile over (H, W), marched axis D cut into chunks of <= 16
-// output planes whose halo planes are real data -- because there the resident-weight kernel
-// (conv_tc.cuh) has to split the output channels four ways and issues N = 48 MMAs at the 47-cycle
-// floor; here an MMA covers 32 output channels x 3 planes (N = 96).
+// plane-sweep volume [D][H][W][C] -- tile over (H, W), marched axis D cut into windows of output
+// planes whose halo planes are real data -- because there the resident-weight kernel
+// (conv_tc.cuh) has to split the output channels four ways and issues N = 48 MMAs; here an MMA
+// covers 32 output channels x 3 planes (N = 96).
 #pragma once
 #include "conv_tc.cuh"
 
@@ -24,18 +26,20 @@ namespace dfm {
 constexpr int NK_BX = 8, NK_BY = 16;           // tile: 8 along y (brick x), 16 along x (brick y)
 constexpr int NK_PX = NK_BX + 2, NK_PY = NK_BY + 2;
 constexpr int NK_ROWS = 186;                    // 180 brick rows padded (== 2 mod 8)
+// accumulator columns per CTA: 64 registers per consumer thread
+constexpr int NK_ACC_COLS = 128;
 // Two shapes of the per-CTA weight image (always 110.6 KB = 9 taps x CG x 3*NCTA x hi/lo):
-//   CG = 32 input channels per group, NCTA = 32 output channels per CTA (any plane count <= 16)
-//   CG = 16, NCTA = 64: every loaded brick feeds twice the MMA columns (N = 192 / 64 instead of
+//   CG = 32 input channels per group, NCTA = 32 output channels per CTA (4 planes per window)
+//   CG = 16, NCTA = 64: every loaded brick feeds twice the MMA columns (N = 128 / 64 instead of
 //   96 / 32) and the output channels are split half as often, i.e. every brick is loaded half as
-//   often -- for layers with <= 8 output planes per tile (64 TMEM columns per plane).  The loaders
-//   bound these kernels, so this is what decides the small-Nz neck layers.
+//   often -- for layers with <= 2 output planes per tile (64 accumulator columns per plane).
 template <int CG>
 struct NkCfg {
   static constexpr int NCH = CG / 8;             // 16-byte channel chunks per stage
   static constexpr int NCTA = 1024 / CG;         // output channels per CTA
   static constexpr int KS = CG / 16;             // K steps per tap
   static constexpr int NSTAGE = CG == 32 ? 4 : 8;
+  static constexpr int ZMAX = NK_ACC_COLS / NCTA;  // (tile, plane) accumulators of an item
   static constexpr uint32_t STAGE_BYTES = 2 * NCH * NK_ROWS * 16;
   static constexpr uint32_t B_LBO16 = 3 * NCTA;  // rows of a group image: [kw block][NCTA]
   static constexpr uint32_t TAP16 = NCH * B_LBO16;   // one in-plane tap, 16-byte units (= 384)
@@ -44,8 +48,9 @@ constexpr uint32_t NK_TAP16 = 4 * 96;           // == NkCfg<32>::TAP16 == NkCfg<
 constexpr uint32_t NK_WHI_BYTES = 9 * NK_TAP16 * 16;
 constexpr uint32_t NK_W_BYTES = 2 * NK_WHI_BYTES;
 constexpr int NK_MAX_NCTA = 64;
-constexpr int NK_LOAD_THREADS = 320;   // 2 groups x 5 warps (15 warps: 128 registers/thread still fit)
-constexpr int NK_THREADS = 128 + NK_LOAD_THREADS + 32;
+constexpr int NK_MMA_THREADS = 256;    // two warpgroups: MMA issue + epilogue, 64 rows each
+constexpr int NK_LOAD_THREADS = 256;   // 2 groups x 4 warps
+constexpr int NK_THREADS = NK_MMA_THREADS + NK_LOAD_THREADS;  // 16 warps: 128 registers/thread
 
 enum { NKZ_S1P1 = 0, NKZ_S2P1 = 1, NKZ_S1P0 = 2 };
 
@@ -126,12 +131,12 @@ struct NeckParams {
   int zmode;
   int tiles_x, tiles_y, nsplit, ncg, n_items;
   int ntiles;   // tiles_x * tiles_y
-  int tpi;      // tiles per item: their accumulators (ZC * 32 columns each) share the 512 TMEM
-                // columns, so one 110 KB weight image serves tpi tiles before it is replaced
+  int tpi;      // tiles per item: their accumulators (ZC * NCTA columns each) share the
+                // NK_ACC_COLS register columns, so one 110 KB weight image serves tpi tiles
   // voxel strides of (tile-y axis "x", tile-x axis "y", marched axis) for the input / output
   long long in_sx, in_sy, in_sz, out_sx, out_sy, out_sz;
   int ZC;       // output planes per item along the marched axis (== Zo unless windowed)
-  int nchunk;   // windows along the marched axis (1 unless windowed; windowed needs NKZ_S1P1)
+  int nchunk;   // windows along the marched axis (1 unless windowed; not for NKZ_S1P0)
   double* stats;            // optional per-output-channel (sum, sum of squares) of the raw output
   int zw_lo, zw_hi;         // planes [zw_lo, zw_hi) enter the statistics with weight zw
   float zw;
@@ -198,13 +203,14 @@ __device__ __forceinline__ void nk_plane_map(int zmode, int iz, int zo_lo, int z
   } else if (zmode == NKZ_S2P1) { // rows [kw=2|0|1]; iz = 2q+1 -> planes q, q+1; iz = 2q -> q
     const int q = iz >> 1;
     if (iz & 1) {
-      n0 = 0;
-      nblk = q + 1 < zo_hi ? 2 : 1;
-      zo0 = q;
+      const int first = max(q, zo_lo), last = min(q + 1, zo_hi - 1);
+      n0 = first - q;
+      nblk = last - first + 1;
+      zo0 = first - zo_lo;
     } else {
       n0 = 2;
       nblk = 1;
-      zo0 = q;
+      zo0 = q - zo_lo;
     }
   } else {                        // pad 0, single output plane: kw = iz
     n0 = iz;
@@ -213,7 +219,7 @@ __device__ __forceinline__ void nk_plane_map(int zmode, int iz, int zo_lo, int z
   }
 }
 
-// item -> (first tile, tiles, marched-axis window)
+// item -> (first tile, tiles, marched-axis window and the input planes it reads)
 struct NkItem {
   int tile0, nt, zo_lo, zo_hi, iz_lo, nzi;
 };
@@ -225,14 +231,36 @@ __device__ __forceinline__ NkItem nk_item(const NeckParams& p, int item) {
   it.nt = min(p.tpi, p.ntiles - it.tile0);
   it.zo_lo = chunk * p.ZC;
   it.zo_hi = min(it.zo_lo + p.ZC, p.Zo);
-  if (p.nchunk > 1) {  // windowed NKZ_S1P1: halo planes are real data where they exist
+  // halo planes of a window are real data where they exist
+  int iz_hi;
+  if (p.zmode == NKZ_S1P1) {
     it.iz_lo = max(it.zo_lo - 1, 0);
-    it.nzi = min(it.zo_hi + 1, p.Zi) - it.iz_lo;
+    iz_hi = min(it.zo_hi + 1, p.Zi);
+  } else if (p.zmode == NKZ_S2P1) {
+    it.iz_lo = max(2 * it.zo_lo - 1, 0);
+    iz_hi = min(2 * it.zo_hi, p.Zi);
   } else {
     it.iz_lo = 0;
-    it.nzi = p.Zi;
+    iz_hi = p.Zi;
   }
+  it.nzi = iz_hi - it.iz_lo;
   return it;
+}
+
+// calls f(Q, NB) with compile-time Q == q, NB == nb (Q + NB <= ZMAX)
+template <int Q, int ZMAX, class F>
+__device__ __forceinline__ void nk_dispatch(int q, int nb, F&& f) {
+  if constexpr (Q < ZMAX) {
+    if (q == Q) {
+      if (nb == 1) f(std::integral_constant<int, Q>(), std::integral_constant<int, 1>());
+      if constexpr (Q + 2 <= ZMAX)
+        if (nb == 2) f(std::integral_constant<int, Q>(), std::integral_constant<int, 2>());
+      if constexpr (Q + 3 <= ZMAX)
+        if (nb == 3) f(std::integral_constant<int, Q>(), std::integral_constant<int, 3>());
+    } else {
+      nk_dispatch<Q + 1, ZMAX>(q, nb, f);
+    }
+  }
 }
 
 template <int NT, int CG>
@@ -240,63 +268,43 @@ __global__ void __launch_bounds__(NK_THREADS, 1)
 neck_conv_kernel(const __grid_constant__ NeckParams p) {
   using Cfg = NkCfg<CG>;
   constexpr int NCH = Cfg::NCH, NK_NCTA = Cfg::NCTA, KS = Cfg::KS, NK_NSTAGE = Cfg::NSTAGE;
+  constexpr int ZMAX = Cfg::ZMAX;
   constexpr uint32_t NK_STAGE_BYTES = Cfg::STAGE_BYTES;
   constexpr uint32_t A_LBO = NK_ROWS * 16, A_SBO = NK_PX * 16, A_HL = NCH * NK_ROWS * 16;
   constexpr uint32_t A_LBO16 = A_LBO >> 4, A_HL16 = A_HL >> 4, B_LBO16 = Cfg::B_LBO16;
-  constexpr uint32_t TMEM_COLS = 512;
   constexpr int NPOS = NK_PX * NK_PY, LG_THREADS = NK_LOAD_THREADS / 2;
   constexpr int NITEM = (NPOS * NCH + LG_THREADS - 1) / LG_THREADS;
   constexpr int LB = NITEM < 6 / NT ? NITEM : 6 / NT;
+  constexpr int NACC = ZMAX * NK_NCTA / 2;
+  constexpr int LOAD_WARP0 = NK_MMA_THREADS / 32;
 
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* w_s = smem;
   uint8_t* a_s = smem + NK_W_BYTES;
   uint64_t* bars = reinterpret_cast<uint64_t*>(a_s + NK_NSTAGE * NK_STAGE_BYTES);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * NK_NSTAGE + 4);
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
   const uint32_t bar0 = smem_u32(bars);
   auto full_a = [&](int s) { return bar0 + 8u * s; };
   auto empty_a = [&](int s) { return bar0 + 8u * (NK_NSTAGE + s); };
   const uint32_t w_full = bar0 + 8u * (2 * NK_NSTAGE), w_empty = w_full + 8;
-  const uint32_t acc_full = w_full + 16, acc_empty = w_full + 24;
-  constexpr int MMA_WARP = NK_THREADS / 32 - 1;
 
   if (tid == 0) {
     for (int s = 0; s < NK_NSTAGE; ++s) {
       mbar_init(full_a(s), LG_THREADS / 32);
-      mbar_init(empty_a(s), 1);
+      mbar_init(empty_a(s), NK_MMA_THREADS / 32);
     }
     mbar_init(w_full, NK_LOAD_THREADS / 32);
-    mbar_init(w_empty, 1);
-    mbar_init(acc_full, 1);
-    mbar_init(acc_empty, 4);
+    mbar_init(w_empty, NK_MMA_THREADS / 32);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == MMA_WARP) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(tmem_slot)),
-                 "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  if (warp < 4) {  // accumulators start at zero and are re-zeroed by the epilogue
-    for (uint32_t c = 0; c < TMEM_COLS; c += 64)
-      tmem_zero<64>(tmem_base + ((uint32_t)(warp * 32) << 16) + c);
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 
   const int split = blockIdx.x % p.nsplit;
 
-  if (warp >= 4 && warp < MMA_WARP) {
+  if (warp >= LOAD_WARP0) {
     // ============================ loaders ============================
-    const int lw = warp - 4, lgrp = lw & 1;
+    const int lw = warp - LOAD_WARP0, lgrp = lw & 1;
     const int lt = (lw >> 1) * 32 + lane, lall = lw * 32 + lane;
     const int chunk = lt % NCH;
     uint32_t stage_ctr = 0, w_ctr = 0;
@@ -363,151 +371,136 @@ neck_conv_kernel(const __grid_constant__ NeckParams p) {
         }
       }
     }
-  } else if (warp == MMA_WARP) {
-    // ============================ MMA issuer (warp-uniform) ============================
+  } else {
+    // ================= consumers: two MMA + epilogue warpgroups (64 rows each) =================
+    // The accumulators of all (tile, plane) pairs of an item stay in registers across the
+    // input-channel groups; plane P = t * ZC + (zo - zo_lo) owns registers [P, P+1) * NCTA / 2.
+    const int wg = warp >> 2, wq = warp & 3;
+    const int xr = lane >> 2, cq = lane & 3;
     const uint32_t w_base = smem_u32(w_s), a_base = smem_u32(a_s);
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-    const uint32_t a_desc_hi = (A_SBO >> 4) | (1u << 14), b_desc_hi = (128u >> 4) | (1u << 14);
+    const uint32_t a_desc_hi = A_SBO >> 4, b_desc_hi = 128u >> 4;
     const uint32_t w_hi16 = NK_WHI_BYTES >> 4;
-    uint32_t stage_ctr = 0, w_ctr = 0, item_ctr = 0;
-    for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++item_ctr) {
-      // the previous item's accumulators must have been drained (and re-zeroed)
-      mbar_wait(acc_empty, (item_ctr & 1) ^ 1, p.err);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    const uint32_t a_wg16 = (uint32_t)wg * 8u * (A_SBO >> 4);
+    float acc[NACC];
+#pragma unroll
+    for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+    constexpr int NST = NK_NCTA / 4;
+    float ssum[NST], ssq[NST];   // GroupNorm sums of this item (p.stats), fp32
+#pragma unroll
+    for (int i = 0; i < NST; ++i) ssum[i] = ssq[i] = 0.f;
+    uint32_t stage_ctr = 0, w_ctr = 0;
+    for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
       const NkItem it = nk_item(p, item);
       const int nt = it.nt;
       for (int cg = 0; cg < p.ncg; ++cg, ++w_ctr) {
         mbar_wait(w_full, w_ctr & 1, p.err);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
         for (int t = 0; t < nt; ++t) {
           for (int izl = 0; izl < it.nzi; ++izl, ++stage_ctr) {
             const int s = stage_ctr % NK_NSTAGE;
             mbar_wait(full_a(s), (stage_ctr / NK_NSTAGE) & 1, p.err);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+            __syncwarp();
             int n0, nblk, zo0;
             nk_plane_map(p.zmode, it.iz_lo + izl, it.zo_lo, it.zo_hi, n0, nblk, zo0);
-            const uint32_t d0 = tmem_u + (uint32_t)(t * p.ZC + zo0) * NK_NCTA;
-            const uint32_t idesc = idesc_bf16(nblk * NK_NCTA);
-            const uint32_t a_lo_stage = (((a_base + s * NK_STAGE_BYTES) >> 4) & 0x3FFF) | (A_LBO16 << 16);
+            const uint32_t a_lo_stage =
+                ((((a_base + s * NK_STAGE_BYTES) >> 4) & 0x3FFF) + a_wg16) | (A_LBO16 << 16);
             const uint32_t b_lo0 = ((w_base >> 4) & 0x3FFF) + (uint32_t)n0 * NK_NCTA + (B_LBO16 << 16);
-            uint64_t da[KS][2], db[KS][2];
-#pragma unroll
-            for (int ks = 0; ks < KS; ++ks) {
-              da[ks][0] = pack64(a_lo_stage + 2 * ks * A_LBO16, a_desc_hi);
-              da[ks][1] = pack64(a_lo_stage + 2 * ks * A_LBO16 + A_HL16, a_desc_hi);
-              db[ks][0] = pack64(b_lo0 + 2 * ks * B_LBO16, b_desc_hi);
-              db[ks][1] = pack64(b_lo0 + 2 * ks * B_LBO16 + w_hi16, b_desc_hi);
-            }
-#pragma unroll 1
-            for (int tap = 0; tap < 9; ++tap) {
-              if (elect_one()) {
-#pragma unroll
-                for (int ks = 0; ks < KS; ++ks) {
-                  umma_bf16(d0, da[ks][0], db[ks][0], idesc, 1u);
-                  umma_bf16(d0, da[ks][1], db[ks][0], idesc, 1u);
-                  umma_bf16(d0, da[ks][0], db[ks][1], idesc, 1u);
-                }
-              }
-              const uint32_t ainc = (tap == 2 || tap == 5) ? (uint32_t)(NK_PX - 2) : 1u;
+            wgmma_fence();
+            nk_dispatch<0, ZMAX>(t * p.ZC + zo0, nblk, [&](auto qc, auto nbc) {
+              constexpr int Q = decltype(qc)::value, NB = decltype(nbc)::value;
+              float* d = acc + Q * (NK_NCTA / 2);
+              uint64_t da[KS][2], db[KS][2];
 #pragma unroll
               for (int ks = 0; ks < KS; ++ks) {
-                desc_add(da[ks][0], ainc);
-                desc_add(da[ks][1], ainc);
-                desc_add(db[ks][0], NK_TAP16);
-                desc_add(db[ks][1], NK_TAP16);
+                da[ks][0] = pack64(a_lo_stage + 2 * ks * A_LBO16, a_desc_hi);
+                da[ks][1] = pack64(a_lo_stage + 2 * ks * A_LBO16 + A_HL16, a_desc_hi);
+                db[ks][0] = pack64(b_lo0 + 2 * ks * B_LBO16, b_desc_hi);
+                db[ks][1] = pack64(b_lo0 + 2 * ks * B_LBO16 + w_hi16, b_desc_hi);
               }
-            }
-            if (elect_one()) umma_commit(empty_a(s));
-            __syncwarp();
-          }
-        }
-        if (elect_one()) umma_commit(w_empty);  // weights may be replaced once these retire
-        __syncwarp();
-      }
-      if (elect_one()) umma_commit(acc_full);
-      __syncwarp();
-    }
-  } else {
-    // ============================ epilogue (warps 0-3) ============================
-    const int m = warp * 32 + lane;
-    uint32_t item_ctr = 0;
-    constexpr int EW = 32, NSUB = NK_NCTA / EW;   // accumulator columns drained per pass
-    float ssum[EW], ssq[EW];   // GroupNorm sums of this item and column block (p.stats), fp32
-#pragma unroll
-    for (int i = 0; i < EW; ++i) ssum[i] = ssq[i] = 0.f;
-    for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++item_ctr) {
-      const NkItem it = nk_item(p, item);
-      mbar_wait(acc_full, item_ctr & 1, p.err);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 #pragma unroll 1
-      for (int sub = 0; sub < NSUB; ++sub) {
-        for (int t = 0; t < it.nt; ++t) {
-          const int tile = it.tile0 + t;
-          const int y = (tile % p.tiles_x) * NK_BX + (m & 7), x = (tile / p.tiles_x) * NK_BY + (m >> 3);
-          const bool ok = x < p.Nx && y < p.Ny;
-          for (int zo = it.zo_lo; zo < it.zo_hi; ++zo) {
-            uint32_t r[EW];
-            const uint32_t ta = tmem_base + ((uint32_t)(warp * 32) << 16) +
-                                (uint32_t)(t * p.ZC + zo - it.zo_lo) * NK_NCTA + sub * EW;
-            tmem_ld<EW>(ta, r);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            tmem_zero<EW>(ta);
-            if (ok) {
-              float4* dst = reinterpret_cast<float4*>(
-                  p.out + (x * p.out_sx + y * p.out_sy + zo * p.out_sz) * p.Cout +
-                  split * NK_NCTA + sub * EW);
+              for (int tap = 0; tap < 9; ++tap) {
 #pragma unroll
-              for (int q = 0; q < EW / 4; ++q)
-                dst[q] = make_float4(__uint_as_float(r[4 * q]), __uint_as_float(r[4 * q + 1]),
-                                     __uint_as_float(r[4 * q + 2]), __uint_as_float(r[4 * q + 3]));
-              if (p.stats) {
-                const float wz = (zo >= p.zw_lo && zo < p.zw_hi) ? p.zw : 1.f;
+                for (int ks = 0; ks < KS; ++ks) {
+                  wgmma_bf16<NB * NK_NCTA>(d, da[ks][0], db[ks][0]);
+                  wgmma_bf16<NB * NK_NCTA>(d, da[ks][1], db[ks][0]);
+                  wgmma_bf16<NB * NK_NCTA>(d, da[ks][0], db[ks][1]);
+                }
+                const uint32_t ainc = (tap == 2 || tap == 5) ? (uint32_t)(NK_PX - 2) : 1u;
 #pragma unroll
-                for (int i = 0; i < EW; ++i) {
-                  const float v = __uint_as_float(r[i]);
-                  ssum[i] = fmaf(wz, v, ssum[i]);
-                  ssq[i] = fmaf(wz * v, v, ssq[i]);
+                for (int ks = 0; ks < KS; ++ks) {
+                  desc_add(da[ks][0], ainc);
+                  desc_add(da[ks][1], ainc);
+                  desc_add(db[ks][0], NK_TAP16);
+                  desc_add(db[ks][1], NK_TAP16);
                 }
               }
-            }
+            });
+            wgmma_commit();
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty_a(s));
           }
         }
-        if (p.stats) {  // one flush per item and column block keeps the fp32 partial sums short
+        __syncwarp();
+        if (lane == 0) mbar_arrive(w_empty);  // weights may be replaced: their MMAs retired
+      }
+      // ---- epilogue: raw conv output of every (tile, plane) of the item ----
+      const int zc = it.zo_hi - it.zo_lo;
 #pragma unroll
-          for (int i = 0; i < EW; ++i) {
-            double a = ssum[i], b = ssq[i];
+      for (int P = 0; P < ZMAX; ++P) {
+        const int t = P / p.ZC, zo = it.zo_lo + P % p.ZC;
+        if (t < nt && P % p.ZC < zc) {
+          const int tile = it.tile0 + t;
 #pragma unroll
-            for (int o = 16; o; o >>= 1) {
-              a += __shfl_xor_sync(0xffffffffu, a, o);
-              b += __shfl_xor_sync(0xffffffffu, b, o);
+          for (int rr = 0; rr < 2; ++rr) {
+            const int y = (tile % p.tiles_x) * NK_BX + xr;
+            const int x = (tile / p.tiles_x) * NK_BY + 8 * wg + 2 * wq + rr;
+            if (x >= p.Nx || y >= p.Ny) continue;
+            float* dst = p.out + (x * p.out_sx + y * p.out_sy + zo * p.out_sz) * p.Cout +
+                         split * NK_NCTA + 2 * cq;
+            const float wz = (zo >= p.zw_lo && zo < p.zw_hi) ? p.zw : 1.f;
+#pragma unroll
+            for (int j = 0; j < NK_NCTA / 8; ++j) {
+              const float v0 = acc[P * (NK_NCTA / 2) + 4 * j + 2 * rr];
+              const float v1 = acc[P * (NK_NCTA / 2) + 4 * j + 2 * rr + 1];
+              *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(v0, v1);
+              if (p.stats) {
+                ssum[2 * j] = fmaf(wz, v0, ssum[2 * j]);
+                ssq[2 * j] = fmaf(wz * v0, v0, ssq[2 * j]);
+                ssum[2 * j + 1] = fmaf(wz, v1, ssum[2 * j + 1]);
+                ssq[2 * j + 1] = fmaf(wz * v1, v1, ssq[2 * j + 1]);
+              }
             }
-            if (lane == 0) {
-              atomicAdd(p.stats + 2 * (split * NK_NCTA + sub * EW + i), a);
-              atomicAdd(p.stats + 2 * (split * NK_NCTA + sub * EW + i) + 1, b);
-            }
-            ssum[i] = ssq[i] = 0.f;
           }
         }
       }
-      asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc_empty);
+#pragma unroll
+      for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+      if (p.stats) {  // one flush per item keeps the fp32 partial sums short
+#pragma unroll
+        for (int k = 0; k < NST; ++k) {
+          double a = ssum[k], b = ssq[k];
+#pragma unroll
+          for (int o = 4; o < 32; o <<= 1) {
+            a += __shfl_xor_sync(0xffffffffu, a, o);
+            b += __shfl_xor_sync(0xffffffffu, b, o);
+          }
+          if (lane < 4) {
+            const int ch = split * NK_NCTA + 8 * (k >> 1) + 2 * lane + (k & 1);
+            atomicAdd(p.stats + 2 * ch, a);
+            atomicAdd(p.stats + 2 * ch + 1, b);
+          }
+          ssum[k] = ssq[k] = 0.f;
+        }
+      }
     }
   }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == MMA_WARP)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(TMEM_COLS));
 }
 
 inline bool neck_launch(NeckParams& p, int nterms, int cg, cudaStream_t st, std::string* err) {
   const size_t stages = cg == 32 ? (size_t)NkCfg<32>::NSTAGE * NkCfg<32>::STAGE_BYTES
                                  : (size_t)NkCfg<16>::NSTAGE * NkCfg<16>::STAGE_BYTES;
   const int nstage = cg == 32 ? NkCfg<32>::NSTAGE : NkCfg<16>::NSTAGE;
-  const size_t smem = NK_W_BYTES + stages + (2 * nstage + 4) * 8 + 16;
+  const size_t smem = NK_W_BYTES + stages + (2 * nstage + 2) * 8;
   p.err = tc_err_flag().get();
   const int sms = tc_sm_count();
   int grid = std::max(p.nsplit, sms / p.nsplit * p.nsplit);
@@ -542,7 +535,7 @@ inline bool neck_launch(NeckParams& p, int nterms, int cg, cudaStream_t st, std:
 inline int neck_group_for(int cin, int cout, int planes, bool windowed = false) {
   static const bool off = getenv("DFM_NECK_CG32") != nullptr;   // A/B runs
   static const bool win = getenv("DFM_NECK_WIN") != nullptr;
-  const bool fits = planes * 64 <= 512 || (windowed && win);
+  const bool fits = planes * 64 <= NK_ACC_COLS || (windowed && win);
   return (!off && fits && cout % 64 == 0 && cin % 16 == 0) ? 16 : 32;
 }
 
@@ -560,14 +553,15 @@ inline bool neck_tc_conv(const Src& s, const NeckTcWeights& w, float* out, const
   p.tiles_y = (g.Di + NK_BY - 1) / NK_BY;   // along Nx
   const int ncta = 1024 / w.cg;
   // more planes than the accumulators hold in this group shape: windows along the short axis
-  // (stride 1, pad 1 only; their halo planes are real data)
+  // (pad 1 only; their halo planes are real data)
+  const int zmax = NK_ACC_COLS / ncta;
   int zc = g.Wo, nchunk = 1;
-  if (g.Wo * ncta > 512) {
-    if (w.zmode != NKZ_S1P1) {
+  if (g.Wo > zmax) {
+    if (w.zmode == NKZ_S1P0) {
       if (err) *err = "neck_tc_conv: the weight image's group shape does not fit this plane count";
       return false;
     }
-    nchunk = (g.Wo * ncta + 511) / 512;
+    nchunk = (g.Wo + zmax - 1) / zmax;
     zc = (g.Wo + nchunk - 1) / nchunk;
     nchunk = (g.Wo + zc - 1) / zc;
   }
@@ -579,11 +573,11 @@ inline bool neck_tc_conv(const Src& s, const NeckTcWeights& w, float* out, const
   p.ZC = zc;
   p.nchunk = nchunk;
   p.stats = nullptr;
-  // tiles per item: as many as the 512 TMEM columns hold (Zo * 32 columns per tile), but not so
+  // tiles per item: as many as the accumulators hold (zc * NCTA columns per tile), but not so
   // many that the persistent grid runs short of items
   const int tpi_env = getenv("DFM_NECK_TPI") ? atoi(getenv("DFM_NECK_TPI")) : 0;  // tests / A-B runs
   {
-    const int cap = std::max(1, 512 / (zc * ncta));
+    const int cap = std::max(1, zmax / zc);
     const int sms0 = tc_sm_count();
     int tpi = std::min(cap, std::max(1, p.ntiles * nchunk * p.nsplit / (2 * sms0)));
     if (tpi_env > 0) tpi = std::min(cap, tpi_env);
@@ -594,7 +588,7 @@ inline bool neck_tc_conv(const Src& s, const NeckTcWeights& w, float* out, const
 }
 
 // Plane-sweep-volume orientation: [D][H][W][C], stride 1, pad 1; tiles over (H: 16, W: 8), the
-// D axis cut into windows of `zc` output planes (<= 16: 32 TMEM columns each).  `w` must have
+// D axis cut into windows of `zc` output planes (<= NK_ACC_COLS / NCTA).  `w` must have
 // been built with dhw = true.  stats: optional GroupNorm sums of the raw output (zeroed by the
 // caller), planes [zw_lo, zw_hi) weighted by zw.
 inline bool neck_dhw_supported(const ConvGeom& g) {
@@ -611,12 +605,12 @@ inline NeckDhwPlan neck_dhw_plan(const ConvGeom& g, int ncta = 32) {
   const int sms = tc_sm_count();
   const int ntiles = ((g.Wi + NK_BX - 1) / NK_BX) * ((g.Hi + NK_BY - 1) / NK_BY);
   const int nsplit = g.Cout / ncta;
-  const int zmax = std::min(g.Do, 512 / ncta);
+  const int zmax = std::min(g.Do, NK_ACC_COLS / ncta);
   NeckDhwPlan best{zmax, 1, 0};
   double best_cost = 1e30;
   for (int zc = zmax; zc >= std::min(g.Do, 4); --zc) {
     const int nchunk = (g.Do + zc - 1) / zc;
-    for (int tpi = 1; tpi <= 512 / (zc * ncta); ++tpi) {
+    for (int tpi = 1; tpi <= NK_ACC_COLS / (zc * ncta); ++tpi) {
       const int items = (ntiles + tpi - 1) / tpi * nchunk * nsplit;
       const int rounds = (items + sms - 1) / sms;
       const double cost = rounds * (tpi * (zc + 2.0) + 1.5);
@@ -655,10 +649,10 @@ inline bool neck_tc_conv_dhw(const Src& s, const NeckTcWeights& w, float* out, c
   // tests / A-B runs (read per call, like DFM_NECK_TPI)
   const int zc_env = getenv("DFM_NECK_ZC") ? atoi(getenv("DFM_NECK_ZC")) : 0;
   const int tpi_env = getenv("DFM_NECK_ZTPI") ? atoi(getenv("DFM_NECK_ZTPI")) : 0;
-  p.ZC = std::min(zc_env > 0 ? std::min(zc_env, 512 / ncta) : plan.zc, g.Do);
+  p.ZC = std::min(zc_env > 0 ? std::min(zc_env, NK_ACC_COLS / ncta) : plan.zc, g.Do);
   p.nchunk = (g.Do + p.ZC - 1) / p.ZC;
   // (the window logic of nk_item serves nchunk == 1 too: iz_lo = 0, nzi = Zi)
-  p.tpi = std::max(1, std::min(512 / (p.ZC * ncta), tpi_env > 0 ? tpi_env : plan.tpi));
+  p.tpi = std::max(1, std::min(NK_ACC_COLS / (p.ZC * ncta), tpi_env > 0 ? tpi_env : plan.tpi));
   p.n_items = (p.ntiles + p.tpi - 1) / p.tpi * p.nchunk * p.nsplit;
   p.stats = stats;
   p.zw_lo = zw_lo; p.zw_hi = zw_hi; p.zw = zw;

@@ -1,5 +1,5 @@
 // C-ABI implementation of include/dfm_b200.h: handles, weight repacking, and the
-// per-frame launch sequence of the DfM plane-sweep cost-volume path on one B200.
+// per-frame launch sequence of the DfM plane-sweep cost-volume path on one H100.
 #include "../../include/dfm_b200.h"
 
 #include <cuda_runtime.h>
@@ -193,8 +193,8 @@ int set_conv(ConvW& cw, const float* h, long long numel, int Cin, int Cout, int 
   cw.ntk.release();
   if (tc_mode == dfm::TC_S1 && !transposed && Cin >= 64 && Cin % 32 == 0 && Cout % 32 == 0) {
     std::string err;
-    // (32-channel groups: on these volumes the 16 / 64 shape measured no better -- 0.283 vs
-    // 0.280 ms at 56x48x156, 0.147 vs 0.122 ms at 20x48x156 -- fewer, larger items balance worse)
+    // (32-channel groups: the 16 / 64 shape holds only NK_ACC_COLS / 64 = 2 planes per window,
+    // so every window would re-load two halo planes for two planes of output)
     if (!cw.ntk.build(p.data(), Cin, Cout, dfm::NKZ_S1P1, &err, /*dhw=*/true, 32))
       return fail(DFM_ERR_CUDA, err);
   }
@@ -297,7 +297,7 @@ int gn_finalize(Norm& n, long long V, int groups, cudaStream_t st) {
 
 int run_gn(const float* raw, long long V, Norm& n, int groups, cudaStream_t st) {
   DFM_TRY(n.begin_stats(st));
-  const int blocks = (int)std::min<long long>(148 * 8, (V * n.C + 255) / 256);
+  const int blocks = (int)std::min<long long>(8LL * dfm::tc_sm_count(), (V * n.C + 255) / 256);
   if (n.C == 32)
     dfm::channel_stats_kernel<32><<<blocks, 256, 0, st>>>(raw, V, n.sums);
   else if (n.C == 64)
@@ -824,8 +824,8 @@ int tower_forward(dfm_backbone* bb, Tower& t, bool mono, const dfm::WarpLoader& 
   g = geom_s(D2, H2, W2, 2 * cv, 2 * cv, 1, 1, 1, 1, 1, 1);
   DFM_TRY(run_conv(src1(term(t.b1, &t.gc1, 1)), t.c2, t.b2.p, g, impl, st, &t.gc2, zw_at(2)));
   g = geom_s(D2, H2, W2, 2 * cv, 2 * cv, 2, 2, 2, 1, 1, 1);
-  // (conv3, half resolution: measured neutral-to-worse with TMA -- 0.106 + 0.100 ms producer vs
-  // 0.149 ms with register loaders -- so it is opt-in)
+  // (conv3, half resolution: TMA is opt-in.  H100 SXM, KITTI D=112: register loaders 0.220 + 0.103
+  // ms (stereo + mono); TMA 0.231 + 0.099 ms plus 0.123 + 0.047 ms of producer passes)
   static const bool tma_c3 = getenv("DFM_TMA_CONV3") != nullptr;
   if (tma_c3 && tma_ok(t.c3) && dfm::tc_mode_of(g) == dfm::TC_S2)
     DFM_TRY(run_conv_presplit(src1(term(t.b2, &t.gc2, 1)), t.ps2, t.c3, t.b3.p, g, st, &t.gc3,
@@ -865,7 +865,7 @@ int tower_forward(dfm_backbone* bb, Tower& t, bool mono, const dfm::WarpLoader& 
   // round-1 tensor-core variant (N = 96 MMA, 1/32 useful columns) for A/B runs; the fp32
   // SIMT bring-up path keeps its own independent kernel.
   // Default: logits_tc_kernel (logits_tc.cuh) -- the 27 per-tap dot products of every input
-  // position as one small tcgen05 GEMM, the stencil as a shared-memory gather.  DFM_LOGITS=simt
+  // position as one small wgmma GEMM, the stencil as a shared-memory gather.  DFM_LOGITS=simt
   // selects the CUDA-core variant (tail_kernels.cuh), DFM_LOGITS=mma the round-1 N = 96 MMA.
   static const char* logits_env = getenv("DFM_LOGITS");
   static const bool logits_tc = getenv("DFM_LOGITS_TC") != nullptr ||
@@ -995,7 +995,7 @@ int dfm_backbone_create(const dfm_backbone_desc_t* desc, dfm_backbone_t** out) {
     return fail(DFM_ERR_INVALID, "feature size not compatible with cost_sample_factor");
   int sm = 0, maj = 0, mnr = 0;
   DFM_TRY(dfm_device_info(&sm, &maj, &mnr, nullptr));
-  if (maj != 10) return fail(DFM_ERR_NOGPU, "this library is built for sm_100a only");
+  if (maj != 9) return fail(DFM_ERR_NOGPU, "this library is built for sm_90a only");
   dfm_backbone* bb = new dfm_backbone();
   bb->d = *desc;
   bb->D = D;
@@ -1164,7 +1164,7 @@ int backbone_forward_impl(dfm_backbone_t* bb, const float* d_cur, const float* d
     }
     const int ng = (bb->D + dfm::GT_PG - 1) / dfm::GT_PG;
     const int ntiles = (HWo + dfm::GT4_TP - 1) / dfm::GT4_TP;
-    // equal rounds per block: 234 tiles -> 117 blocks x 2 rather than 148 blocks with 86 doing 2
+    // equal rounds per block: e.g. 234 tiles on 132 SMs -> 117 blocks x 2 rather than 132 blocks with 102 doing 2
     const int sms = dfm::tc_sm_count();
     const int rounds = (ntiles + sms - 1) / sms;
     const int grid = (ntiles + rounds - 1) / rounds;
@@ -1491,7 +1491,7 @@ int dfm_op_conv3d(const float* d_x, int Cin, int Di, int Hi, int Wi, const float
       std::string err;
       // DFM_NTK_CG16=1: exercise the 16-channel-group / 64-output shape in this orientation too
       if (!w.ntk.build(packed.data(), Cin, Cout, dfm::NKZ_S1P1, &err, true,
-                       getenv("DFM_NTK_CG16") ? dfm::neck_group_for(Cin, Cout, 8) : 32) ||
+                       getenv("DFM_NTK_CG16") ? dfm::neck_group_for(Cin, Cout, 1) : 32) ||
           !dfm::neck_tc_conv_dhw(src1(term(xin, nullptr, 0)), w.ntk, yout.p, g, nullptr, 0, 0, 1.f,
                                  st, &err))
         rc = fail(DFM_ERR_CUDA, err);

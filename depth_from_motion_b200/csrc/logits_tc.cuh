@@ -1,25 +1,18 @@
 // 32 -> 1 channel 3x3x3 "logits" conv (build_depth_pred_module's last layer,
 // dfm_backbone.py:128) on the tensor cores, third formulation.
 //
-// With one output channel an implicit-GEMM conv has N = 1: the round-1 kernel ran it as an
-// N = 96 MMA with 1/32 useful columns (0.58 ms per frame), the CUDA-core kernel of
-// tail_kernels.cuh is FMA-pipe / latency bound (0.45 ms).  Here the GEMM is turned around: per
+// With one output channel an implicit-GEMM conv has N = 1.  Here the GEMM is turned around: per
 // INPUT position the 27 per-tap dot products q_t = <x, w_t> are ONE small GEMM
 //     Q[128 positions x 32 (27 taps)] = X[128 x 32 channels] * W^T[32 channels x 32]
-// -- 6 tcgen05.mma (2 K steps x 3 bf16 hi/lo terms) per 128 positions and plane instead of 864
-// FMAs per position -- and the 3x3x3 stencil becomes a gather of Q over the 27 shifted
-// neighbours, done by the epilogue warps from shared memory with three running sums per
-// output pixel along z.
+// -- 12 wgmma (2 halves of 64 positions x 2 K steps x 3 bf16 hi/lo terms) per 128 positions
+// and plane instead of 864 FMAs per position -- and the 3x3x3 stencil becomes a gather of Q over
+// the 27 shifted neighbours, done from shared memory with three running sums per output pixel
+// along z.
 //   * CTA tile: 16 (x) x 8 (y) input positions = 128 accumulator rows, 14 x 6 outputs;
 //     persistent over (tile, z chunk) items, one pipeline stage per input plane.
-//   * warps 0-3 epilogue (TMEM lane = position), 4-11 loaders (the same fused GroupNorm + ReLU
-//     + bf16 split loader as conv_tc.cuh), 12 MMA issuer; two CTAs per SM.
-//   * measured (B200): 0.26 + 0.10 ms for the two towers (CUDA-core kernel 0.31 + 0.14, round-1
-//     N = 96 MMA 0.42 + 0.16).  A variant that staged the raw fp32 rows with cp.async.bulk
-//     (eight 2 KB row copies per plane into a three-deep ring, transform warps reading shared
-//     memory only) was NOT faster (0.28 + 0.11): ncu shows its transform warps waiting for the
-//     row copies -- small bulk copies have a long per-request latency -- so the register
-//     loaders stayed.
+//   * warps 0-3: one consumer warpgroup (wgmma into registers, Q to shared memory, gather),
+//     4-11 loaders (the same fused GroupNorm + ReLU + bf16 split loader as conv_tc.cuh); two
+//     CTAs per SM.
 #pragma once
 #include "conv_tc.cuh"
 
@@ -28,14 +21,14 @@ namespace dfm {
 constexpr int LT_PX = 16, LT_PY = 8;                 // input positions of a tile
 constexpr int LT_OX = LT_PX - 2, LT_OY = LT_PY - 2;  // outputs of a tile
 constexpr int LT_ZC = 16;                            // output planes per item
-constexpr int LT_NSTAGE = 4, LT_NSLOT = 2;          // operand stages, accumulator slots
+constexpr int LT_NSTAGE = 4;                        // operand stages
 constexpr uint32_t LT_A_LBO = 128 * 16;              // chunk stride (128 rows x 16 B)
 constexpr uint32_t LT_A_HL = 4 * LT_A_LBO;           // hi -> lo
 constexpr uint32_t LT_STAGE_BYTES = 2 * LT_A_HL;     // 16 KB
 constexpr uint32_t LT_B_LBO = 32 * 16;               // weight image: [chunk][32 tap rows][16 B]
 constexpr uint32_t LT_B_HL = 4 * LT_B_LBO;
 constexpr uint32_t LT_W_BYTES = 2 * LT_B_HL;         // 4 KB
-constexpr int LT_THREADS = 128 + 256 + 32;
+constexpr int LT_THREADS = 128 + 256;              // consumer warpgroup | loaders
 
 struct LogitsTcParams {
   const uint8_t* wimg;   // device, LT_W_BYTES: hi image then lo image
@@ -66,26 +59,17 @@ logits_tc_kernel(const __grid_constant__ LogitsTcParams p, const SrcLoader8<1> l
   uint8_t* a_s = smem + LT_W_BYTES;                        // operand stages, 16 KB each
   float* q_s = reinterpret_cast<float*>(a_s + LT_NSTAGE * LT_STAGE_BYTES);  // [2][27][128]
   uint64_t* bars = reinterpret_cast<uint64_t*>(q_s + 2 * 27 * 128);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * LT_NSTAGE + 2 * LT_NSLOT);
 
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
   const uint32_t bar0 = smem_u32(bars);
   auto full_a = [&](int s) { return bar0 + 8u * s; };
   auto empty_a = [&](int s) { return bar0 + 8u * (LT_NSTAGE + s); };
-  auto full_acc = [&](int s) { return bar0 + 8u * (2 * LT_NSTAGE + s); };
-  auto empty_acc = [&](int s) { return bar0 + 8u * (2 * LT_NSTAGE + LT_NSLOT + s); };
-  constexpr int MMA_WARP = 12;
-  constexpr uint32_t TMEM_COLS = 64;
 
   if (tid == 0) {
     for (int s = 0; s < LT_NSTAGE; ++s) {
       mbar_init(full_a(s), 4);    // one arrival per loader warp of the group
-      mbar_init(empty_a(s), 1);
-    }
-    for (int s = 0; s < LT_NSLOT; ++s) {
-      mbar_init(full_acc(s), 1);
-      mbar_init(empty_acc(s), 4);
+      mbar_init(empty_a(s), 4);   // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -93,16 +77,7 @@ logits_tc_kernel(const __grid_constant__ LogitsTcParams p, const SrcLoader8<1> l
   for (int i = tid; i < (int)(LT_W_BYTES / 16); i += LT_THREADS)
     reinterpret_cast<uint4*>(w_s)[i] = __ldg(reinterpret_cast<const uint4*>(p.wimg) + i);
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  if (warp == MMA_WARP) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(tmem_slot)),
-                 "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
   const long long plane = (long long)p.H * p.W;
 
   auto item_geom = [&](int item, int& x0, int& y0, int& z_lo, int& z_hi) {
@@ -117,7 +92,7 @@ logits_tc_kernel(const __grid_constant__ LogitsTcParams p, const SrcLoader8<1> l
     z_hi = min(p.D, z_lo + LT_ZC);
   };
 
-  if (warp >= 4 && warp < MMA_WARP) {
+  if (warp >= 4) {
     // ============================ loaders ============================
     const int lgrp = (warp - 4) & 1;
     const int lt = ((warp - 4) >> 1) * 32 + lane;   // 0..127 inside the group
@@ -162,67 +137,65 @@ logits_tc_kernel(const __grid_constant__ LogitsTcParams p, const SrcLoader8<1> l
         if (lane == 0) mbar_arrive(full_a(s));
       }
     }
-  } else if (warp == MMA_WARP) {
-    // ============================ MMA issuer ============================
-    const uint32_t w_base = smem_u32(w_s), a_base = smem_u32(a_s);
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-    const uint32_t desc_hi = (128u >> 4) | (1u << 14);   // SBO = 128 B (dense 8-row groups)
-    const uint32_t idesc = idesc_bf16(32);
-    uint32_t stage_ctr = 0, plane_ctr = 0;
-    for (int item = blockIdx.x; item < p.nitems; item += gridDim.x) {
-      int x0, y0, z_lo, z_hi;
-      item_geom(item, x0, y0, z_lo, z_hi);
-      for (int zi = max(z_lo - 1, 0); zi <= min(z_hi, p.D - 1); ++zi, ++stage_ctr, ++plane_ctr) {
-        const int s = stage_ctr % LT_NSTAGE, slot = plane_ctr % LT_NSLOT;
-        mbar_wait(empty_acc(slot), ((plane_ctr / LT_NSLOT) & 1) ^ 1, p.err);
-        mbar_wait(full_a(s), (stage_ctr / LT_NSTAGE) & 1, p.err);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t a_lo = (((a_base + s * LT_STAGE_BYTES) >> 4) & 0x3FFF) |
-                              ((LT_A_LBO >> 4) << 16);
-        const uint32_t b_lo = ((w_base >> 4) & 0x3FFF) | ((LT_B_LBO >> 4) << 16);
-        const uint32_t d0 = tmem_u + slot * 32;
-        if (elect_one()) {
-#pragma unroll
-          for (int ks = 0; ks < 2; ++ks) {
-            const uint64_t ah = pack64(a_lo + 2 * ks * (LT_A_LBO >> 4), desc_hi);
-            const uint64_t al = pack64(a_lo + 2 * ks * (LT_A_LBO >> 4) + (LT_A_HL >> 4), desc_hi);
-            const uint64_t bh = pack64(b_lo + 2 * ks * (LT_B_LBO >> 4), desc_hi);
-            const uint64_t bl = pack64(b_lo + 2 * ks * (LT_B_LBO >> 4) + (LT_B_HL >> 4), desc_hi);
-            umma_bf16(d0, ah, bh, idesc, ks == 0 ? 0u : 1u);   // first MMA overwrites
-            umma_bf16(d0, al, bh, idesc, 1u);
-            umma_bf16(d0, ah, bl, idesc, 1u);
-          }
-          umma_commit(empty_a(s));
-          umma_commit(full_acc(slot));
-        }
-        __syncwarp();
-      }
-    }
   } else {
-    // ============================ epilogue (warps 0-3) ============================
-    const int m = warp * 32 + lane;                  // position == TMEM lane
+    // ============ consumer warpgroup (warps 0-3): MMA issue, then the stencil gather ============
+    // Two m64n32 wgmma chains per plane (positions 0-63 and 64-127); thread m == position in
+    // the gather.
+    const uint32_t w_base = smem_u32(w_s), a_base = smem_u32(a_s);
+    const uint32_t desc_hi = 128u >> 4;   // SBO = 128 B (dense 8-row groups)
+    const int m = tid;                    // position of the gather
     const int bx = m % LT_PX, by = m / LT_PX;
     const bool inner = bx >= 1 && bx <= LT_OX && by >= 1 && by <= LT_OY;
-    uint32_t plane_ctr = 0;
+    float acc[2][16];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < 16; ++i) acc[h][i] = 0.f;
+    uint32_t stage_ctr = 0;
     for (int item = blockIdx.x; item < p.nitems; item += gridDim.x) {
       int x0, y0, z_lo, z_hi;
       item_geom(item, x0, y0, z_lo, z_hi);
       const int ox = x0 + bx - 1, oy = y0 + by - 1;
       const bool olive = inner && ox < p.W && oy < p.H;
       float accA = 0.f, accB = 0.f;                  // output planes zi-1 and zi
-      for (int zi = max(z_lo - 1, 0); zi <= min(z_hi, p.D - 1); ++zi, ++plane_ctr) {
-        const int slot = plane_ctr % LT_NSLOT;
-        float* qb = q_s + (plane_ctr & 1) * (27 * 128);
-        mbar_wait(full_acc(slot), (plane_ctr / LT_NSLOT) & 1, p.err);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        uint32_t r[32];
-        tmem_ld<32>(tmem_base + ((uint32_t)(warp * 32) << 16) + slot * 32, r);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+      for (int zi = max(z_lo - 1, 0); zi <= min(z_hi, p.D - 1); ++zi, ++stage_ctr) {
+        const int s = stage_ctr % LT_NSTAGE;
+        float* qb = q_s + (stage_ctr & 1) * (27 * 128);
+        mbar_wait(full_a(s), (stage_ctr / LT_NSTAGE) & 1, p.err);
         __syncwarp();
-        if (lane == 0) mbar_arrive(empty_acc(slot));
+        const uint32_t a_lo = (((a_base + s * LT_STAGE_BYTES) >> 4) & 0x3FFF) |
+                              ((LT_A_LBO >> 4) << 16);
+        const uint32_t b_lo = ((w_base >> 4) & 0x3FFF) | ((LT_B_LBO >> 4) << 16);
+        wgmma_fence();
 #pragma unroll
-        for (int t = 0; t < 27; ++t) qb[t * 128 + m] = __uint_as_float(r[t]);
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int ks = 0; ks < 2; ++ks) {
+            const uint32_t al0 = a_lo + 64u * h + 2 * ks * (LT_A_LBO >> 4);
+            const uint64_t ah = pack64(al0, desc_hi);
+            const uint64_t al = pack64(al0 + (LT_A_HL >> 4), desc_hi);
+            const uint64_t bh = pack64(b_lo + 2 * ks * (LT_B_LBO >> 4), desc_hi);
+            const uint64_t bl = pack64(b_lo + 2 * ks * (LT_B_LBO >> 4) + (LT_B_HL >> 4), desc_hi);
+            wgmma_bf16<32>(acc[h], ah, bh);
+            wgmma_bf16<32>(acc[h], al, bh);
+            wgmma_bf16<32>(acc[h], ah, bl);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_a(s));
+        // Q of this plane to shared memory: register i holds position 64h + 16*warp + lane/4 +
+        // 8*((i/2)&1), tap 8*(i/4) + 2*(lane%4) + (i&1)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            const int t = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+            const int pos = 64 * h + 16 * warp + (lane >> 2) + 8 * ((i >> 1) & 1);
+            if (t < 27) qb[t * 128 + pos] = acc[h][i];
+            acc[h][i] = 0.f;
+          }
         // all 128 positions of this plane are in shared memory (the other q buffer still
         // belongs to the previous plane's gather, which every thread has left by now)
         asm volatile("bar.sync 1, 128;" ::: "memory");
@@ -247,12 +220,6 @@ logits_tc_kernel(const __grid_constant__ LogitsTcParams p, const SrcLoader8<1> l
         p.out[(long long)(p.D - 1) * plane + (long long)oy * p.W + ox] = accA;
     }
   }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == MMA_WARP)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(TMEM_COLS));
 }
 
 struct LogitsTcWeights {
@@ -286,7 +253,7 @@ inline bool logits_tc_launch(const Src& s, const LogitsTcWeights& w, float* out,
   p.nitems = (int)items;
   p.err = tc_err_flag().get();
   const size_t smem = LT_W_BYTES + LT_NSTAGE * LT_STAGE_BYTES + 2 * 27 * 128 * 4 +
-                      (2 * LT_NSTAGE + 2 * LT_NSLOT) * 8 + 16;
+                      2 * LT_NSTAGE * 8;
   bool& attr_done = per_device<bool, 31>();
   if (!attr_done) {
     if (cudaFuncSetAttribute(logits_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -294,8 +261,8 @@ inline bool logits_tc_launch(const Src& s, const LogitsTcWeights& w, float* out,
       return false;
     attr_done = true;
   }
-  // two CTAs per SM (96 KB of shared memory, 64 TMEM columns each): the loaders are latency
-  // bound, a second CTA fills their stalls
+  // two CTAs per SM (96 KB of shared memory each): the loaders are latency bound, a second
+  // CTA fills their stalls
   const int grid = (int)std::min<long long>(items, 2LL * tc_sm_count());
   logits_tc_kernel<<<grid, LT_THREADS, smem, st>>>(p, SrcLoader8<1>{s, 32, H, W});
   return cudaGetLastError() == cudaSuccess;

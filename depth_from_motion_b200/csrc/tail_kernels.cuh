@@ -1,8 +1,8 @@
 // HBM-bound tail of the KITTI path, second generation (round 2):
 //   * logits_conv_kernel  -- the 32 -> 1 channel 3x3x3 conv of build_depth_pred_module
 //     (dfm_backbone.py:128) as a CUDA-core kernel.  The op reads V*32 floats and writes V
-//     (0.43 GB -> ~0.07 ms at the copy bandwidth); on the tensor-core conv it ran as an N = 96
-//     MMA with 1/32 useful columns (0.58 ms per frame).  Formulation: per INPUT voxel, the 27
+//     (0.43 GB); on the tensor-core conv it would run as an N = 96 MMA with 1/32 useful
+//     columns.  Formulation: per INPUT voxel, the 27
 //     per-tap dot products q_t = <x, w_t> (864 FMAs whose weight operands come from the
 //     constant bank: the weights are a __grid_constant__ kernel parameter and every index is a
 //     compile-time constant), staged in shared memory; per OUTPUT voxel, out(o) = sum_t q_t(o + off_t) is 27 shared-memory reads.
@@ -32,12 +32,7 @@ struct LogitsConvParams {
   int tiles_x, tiles_y, zchunks;
 };
 
-// Variants measured on B200 (profiles/r02_tail_kernels.md): this one (weights from the constant
-// bank, one position at a time) 0.31 + 0.14 ms for the two towers; a persistent grid with
-// software-prefetched positions 0.39 + 0.16; packed fma.rn.f32x2 with shared-memory weights
-// 0.40 + 0.18 (FFMA2 halves the issue slots but not the FMA-pipe cycles, and the weight reads
-// move to the LSU).  ncu: FMA pipe 39 % active, top stalls long-scoreboard (the 128-byte row
-// of a position) and the two barriers per plane.
+// Weights come from the constant bank; one position at a time.
 __global__ void __launch_bounds__(LC_THREADS)
 logits_conv_kernel(const __grid_constant__ LogitsConvParams p, float* __restrict__ out) {
   extern __shared__ float lc_q[];   // [27][LC_NPOS]
@@ -168,11 +163,11 @@ inline bool logits_conv_launch(const Src& s, const float* h_w /*[27][32] host*/,
 
 // ---------------------------------------------------------------------------------
 // DepthHead.forward, four x pixels per thread (requires (Wo * f) % 4 == 0).
-// Structure chosen from the ncu profile of the first version (issue-bound at 120 instructions
-// per 4-pixel depth bin): the two low-res rows a block interpolates between are blended ONCE
+// Structure chosen to cut the instructions per 4-pixel depth bin (the first version was
+// issue-bound): the two low-res rows a block interpolates between are blended ONCE
 // while staging (R[z][c] = ly0*row0 + ly1*row1), the depth loop walks low-res intervals with
 // the carried pair (b0, b1) and an inner loop over the bins of the interval, all per-bin
-// constants come from shared-memory tables.  ~38 instructions per 4-pixel bin and pass.
+// constants come from shared-memory tables.
 // ---------------------------------------------------------------------------------
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;

@@ -15,7 +15,7 @@ of PyTorch ops:
 The ``nn.Conv3d`` / ``nn.GroupNorm`` / ``nn.BatchNorm3d`` children below are
 parameter containers only (they give the exact reference ``state_dict`` layout so
 reference checkpoints load with ``strict=True``); their ``forward`` is never
-called.  There is no PyTorch fallback: without the built library or a B200 the
+called.  There is no PyTorch fallback: without the built library or an H100 the
 modules raise.
 """
 import ctypes

@@ -6,7 +6,7 @@ mmdet's ``BACKBONES`` / ``HEADS``, dfm_backbone.py:11-14, depth_head.py:10-13;
 ``DfMNeck`` / ``OutdoorImVoxelNeck`` into mmdet3d's ``NECKS``, dfm_neck.py:6-10).
 
 When mmcv/mmdet are importable, ``register_into_mmdet()`` registers the
-B200-native classes under the same names with ``force=True`` so an unmodified
+H100-native classes under the same names with ``force=True`` so an unmodified
 ``configs/dfm/*.py`` builds them.  mmcv is not installed in this image, so the
 module also carries a minimal ``Registry`` + ``Config`` with the same call
 shapes (``register_module()``, ``build(cfg)``, ``Config.fromfile``) -- enough to
@@ -123,7 +123,7 @@ class Config:
 
 
 def register_into_mmdet():
-    """Registers the B200-native classes into the real mmdet / mmdet3d registries
+    """Registers the H100-native classes into the real mmdet / mmdet3d registries
     (same names as the reference, ``force=True``).  Returns False when mmcv/mmdet
     are not installed."""
     try:

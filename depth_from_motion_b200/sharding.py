@@ -8,8 +8,8 @@ MAX-reduction of the per-rank step time for reporting.
 Depth-slab sharding of ONE frame (what BASELINE.json's north_star sketches) is not a
 single-exchange partition: every GroupNorm needs a global per-channel sum (18
 all-reduces per frame) and every 3x3x3 conv a one-plane halo at its own resolution
-(22 exchanges); with a ~7 ms single-GPU frame made of ~0.05-0.8 ms kernels those ~40
-latency-bound exchanges cannot pay off.  It is documented in DESIGN.md and left out.
+(22 exchanges); with a single-GPU frame of ~10 ms (H100) made of sub-millisecond kernels those
+~40 latency-bound exchanges cannot pay off.  It is documented in DESIGN.md and left out.
 """
 import torch
 import torch.distributed as dist

@@ -1,5 +1,5 @@
 /*
- * dfm_b200.h -- C ABI of the B200-native DfM plane-sweep cost-volume path.
+ * dfm_b200.h -- C ABI of the H100-native (sm_90a) DfM plane-sweep cost-volume path.
  *
  * The reference (Tai-Wang/Depth-from-Motion @ e2321189) has no FFI: its hot path
  * is a chain of PyTorch calls inside mmcv-registry modules.  This header is the
@@ -29,13 +29,13 @@ extern "C" {
 #define DFM_ERR_INVALID 1 /* bad argument / unsupported shape           */
 #define DFM_ERR_CUDA 2    /* CUDA runtime error (message has the cause)  */
 #define DFM_ERR_STATE 3   /* missing parameter, depths not set, ...      */
-#define DFM_ERR_NOGPU 4   /* no sm_100 device visible                    */
+#define DFM_ERR_NOGPU 4   /* no sm_90 device visible                     */
 
 /* conv implementation selector (dfm_backbone_desc_t.conv_impl, dfm_op_conv3d) */
-#define DFM_CONV_AUTO 0 /* tcgen05 tensor-core kernels where implemented, SIMT else */
+#define DFM_CONV_AUTO 0 /* tensor-core (wgmma) kernels where implemented, SIMT else */
 #define DFM_CONV_SIMT 1 /* fp32 CUDA-core kernels everywhere (bring-up / cross-check) */
-#define DFM_CONV_TC 2   /* tcgen05 only; error if a layer has no tensor-core kernel   */
-#define DFM_CONV_TC_NECK 3 /* dfm_op_conv3d only: force the K-outer tcgen05 kernel of the BEV
+#define DFM_CONV_TC 2   /* wgmma only; error if a layer has no tensor-core kernel     */
+#define DFM_CONV_TC_NECK 3 /* dfm_op_conv3d only: force the K-outer wgmma kernel of the BEV
                               necks (64..256 channels, W <= 16, strides (1,1,1) / (1,1,2))  */
 #define DFM_CONV_TC_NECK_DHW 4 /* dfm_op_conv3d only: force the same kernel in [D][H][W]
                                   orientation, D cut into windows (stride 1, pad 1, Cin >= 64) */
@@ -137,7 +137,7 @@ int dfm_sync_check(void* stream);
  * (NUL-terminated, truncated to cap) and clears the record. */
 int dfm_profile_enable(int on);
 int dfm_profile_report(char* buf, int cap);
-/* Counters since creation: kernels launched by this library / of which tcgen05. */
+/* Counters since creation: kernels launched by this library / of which tensor-core. */
 int dfm_launch_counters(long long* launches, long long* tc_launches);
 
 /* ------------------------------------------------------------------------------------
@@ -385,7 +385,7 @@ int dfm_pipeline_wait(dfm_backbone_t* bb);
 /* dfm_backbone_prefetch_host for the pipeline: also stages the NEXT frame's sem features
  * (`sem_numel` floats, may be NULL / 0) together with its pair on the side stream.  A small
  * host->device copy issued at submit time would queue on the copy engine behind this bulk
- * copy and stall the compute stream (measured: ~1 ms per frame), so everything a frame reads
+ * copy and stall the compute stream, so everything a frame reads
  * from the host should be handed over here, one frame ahead. */
 int dfm_pipeline_prefetch_host(dfm_backbone_t* bb, const float* h_cur, const float* h_prev,
                                const float* h_sem, long long sem_numel);

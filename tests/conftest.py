@@ -7,4 +7,4 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a B200 (run with -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs an H100 (run with -m gpu)')

@@ -1,6 +1,7 @@
 """CPU tests: the oracle restatement against (1) the reference's own golden vectors
 for this path (SURVEY.md section 8c) and (2) fixtures produced by the unmodified
 reference sources (tests/golden/make_golden.py)."""
+import math
 import os
 
 import numpy as np
@@ -9,7 +10,7 @@ import torch
 
 from depth_from_motion_b200 import synthetic as syn
 from oracle import dfm_oracle as O
-from tests.util import GOLDEN, KITTI_CASES, load_kitti_case
+from tests.util import GOLDEN, KITTI_CASES, assert_close, load_kitti_case
 
 
 def test_points_img2cam_kat():
@@ -70,13 +71,14 @@ def test_backbone_matches_reference_fixture(name):
             img_scale_factor=spec[6])
         cost, stereo, mono = O.dfm_backbone_forward(params, cur, prev, metas, cfg)
         _, sm, preds = O.depth_head_forward(cost, O.depth_samples(cfg))
-    # same ATen ops, same order, same machine class: tiny tolerance only for
-    # thread-count dependent summation order
+    # same ATen ops in the same order; CPU kernels of another instruction set round
+    # differently (FMA contraction in grid_sample / conv): up to ~2e-4 absolute on values of a
+    # few units, so the absolute term scales with the tensor (|d| <= 1e-4 |b| + 5e-5 max|b|)
     for got, key in ((vol, 'volume'), (cost, 'cost'), (stereo, 'stereo'),
                      (mono, 'mono'), (preds, 'depth_preds')):
         ref = torch.from_numpy(gold[key])
         assert got.shape == ref.shape, key
-        assert torch.allclose(got, ref, rtol=1e-4, atol=1e-5), key
+        assert_close(got, ref, key, rtol=1e-4, atol_frac=5e-5)
     assert torch.allclose(sm[0, 0, :, ::8, ::8],
                           torch.from_numpy(gold['softmax_slice']), atol=1e-6)
 
@@ -123,8 +125,9 @@ def test_neck_multitile_fixture(name):
     from tests.util import make_neck_mt_case
     gold = np.load(os.path.join(GOLDEN, name + '.npz'))
     rng, x = make_neck_mt_case(name)
-    assert float(x.double().sum()) == float(gold['x_sum'])
-    assert float(x.double().abs().sum()) == float(gold['x_abs'])
+    # (a double sum: its last bit depends on the host's summation kernel)
+    assert math.isclose(float(x.double().sum()), float(gold['x_sum']), rel_tol=1e-14)
+    assert math.isclose(float(x.double().abs().sum()), float(gold['x_abs']), rel_tol=1e-14)
     mod = (modules.DfMNeck(64, 256, num_frames=2) if name == 'neck_dfm_mt'
            else modules.OutdoorImVoxelNeck(64, 256))
     sd = syn.make_neck_params(rng, mod.state_dict())
@@ -156,7 +159,7 @@ def test_frustum_to_voxel_matches_reference_fixture():
                                      c['coordinates_3d'], cfg)
     ref = torch.from_numpy(gold['out'])
     assert out.shape == ref.shape == (1, 32, 2, 20, 24)
-    assert float((out - ref).abs().max()) <= 1e-6
+    assert_close(out, ref, 'frustum', rtol=1e-5, atol_frac=1e-6)
     # the grid of the shipped config (detectors/dfm.py:174-211)
     full = O.frustum_coordinates_3d(dict(point_cloud_range=syn.KITTI_POINT_CLOUD_RANGE,
                                          voxel_size=syn.KITTI_VOXEL_SIZE))
@@ -165,16 +168,8 @@ def test_frustum_to_voxel_matches_reference_fixture():
                                                      (288, 304, 20)))
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference/mmdet3d'), reason='reference tree not mounted')
-@pytest.mark.parametrize('flip,aligned', [(False, True), (True, True), (False, False)])
-def test_voxel_sample_matches_reference_source(flip, aligned):
-    """SURVEY.md row a8 (oracle only): the restatement against the reference function executed
-    verbatim (point_fusion.py:324-410)."""
-    import torch.nn.functional as F
-    from oracle.ref_loader import load_reference, reference_function
-    ns = load_reference()
-    ref = reference_function('mmdet3d/models/fusion_layers/point_fusion.py', 'voxel_sample',
-                             dict(torch=torch, F=F, points_img2cam=ns.points_img2cam))
+def voxel_sample_args(flip):
+    """Inputs of the voxel_sample comparison (also used by tests/golden/make_reference_io.py)."""
     g = torch.Generator().manual_seed(3)
     vox = torch.randn(1, 6, 20, 16, 8, generator=g)
     vrange, vsize = [0.0, -8.0, -2.0, 20.0, 8.0, 2.0], [1.0, 1.0, 0.5]
@@ -183,12 +178,22 @@ def test_voxel_sample_matches_reference_source(flip, aligned):
     k = torch.tensor([[40., 0, 32, 0], [0, 40., 16, 0], [0, 0, 1, 0], [0, 0, 0, 1]])
     l2c = torch.tensor([[0., -1, 0, 0], [0, 0, -1, 0.3], [1, 0, 0, 0.1], [0, 0, 0, 1]])
     proj = k @ l2c
-    args = (vox, vrange, vsize, depths, proj, 4, torch.tensor([1.02, 0.98]),
+    return (vox, vrange, vsize, depths, proj, 4, torch.tensor([1.02, 0.98]),
             torch.tensor([1.0, 2.0]), flip, (32, 64), (30, 62))
-    a = ref(*args, aligned=aligned)
-    b = O.voxel_sample(*args, aligned=aligned)
+
+
+def _reference_io(key):
+    return torch.from_numpy(np.load(os.path.join(GOLDEN, 'reference_io.npz'))[key])
+
+
+@pytest.mark.parametrize('flip,aligned', [(False, True), (True, True), (False, False)])
+def test_voxel_sample_matches_reference_source(flip, aligned):
+    """SURVEY.md row a8 (oracle only): the restatement against the output of the reference
+    function executed verbatim (point_fusion.py:324-410), stored in reference_io.npz."""
+    a = _reference_io(f'voxel_sample_{int(flip)}_{int(aligned)}')
+    b = O.voxel_sample(*voxel_sample_args(flip), aligned=aligned)
     assert a.shape == b.shape == (1, 6, 4, 8, 16)
-    assert torch.equal(a, b)
+    assert_close(b, a, 'voxel_sample', rtol=1e-5, atol_frac=2e-6)   # (stored on another host)
     assert float(a.abs().sum()) > 0
 
 
@@ -197,7 +202,7 @@ def test_bev_stage_matches_reference_fixture():
     (class scores, 3-D box regressions, direction logits) against the verbatim reference run."""
     gold = np.load(os.path.join(GOLDEN, 'bev_stage.npz'))
     c = syn.make_bev_case(**syn.BEV_CASE)
-    assert float(c['volume'].double().sum()) == float(gold['x_sum'])
+    assert math.isclose(float(c['volume'].double().sum()), float(gold['x_sum']), rel_tol=1e-14)
     v = c['volume']
     with torch.no_grad():
         prehg, bev = O.bev_hourglass_forward(c['bev'], v.reshape(1, -1, v.shape[3], v.shape[4]))
@@ -210,42 +215,31 @@ def test_bev_stage_matches_reference_fixture():
     assert outs[0].shape[1] == 18 and outs[1].shape[1] == 42 and outs[2].shape[1] == 12
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference/mmdet3d'), reason='reference tree not mounted')
 def test_bev_stage_oracle_equals_reference_source():
-    """Bit-for-bit against the reference classes executed in place (only where mounted)."""
-    from oracle.ref_loader import load_reference
-    ns = load_reference()
+    """Against the output of the reference classes executed in place (reference_io.npz); the
+    tolerance covers CPU kernels that round differently on another host."""
     c = syn.make_bev_case(seed=5, nz=5, ny=12, nx=16)
-    gn = dict(type='GN', num_groups=32, requires_grad=True)
-    bev = ns.BEVHourglass(160, 64, norm_cfg=gn).eval()
-    head = ns.LIGAAnchor3DHead(3, 64, 64, 6, norm_cfg=gn).eval()
-    bev.load_state_dict(c['bev'], strict=True)
-    head.load_state_dict(c['head'], strict=True)
-    x = c['volume'].reshape(1, 160, 12, 16)
     with torch.no_grad():
-        _, feat = bev(x)
-        ref = head.forward_single(feat)
         got = O.dfm_bev_stage(c['bev'], c['head'], c['volume'])
-    for a, b in zip(got, ref):
-        assert torch.equal(a, b)
+    assert len(got) == 3
+    for i, a in enumerate(got):
+        ref = _reference_io(f'bev_small_{i}')
+        assert_close(a, ref, f'bev output {i}', rtol=1e-5, atol_frac=2e-6)
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference/mmdet3d'), reason='reference tree not mounted')
 def test_spp_unet_lastconv_equals_reference_module():
     """SURVEY.md section 8(f) row 2: the oracle restatement of SPPUNetNeck.lastconv against the
-    reference class executed in place (spp_unet_neck.py:60-75, :110)."""
-    from oracle.ref_loader import load_reference
-    ns = load_reference()
-    gn = dict(type='GN', num_groups=32, requires_grad=True)
-    m = ns.SPPUNetNeck(in_channels=[3, 64, 128, 128, 128], start_level=2, sem_channels=[128, 32],
-                       stereo_channels=[32, 32], with_upconv=True, cat_img_feature=True,
-                       norm_cfg=gn).eval()
-    p = {k: v for k, v in m.state_dict().items() if k.startswith('lastconv')}
+    reference class executed in place (spp_unet_neck.py:60-75, :110), stored with its randomly
+    initialised parameters in reference_io.npz."""
+    gold = np.load(os.path.join(GOLDEN, 'reference_io.npz'))
+    p = {k.split(':', 1)[1]: torch.from_numpy(gold[k]) for k in gold.files
+         if k.startswith('lastconv_param:')}
     assert sorted(p) == ['lastconv.0.conv.weight', 'lastconv.0.gn.bias', 'lastconv.0.gn.weight',
                          'lastconv.1.weight']
     x = torch.randn(1, 32, 24, 40, generator=torch.Generator().manual_seed(4))
     with torch.no_grad():
-        assert torch.equal(m.lastconv(x), O.spp_unet_lastconv(p, x))
+        assert_close(O.spp_unet_lastconv(p, x), torch.from_numpy(gold['lastconv_out']), 'lastconv',
+                     rtol=1e-5, atol_frac=2e-6)
     # the mirror takes the same keys
     from depth_from_motion_b200 import modules
     modules.SPPUNetNeckTail().load_state_dict(p, strict=True)

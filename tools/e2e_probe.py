@@ -1,6 +1,6 @@
 """Where does the end-to-end (host buffers in / out) step spend its time?
 
-Runs the DfM.simple_test hot-path segment (HotPathPipeline) on a B200 in four ways and prints
+Runs the DfM.simple_test hot-path segment (HotPathPipeline) on an H100 in four ways and prints
 one JSON line: (a) per-kernel profile of one synchronous frame, (b) asynchronous loop with all
 copies (what bench.py reports as e2e), (c) the same loop fed the SAME already-staged pair (no
 H2D of the pair), (d) the same without collecting outputs on the host path differences.

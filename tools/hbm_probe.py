@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Write-only / read-only / copy bandwidth of this GPU (context for the HBM-bound kernels'
-roofline fractions: MEASURED_PEAKS.json holds the copy figure only).  Run on a B200."""
+roofline fractions: MEASURED_PEAKS.json holds the copy figure only).  Run on an H100."""
 import json
 
 import torch

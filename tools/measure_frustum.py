@@ -3,7 +3,7 @@
 (configs/dfm/dfm_r34_1x8_kitti-3d-3class.py: stereo_feat [32,112,96,312], softmax
 [448,384,1248], voxels 20x304x288) with the materialised softmax volume (the reference's
 argument) and with the fused logits path, plus the per-kernel split.  Prints one JSON line;
-run on a B200."""
+run on an H100."""
 import json
 import os
 import sys

@@ -2,7 +2,7 @@
 """Times the Waymo-side rows (SURVEY.md 8a: a6 lifting, a7 necks) at the shipped sizes
 (configs/dfm/multiview-dfm_r101_dcn_2x16_waymoD5-3d-3class_camsync[_10sweeps].py):
 T*Nv x [64, 208, 312] features -> [64(*T), 220, 300, 12] voxels -> BEV [256, 300, 220].
-Prints one JSON line; run on a B200."""
+Prints one JSON line; run on an H100."""
 import json
 import os
 import sys
@@ -59,7 +59,7 @@ def main():
         x = torch.from_numpy(rng.standard_normal((1, cin, 220, 300, 12)).astype(np.float32)).cuda()
         ms = timeit(lambda: mod(x), n=1)
         flops = 3.212e12 if cin == 64 else 7.649e12
-        out[name] = dict(ms=round(ms, 1), tflops=round(flops / ms / 1e9, 2), impl='tcgen05 K-outer conv (conv_tc_neck.cuh)')
+        out[name] = dict(ms=round(ms, 1), tflops=round(flops / ms / 1e9, 2), impl='wgmma K-outer conv (conv_tc_neck.cuh)')
     print(json.dumps(out))
 
 
