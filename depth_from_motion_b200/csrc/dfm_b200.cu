@@ -330,7 +330,9 @@ int run_conv_impl(const L& simt_loader, TCFN tc_fn, const char* loader_name, con
     std::string err;
     if (gn) DFM_TRY(gn->begin_stats(st));
     {
-      ProfScope ps(conv_class("conv_tc", g, loader_name), conv_flops(g), st);
+      // K-sliced launches carry their own tag: they also run the slice-reduce kernel
+      ProfScope ps(conv_class(w.tc.kslice ? "conv_tc_ks" : "conv_tc", g, loader_name),
+                   conv_flops(g), st);
       if (!tc_fn(gn ? gn->sums : nullptr, &err)) return fail(DFM_ERR_CUDA, err);
     }
     g_launches.fetch_add(w.tc.kslice ? 2 : 1);  // K-slice convs run a slice-reduce kernel too
@@ -395,7 +397,7 @@ int run_conv_presplit(const dfm::Src& s, DevBuf& ps, const ConvW& w, float* out,
   if (gn) DFM_TRY(gn->begin_stats(st));
   {
     std::string err;
-    ProfScope pc(conv_class("conv_tc", g, "tma"), conv_flops(g), st);
+    ProfScope pc(conv_class(w.tc.kslice ? "conv_tc_ks" : "conv_tc", g, "tma"), conv_flops(g), st);
     dfm::TcOpts o;
     o.zw_lo = zw.lo;
     o.zw_hi = zw.hi;
@@ -539,6 +541,9 @@ struct Tower {
   Norm g0, g1, gc1, gc2, gc3, gc4, gc5, gc6, gp0;
   DevBuf raw0, raw1, b1, b2, b3, b4, b5, b6, cur, p0b, logit;
   DevBuf ps0, ps2;  // pre-split (bf16 hi / lo) inputs of the two stride-2 convs, read by TMA
+  // what the last forward wrote (dfm_backbone_debug_tensor refuses the rest): the z-class
+  // path keeps dres0_mono's output in cls3 only, and only that path writes cls3
+  bool raw0_written = false, cls3_written = false;
 };
 
 struct dfm_backbone {
@@ -565,7 +570,11 @@ struct dfm_backbone {
   std::vector<float> pipe_samples_host;  // what pipe_samples holds (re-uploaded on change only)
   bool depths_set = false;
   std::set<std::string> missing;
-  std::map<std::string, std::pair<const DevBuf*, int>> dbg;  // name -> (buffer, channels)
+  struct DebugTensor {
+    const DevBuf* buf;
+    const bool* written;  // null: every forward writes it
+  };
+  std::map<std::string, DebugTensor> dbg;
 };
 
 namespace {
@@ -750,6 +759,8 @@ int tower_forward(dfm_backbone* bb, Tower& t, bool mono, const dfm::WarpLoader& 
                        getenv("DFM_NO_ZSHORTEN") == nullptr;
   const int D = shorten ? 2 * kZHead + kZMid : Dfull;  // planes actually computed
   const long long V = (long long)D * Ho * Wo;           // computed voxels
+  t.raw0_written = !(zinv && mono);
+  t.cls3_written = zinv;
   dfm::ZExpand ze{Dfull, Dfull, 0, 0};                  // identity
   if (shorten) ze = dfm::ZExpand{kZHead, Dfull - kZHead, Dfull - D, kZHead};
   if (zexp_out) *zexp_out = ze;
@@ -1021,16 +1032,18 @@ int dfm_backbone_create(const dfm_backbone_desc_t* desc, dfm_backbone_t** out) {
   for (int m = 0; m < 2; ++m) {
     Tower& t = m ? bb->mo : bb->st;
     const std::string s = m ? "_mono" : "";
-    bb->dbg["raw0" + s] = {&t.raw0, 32};
-    bb->dbg["raw1" + s] = {&t.raw1, 32};
-    bb->dbg["c1" + s] = {&t.b1, 64};
-    bb->dbg["c2" + s] = {&t.b2, 64};
-    bb->dbg["c3" + s] = {&t.b3, 64};
-    bb->dbg["c4" + s] = {&t.b4, 64};
-    bb->dbg["c5" + s] = {&t.b5, 64};
-    bb->dbg["c6" + s] = {&t.b6, 32};
-    bb->dbg["p0" + s] = {&t.p0b, 32};
-    bb->dbg["logit" + s] = {&t.logit, 1};
+    bb->dbg["raw0" + s] = {&t.raw0, &t.raw0_written};
+    bb->dbg["cls3" + s] = {&t.cls3, &t.cls3_written};
+    bb->dbg["raw1" + s] = {&t.raw1, nullptr};
+    bb->dbg["c1" + s] = {&t.b1, nullptr};
+    bb->dbg["c2" + s] = {&t.b2, nullptr};
+    bb->dbg["c3" + s] = {&t.b3, nullptr};
+    bb->dbg["c4" + s] = {&t.b4, nullptr};
+    bb->dbg["c5" + s] = {&t.b5, nullptr};
+    bb->dbg["c6" + s] = {&t.b6, nullptr};
+    bb->dbg["cur" + s] = {&t.cur, nullptr};
+    bb->dbg["p0" + s] = {&t.p0b, nullptr};
+    bb->dbg["logit" + s] = {&t.logit, nullptr};
   }
   *out = bb;
   return DFM_OK;
@@ -1168,7 +1181,7 @@ int backbone_forward_impl(dfm_backbone_t* bb, const float* d_cur, const float* d
     const int sms = dfm::tc_sm_count();
     const int rounds = (ntiles + sms - 1) / sms;
     const int grid = (ntiles + rounds - 1) / rounds;
-    ProfScope ps("gate", 0.0, st);
+    ProfScope ps("gate_tile4", 0.0, st);
     dfm::gate_tile4_kernel<<<grid, 32 * ng, gsm4, st>>>(bb->st.logit.p, bb->mo.logit.p,
                                                        bb->waggT.p, bb->cost.p, bb->D, HWo,
                                                        ze_mono);
@@ -1185,7 +1198,7 @@ int backbone_forward_impl(dfm_backbone_t* bb, const float* d_cur, const float* d
     const int ng = (bb->D + dfm::GT_PG - 1) / dfm::GT_PG;
     const int nh = dfm::gate_halves(bb->D);
     const int grid = std::min((HWo + 32 * nh - 1) / (32 * nh), dfm::tc_sm_count());
-    ProfScope ps("gate", 0.0, st);
+    ProfScope ps("gate_persistent", 0.0, st);
     dfm::gate_persistent_kernel<<<grid, 32 * ng * nh, gsm, st>>>(bb->st.logit.p, bb->mo.logit.p,
                                                             bb->waggT.p, bb->cost.p, bb->D, HWo,
                                                             ze_mono);
@@ -1194,7 +1207,7 @@ int backbone_forward_impl(dfm_backbone_t* bb, const float* d_cur, const float* d
     if (smem > 48 * 1024)
       CU_TRY(cudaFuncSetAttribute(dfm::gate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   (int)smem));
-    ProfScope ps("gate", 0.0, st);
+    ProfScope ps("gate_v1", 0.0, st);
     dfm::gate_kernel<<<(HWo + 31) / 32, 128, smem, st>>>(bb->st.logit.p, bb->mo.logit.p,
                                                          bb->wagg.p, bb->cost.p, bb->D, HWo, ze_mono);
   }
@@ -1409,7 +1422,9 @@ int dfm_backbone_debug_tensor(dfm_backbone_t* bb, const char* name, float* d_out
   if (!bb || !name || !d_out) return fail(DFM_ERR_INVALID, "null argument");
   auto it = bb->dbg.find(name);
   if (it == bb->dbg.end()) return fail(DFM_ERR_INVALID, std::string("unknown tensor ") + name);
-  const DevBuf* b = it->second.first;
+  const DevBuf* b = it->second.buf;
+  if (it->second.written && !*it->second.written)
+    return fail(DFM_ERR_STATE, std::string(name) + " was not written by the last forward");
   if ((size_t)numel > b->n) return fail(DFM_ERR_INVALID, "numel larger than the tensor");
   CU_TRY(cudaMemcpyAsync(d_out, b->p, numel * sizeof(float), cudaMemcpyDeviceToDevice,
                          (cudaStream_t)stream));

@@ -124,8 +124,12 @@ const float* dfm_backbone_cost_device(const dfm_backbone_t* bb);
  * the next one): hand it to dfm_frustum_forward with DFM_LAYOUT_DHWC to skip a transpose. */
 const float* dfm_backbone_stereo_feat_device(const dfm_backbone_t* bb);
 /* Test hook: copies a named intermediate (channels-last [D][H][W][C]) to d_out.
- * Names: "raw0", "raw1", "c1".."c6", "p0", "logit", with suffix "_mono" for the mono tower
- * (which may hold the z-shortened volume, see DESIGN.md). */
+ * Names: "raw0", "raw1", "c1".."c6", "p0", "logit", "cur" (cur_cost = cost0 + gn6(c6), the
+ * input of the pred conv) and "cls3" (the cur-frame half's dres0 response on the first /
+ * interior / last plane: [3][H][W][C]), with suffix "_mono" for the mono tower (which may
+ * hold the z-shortened volume, see DESIGN.md).  Only the z-class first layer writes "cls3";
+ * on that path the mono tower keeps dres0's output in "cls3_mono" and never writes
+ * "raw0_mono".  A tensor the last forward did not write fails with DFM_ERR_STATE. */
 int dfm_backbone_debug_tensor(dfm_backbone_t* bb, const char* name, float* d_out,
                               long long numel, void* stream);
 /* Synchronises `stream` and reports asynchronous failures of this library's kernels
