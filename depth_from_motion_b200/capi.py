@@ -42,6 +42,8 @@ SYMBOLS = (
     'dfm_anchor_head_missing_params', 'dfm_anchor_head_forward', 'dfm_voxel_sample',
     'dfm_backbone_forward_cl', 'dfm_stereo_tail_create', 'dfm_stereo_tail_destroy',
     'dfm_stereo_tail_set_param', 'dfm_stereo_tail_missing_params', 'dfm_stereo_tail_forward',
+    'dfm_neck_debug_tensor', 'dfm_frustum_debug_tensor', 'dfm_bev_hourglass_debug_tensor',
+    'dfm_anchor_head_debug_tensor',
 )
 
 
@@ -201,6 +203,8 @@ def lib():
     L.dfm_stereo_tail_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
     L.dfm_stereo_tail_missing_params.argtypes = [vp]
     L.dfm_stereo_tail_forward.argtypes = [vp, vp, vp, vp, vp]
+    for f in ('neck', 'frustum', 'bev_hourglass', 'anchor_head'):
+        getattr(L, f'dfm_{f}_debug_tensor').argtypes = [vp, c_char_p, vp, c_longlong, vp]
     L.dfm_voxel_sample.argtypes = [POINTER(VoxelSampleDesc), vp, vp, POINTER(c_double), vp, vp]
     _lib = L
     return L

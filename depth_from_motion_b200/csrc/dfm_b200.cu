@@ -94,8 +94,17 @@ double conv_flops(const dfm::ConvGeom& g) {
 }
 std::string conv_class(const char* kind, const dfm::ConvGeom& g, const char* loader) {
   return std::string(kind) + "<" + std::to_string(g.Cin) + "->" + std::to_string(g.Cout) +
-         (g.transposed ? ",T" : g.sd == 2 ? ",s2" : ",s1") + "," + loader + ">@" +
+         (g.transposed ? ",T" : (g.sd == 2 || g.sh == 2 || g.sw == 2) ? ",s2" : ",s1") + "," +
+         loader + ">@" +
          std::to_string(g.Do) + "x" + std::to_string(g.Ho) + "x" + std::to_string(g.Wo);
+}
+// launches of the BEV-neck kernel (conv_tc_neck.cuh) also name the short-axis mode (s1, z2 =
+// stride (1,1,2), p0 = pad (1,1,0)) and the weight-group shape (g32 / g16 input channels)
+std::string neck_class(const char* kind, const dfm::ConvGeom& g, const dfm::NeckTcWeights& w) {
+  const char* zm = w.zmode == dfm::NKZ_S2P1 ? "z2" : w.zmode == dfm::NKZ_S1P0 ? "p0" : "s1";
+  return std::string(kind) + "<" + std::to_string(g.Cin) + "->" + std::to_string(g.Cout) + "," +
+         zm + ",g" + std::to_string(w.cg) + ",src>@" + std::to_string(g.Do) + "x" +
+         std::to_string(g.Ho) + "x" + std::to_string(g.Wo);
 }
 
 struct DevBuf {
@@ -116,6 +125,20 @@ struct DevBuf {
     n = 0;
   }
 };
+
+// Test hooks of the downstream handles (dfm_neck_debug_tensor, ...): copies the `written`
+// floats the last forward left in `b`.  written == 0: that forward did not write the tensor.
+int debug_copy(const DevBuf& b, long long written, const std::string& name, float* d_out,
+               long long numel, void* stream) {
+  if (written <= 0 || !b.p)
+    return fail(DFM_ERR_STATE, name + " was not written by the last forward");
+  if (numel != written)
+    return fail(DFM_ERR_INVALID, name + ": the last forward wrote " + std::to_string(written) +
+                                     " elements, not " + std::to_string(numel));
+  CU_TRY(cudaMemcpyAsync(d_out, b.p, numel * sizeof(float), cudaMemcpyDeviceToDevice,
+                         (cudaStream_t)stream));
+  return DFM_OK;
+}
 
 struct Norm {  // GroupNorm (statistics computed per frame) or folded BatchNorm (static)
   int C = 0;

@@ -340,11 +340,18 @@ class DfMBackbone(_CudaMirror):
 
     def debug_tensor(self, name, shape):
         """Channels-last copy of an intermediate (tests only)."""
-        out = torch.empty(shape, device='cuda', dtype=torch.float32)
-        capi.check(capi.lib().dfm_backbone_debug_tensor(
-            self._handle, name.encode(), _ptr(out), out.numel(), _stream()),
-            'dfm_backbone_debug_tensor')
-        return out
+        return _debug_tensor(self._handle, 'dfm_backbone_debug_tensor', name, shape)
+
+
+def _debug_tensor(handle, fn, name, shape):
+    """Channels-last copy of the intermediate `name` the handle's last forward wrote, through
+    the test hook `fn` of include/dfm_b200.h (shape must hold exactly that tensor)."""
+    if handle is None:
+        raise RuntimeError(f'{fn}: no forward has run')
+    out = torch.empty(shape, device='cuda', dtype=torch.float32)
+    capi.check(getattr(capi.lib(), fn)(handle, name.encode(), _ptr(out), out.numel(), _stream()),
+               f'{fn}({name})')
+    return out
 
 
 def build_dfm_cost(cur_feats, prev_feats, depths, feat_sample_factor,
@@ -511,6 +518,11 @@ class _NeckBase(_CudaMirror):
             outs.append(bev)
         return [torch.stack(outs)]
 
+    def debug_tensor(self, name, shape):
+        """Raw output of conv layer i of a tower, [Nx, Ny, Zo, C] ('mono.<i>' / 'stereo.<i>';
+        OutdoorImVoxelNeck's one tower is 'mono'), from the last forward (tests only)."""
+        return _debug_tensor(getattr(self, '_handle', None), 'dfm_neck_debug_tensor', name, shape)
+
     def release(self):
         if getattr(self, '_handle', None) is not None:
             capi.lib().dfm_neck_destroy(self._handle)
@@ -626,6 +638,11 @@ class FrustumToVoxel(_CudaMirror):
 
     def init_weights(self):
         pass
+
+    def debug_tensor(self, name, shape):
+        """'vox' ([nz, ny, nx, cv], the gathered conv input) or 'conv<i>' (raw output of
+        voxel_convs[i], [nz, ny, nx, 32]) of the last forward (tests only)."""
+        return _debug_tensor(self._handle, 'dfm_frustum_debug_tensor', name, shape)
 
     def release(self):
         if getattr(self, '_handle', None) is not None:
@@ -991,6 +1008,10 @@ class BEVHourglass(_HandleMirror):
                 _ptr(out[i]), _stream()), 'dfm_bev_hourglass_forward')
         return (pre, out) if self.output_prehg_feat else out   # bev_hourglass.py:46-50
 
+    def debug_tensor(self, name, shape):
+        """Raw output [H, W, C] of 'compress' or 'conv1' .. 'conv6' (tests only)."""
+        return _debug_tensor(self._handle, 'dfm_bev_hourglass_debug_tensor', name, shape)
+
 
 @HEADS.register_module()
 class LIGAAnchor3DHead(_HandleMirror):
@@ -1074,6 +1095,11 @@ class LIGAAnchor3DHead(_HandleMirror):
                 _ptr(dirc[i]) if dirc is not None else None, _stream()),
                 'dfm_anchor_head_forward')
         return cls, box, dirc
+
+    def debug_tensor(self, name, shape):
+        """Raw output [ny, nx, C] of 'cls<i>' / 'reg<i>' or of the output convs 'cls_out'
+        (cls + dir channels) / 'reg_out', at their widths padded to 32 (tests only)."""
+        return _debug_tensor(self._handle, 'dfm_anchor_head_debug_tensor', name, shape)
 
 
 def aligned_voxel_centers(n_voxels, voxel_range):

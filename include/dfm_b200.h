@@ -235,6 +235,13 @@ int dfm_neck_missing_params(const dfm_neck_t* neck);
 int dfm_neck_forward(dfm_neck_t* neck, const float* d_x, float* d_bev, void* stream);
 /* d_x_cl: channels-last [Nx][Ny][Nz][C*T] (dfm_multiview_lift_cl's output) */
 int dfm_neck_forward_cl(dfm_neck_t* neck, const float* d_x_cl, float* d_bev, void* stream);
+/* Test hook: copies the raw (pre-BatchNorm) output of conv layer i of a tower, channels-last
+ * [Nx][Ny][Zo][C], to d_out.  Names "mono.0" .. "mono.8" and "stereo.0" .. "stereo.8" (layer
+ * order: res0.conv0, res0.conv1, down1, res2.conv0, res2.conv1, down3, res4.conv0, res4.conv1,
+ * out5); OutdoorImVoxelNeck has only the "mono" tower.  A tensor the last forward did not write
+ * fails with DFM_ERR_STATE, a numel other than the tensor's with DFM_ERR_INVALID. */
+int dfm_neck_debug_tensor(dfm_neck_t* neck, const char* name, float* d_out, long long numel,
+                          void* stream);
 
 /* ------------------------------------------------------------------------------------
  * FrustumToVoxel (mmdet3d/models/necks/feature_transformation.py:12-173), the stage that
@@ -284,6 +291,12 @@ int dfm_frustum_forward(dfm_frustum_t* f, const float* d_stereo_feat, int stereo
                         const float* d_depth_samples, float* d_depth_preds, const float* d_sem,
                         const double* cam2img, int pad_h, int pad_w, float* d_out,
                         void* stream);
+/* Test hook: copies "vox" (the gathered conv input, channels-last [nz][ny][nx][cv]) or "conv<i>"
+ * (the raw output of voxel_convs[i], [nz][ny][nx][32]) to d_out.  The raw outputs share two
+ * buffers, so "conv<i>" is gone once conv i + 2 ran: asking for it, or for a conv beyond
+ * num_3dconvs, fails with DFM_ERR_STATE; a numel other than the tensor's with DFM_ERR_INVALID. */
+int dfm_frustum_debug_tensor(dfm_frustum_t* f, const char* name, float* d_out, long long numel,
+                             void* stream);
 
 /* ------------------------------------------------------------------------------------
  * The hot-path segment of DfM.simple_test as one call with HOST buffers
@@ -329,6 +342,10 @@ int dfm_bev_hourglass_missing_params(const dfm_bev_hourglass_t* b);
  * [out][ny][nx] (spatial_features_2d_prehg, spatial_features_2d). */
 int dfm_bev_hourglass_forward(dfm_bev_hourglass_t* b, const float* d_x, float* d_prehg,
                               float* d_out, void* stream);
+/* Test hook: the raw output of "compress" or "conv1" .. "conv6", channels-last [H][W][C], as
+ * the last forward wrote it (DFM_ERR_STATE otherwise; DFM_ERR_INVALID for a wrong numel). */
+int dfm_bev_hourglass_debug_tensor(dfm_bev_hourglass_t* b, const char* name, float* d_out,
+                                   long long numel, void* stream);
 
 typedef struct dfm_anchor_head dfm_anchor_head_t;
 typedef struct dfm_anchor_head_desc {
@@ -352,6 +369,12 @@ int dfm_anchor_head_missing_params(const dfm_anchor_head_t* h);
  * [dir_channels][ny][nx]. */
 int dfm_anchor_head_forward(dfm_anchor_head_t* h, const float* d_x, float* d_cls, float* d_bbox,
                             float* d_dir, void* stream);
+/* Test hook: the raw output, channels-last [ny][nx][C], of "cls<i>" / "reg<i>" (i < num_convs)
+ * or of the output convs "cls_out" (conv_cls + conv_dir_cls, C = cls + dir channels padded to
+ * a multiple of 32) and "reg_out" (C = reg channels padded likewise), without bias.  A tensor
+ * the last forward did not write fails with DFM_ERR_STATE, a wrong numel with DFM_ERR_INVALID. */
+int dfm_anchor_head_debug_tensor(dfm_anchor_head_t* h, const char* name, float* d_out,
+                                 long long numel, void* stream);
 
 /* ------------------------------------------------------------------------------------
  * voxel_sample (mmdet3d/models/fusion_layers/point_fusion.py:324-410): frustum-from-voxel

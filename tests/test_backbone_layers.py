@@ -21,6 +21,7 @@ split ``x_hi w_hi + x_lo w_hi + x_hi w_lo`` (bf16 operand pairs) commits in exac
 error is below ``max(K_E3 * e3, fp32 accumulation floor)``, and that bound must stay at least
 ``SEPARATION`` times below ``e2``, so no bound can admit a lost term.  The CPU test
 ``test_bounds_separate_lost_term`` checks that separation on oracle inputs without a GPU.
+The reference convs, the emulation and the bounds live in ``tests/layer_check.py``.
 
 The shortened mono tower (D >= 48) computes 16 head, 8 interior and 16 tail planes at full
 resolution (20 / 10 at the lower levels).  Its inputs are expanded to full depth with the phase
@@ -30,7 +31,6 @@ and the computed planes are compared with the matching full planes; this checks 
 statistics sums of the epilogues directly.
 """
 import copy
-import math
 import os
 import subprocess
 import sys
@@ -41,22 +41,8 @@ import torch
 import torch.nn.functional as F
 
 from oracle import dfm_oracle as O
-
-# 3-term error -> bound, and the margin the bound must keep below a lost term.  K_E3 was chosen
-# from the measured H100 errors (DESIGN.md section 1, per-layer table).
-K_E3 = 6.0
-SEPARATION = 3.0
-U32 = 2.0 ** -24       # fp32 unit roundoff
-FLOOR_C = 4.0          # fp32 accumulation floor: FLOOR_C * sqrt(K) * u
-
-
-def acc_floor(k):
-    return FLOOR_C * math.sqrt(k) * U32
-
-
-def layer_bound(e3, k):
-    return max(K_E3 * e3, acc_floor(k))
-
+from tests import layer_check as LC
+from tests.layer_check import SEPARATION, elementwise_errors, layer_bound
 
 # ---------------------------------------------------------------------------------------------
 # shapes (D, Ho = h/4 and Wo = w/4 are multiples of 4)
@@ -111,66 +97,31 @@ def _gn(x, p, prefix):
     return F.group_norm(x, 32, p[prefix + '.weight'], p[prefix + '.bias'], O.GN_EPS)
 
 
+def geom(mode, z0, z1):
+    """Geometry (tests/layer_check.py) of output planes [z0, z1) of conv3d(k3, p1, stride 1 | 2)
+    ('s1' | 's2') or conv_transpose3d(k3, s2, p1, op1) ('t').  z0 must be even for 't'."""
+    return dict(stride=2 if mode == 's2' else 1, transposed=mode == 't',
+                region=((z0, z1), None, None))
+
+
 def conv_planes(x, w, mode, z0, z1):
-    """Output planes [z0, z1) of conv3d(k3, p1, stride 1 | 2) ('s1' | 's2') or
-    conv_transpose3d(k3, s2, p1, op1) ('t') of the full-depth input x, from x's planes
-    [z0, z1) plus halo.  z0 must be even for 't'."""
-    if mode == 't':
-        i0, i1 = z0 // 2, min(z1 // 2 + 1, x.shape[2])
-        return F.conv_transpose3d(x[:, :, i0:i1], w, None, 2, 1, 1)[:, :, :z1 - z0]
-    s = 2 if mode == 's2' else 1
-    xp = F.pad(x, (0, 0, 0, 0, 1, 1))
-    return F.conv3d(xp[:, :, s * z0:s * (z1 - 1) + 3], w, None, s, (0, 1, 1))
-
-
-def split16(x):
-    """The bf16 (hi, lo) pair the kernels keep of an fp32 operand."""
-    x = x.float()
-    hi = O.bf16_round(x)
-    return hi.double(), O.bf16_round(x - hi).double()
+    return LC.conv_planes(x, w, **geom(mode, z0, z1))
 
 
 def emulated_outputs(x, w, mode, z0, z1):
-    """Planes [z0, z1) of the 3-term split x_hi w_hi + x_lo w_hi + x_hi w_lo and of its two
-    2-term variants (x_lo term dropped, w_lo term dropped), in exact (fp64) accumulation."""
-    xh, xl = split16(x)
-    wh, wl = split16(w)
-    a = conv_planes(xh, wh, mode, z0, z1)
-    b = conv_planes(xl, wh, mode, z0, z1)
-    c = conv_planes(xh, wl, mode, z0, z1)
-    return a + b + c, a + c, a + b
+    return LC.emulated_outputs(x, w, **geom(mode, z0, z1))
 
 
 def emulate(x, w, mode, z0, z1, ref):
-    """(e3, e2): normalised max-norm error of the 3-term split and of the better 2-term
-    variant against ref = the layer's planes [z0, z1)."""
-    y3, y2x, y2w = emulated_outputs(x, w, mode, z0, z1)
-    s = float(ref.abs().max())
-    e3 = float((y3 - ref).abs().max()) / s
-    e2 = min(float((y2x - ref).abs().max()), float((y2w - ref).abs().max())) / s
-    return e3, e2
+    return LC.emulate(x, w, ref, **geom(mode, z0, z1))
 
 
 def product_scale(x, w, mode, z0, z1):
-    """sum |x| |w| over each output's products: the scale of that output's rounding error,
-    which stays meaningful where the output itself is small (z ends, zero-padded halo)."""
-    return conv_planes(x.abs(), w.abs(), mode, z0, z1)
-
-
-def elementwise_errors(got, ref, y3, y2x, y2w, scale, k):
-    """Element-wise form of the layer bound: the worst |a - ref| / scale over the elements
-    given, for the GPU (a = got), the 3-term split and the better 2-term variant, and the bound
-    max(K_E3 * e3, floor) that the GPU ratio must meet.  Returns (gpu, e3, e2, bound)."""
-    s = scale.clamp_min(1e-12 * float(scale.max()))
-
-    def worst(a):
-        return float(((a - ref).abs() / s).max())
-    e3 = worst(y3)
-    return worst(got), e3, min(worst(y2x), worst(y2w)), layer_bound(e3, k)
+    return LC.product_scale(x, w, **geom(mode, z0, z1))
 
 
 def k_of(cin, mode):
-    return cin * (8 if mode == 't' else 27)
+    return LC.k_of(cin, mode == 't')
 
 
 def tower_layers(vol, p, mono, fetch):
