@@ -44,6 +44,8 @@ SYMBOLS = (
     'dfm_stereo_tail_set_param', 'dfm_stereo_tail_missing_params', 'dfm_stereo_tail_forward',
     'dfm_neck_debug_tensor', 'dfm_frustum_debug_tensor', 'dfm_bev_hourglass_debug_tensor',
     'dfm_anchor_head_debug_tensor',
+    'dfm_anchor3d_head_create', 'dfm_anchor3d_head_destroy', 'dfm_anchor3d_head_set_param',
+    'dfm_anchor3d_head_missing_params', 'dfm_anchor3d_head_forward',
 )
 
 
@@ -101,6 +103,13 @@ class AnchorHeadDesc(ctypes.Structure):
     _fields_ = [(n, c_int) for n in
                 ('in_channels', 'feat_channels', 'num_convs', 'cls_channels', 'reg_channels',
                  'dir_channels', 'ny', 'nx', 'conv_impl')]
+
+
+class Anchor3DHeadDesc(ctypes.Structure):
+    """``dfm_anchor3d_head_desc_t``."""
+    _fields_ = [(n, c_int) for n in
+                ('feat_channels', 'cls_channels', 'reg_channels', 'dir_channels', 'ny', 'nx',
+                 'conv_impl')]
 
 
 class VoxelSampleDesc(ctypes.Structure):
@@ -197,6 +206,11 @@ def lib():
     L.dfm_anchor_head_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
     L.dfm_anchor_head_missing_params.argtypes = [vp]
     L.dfm_anchor_head_forward.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.dfm_anchor3d_head_create.argtypes = [POINTER(Anchor3DHeadDesc), POINTER(vp)]
+    L.dfm_anchor3d_head_destroy.argtypes = [vp]
+    L.dfm_anchor3d_head_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
+    L.dfm_anchor3d_head_missing_params.argtypes = [vp]
+    L.dfm_anchor3d_head_forward.argtypes = [vp, vp, vp, vp, vp, vp]
     L.dfm_backbone_forward_cl.argtypes = [vp, vp, vp, POINTER(Geometry), vp, vp, vp, vp]
     L.dfm_stereo_tail_create.argtypes = [c_int, c_int, c_int, POINTER(vp)]
     L.dfm_stereo_tail_destroy.argtypes = [vp]

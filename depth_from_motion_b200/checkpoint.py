@@ -6,6 +6,7 @@ sub-module names of ``mmdet3d/models/detectors/dfm.py:54-76``:
     backbone_stereo.*          -> DfMBackbone
     feature_transformation.*   -> FrustumToVoxel
     neck_3d.*                  -> DfMNeck / OutdoorImVoxelNeck (multiview_dfm.py)
+    bbox_head_3d.*             -> Anchor3DHead (MultiViewDfM; mmdet3d-style keys only)
 
 and the original LIGA-DfM release uses older names that the reference's
 ``tools/model_converters/convert_dfm_checkpoints.py:34-63`` renames (first matching
@@ -26,7 +27,7 @@ _LIGA_RENAMES = (
     ('backbone_3d', 'backbone_stereo'),
 )
 
-HOT_PATH_PREFIXES = ('backbone_stereo', 'feature_transformation', 'neck_3d')
+HOT_PATH_PREFIXES = ('backbone_stereo', 'feature_transformation', 'neck_3d', 'bbox_head_3d')
 
 
 def convert_liga_key(key):
@@ -63,14 +64,16 @@ def hot_path_state_dicts(state_dict, liga=False):
 
 
 def load_hot_path(state_dict, backbone=None, frustum=None, neck=None, strict=True,
-                  liga=False):
+                  liga=False, head=None):
     """Loads the matching sub-dicts into the given mirror modules
-    (``DfMBackbone`` / ``FrustumToVoxel`` / ``DfMNeck`` or ``OutdoorImVoxelNeck``).
+    (``DfMBackbone`` / ``FrustumToVoxel`` / ``DfMNeck`` or ``OutdoorImVoxelNeck`` /
+    ``Anchor3DHead``, the latter from mmdet3d-style ``bbox_head_3d.*`` keys).
     Returns the ``{prefix: load_state_dict result}`` dict."""
     parts = hot_path_state_dicts(state_dict, liga=liga)
     res = {}
     for prefix, module in (('backbone_stereo', backbone),
-                           ('feature_transformation', frustum), ('neck_3d', neck)):
+                           ('feature_transformation', frustum), ('neck_3d', neck),
+                           ('bbox_head_3d', head)):
         if module is None:
             continue
         if strict and not parts[prefix]:

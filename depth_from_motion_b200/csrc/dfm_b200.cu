@@ -19,6 +19,7 @@
 #include "frustum_kernels.cuh"
 #include "tail_kernels.cuh"
 #include "logits_tc.cuh"
+#include "head1x1_tc.cuh"
 
 namespace {
 
@@ -1580,5 +1581,6 @@ int dfm_depth_head_forward(const float* d_cost, const float* d_depth_samples, in
 #include "frustum_api.inc"
 #include "pipeline_api.inc"
 #include "bev_api.inc"
+#include "anchor3d_head_api.inc"
 #include "voxel_sample_api.inc"
 #include "stereo_tail_api.inc"

@@ -11,6 +11,7 @@ of PyTorch ops:
     OutdoorImVoxelNeck   mmdet3d/models/necks/imvoxel_neck.py:8-68
     multiview_lift       mmdet3d/models/detectors/multiview_dfm.py:119-209
     FrustumToVoxel       mmdet3d/models/necks/feature_transformation.py:12-173
+    Anchor3DHead         mmdet3d/models/dense_heads/anchor3d_head.py:139-185 (forward)
 
 The ``nn.Conv3d`` / ``nn.GroupNorm`` / ``nn.BatchNorm3d`` children below are
 parameter containers only (they give the exact reference ``state_dict`` layout so
@@ -1100,6 +1101,99 @@ class LIGAAnchor3DHead(_HandleMirror):
         """Raw output [ny, nx, C] of 'cls<i>' / 'reg<i>' or of the output convs 'cls_out'
         (cls + dir channels) / 'reg_out', at their widths padded to 32 (tests only)."""
         return _debug_tensor(self._handle, 'dfm_anchor_head_debug_tensor', name, shape)
+
+
+@HEADS.register_module()
+class Anchor3DHead(_HandleMirror):
+    """Forward of the reference ``Anchor3DHead`` (dense_heads/anchor3d_head.py:15-185), the
+    ``bbox_head_3d`` of both MultiViewDfM (Waymo) configs: ``forward(feats) -> ([cls_score],
+    [bbox_pred], [dir_cls_preds or None])``.  The three 1x1 convs run as one tensor-core GEMM
+    that reads the BEV map once (``csrc/head1x1_tc.cuh``).  Anchor generation, target
+    assignment, losses and ``get_bboxes`` (NMS) stay with the reference's PyTorch code; the
+    constructor keeps their arguments so the config block builds unchanged, and the
+    ``state_dict`` (``conv_cls`` / ``conv_reg`` / ``conv_dir_cls``) is the reference's."""
+    _destroy = 'dfm_anchor3d_head_destroy'
+
+    def __init__(self, num_classes, in_channels, train_cfg=None, test_cfg=None,
+                 feat_channels=256, use_direction_classifier=True,
+                 anchor_generator=dict(type='Anchor3DRangeGenerator',
+                                       range=[0, -39.68, -1.78, 69.12, 39.68, -1.78],
+                                       strides=[2], sizes=[[3.9, 1.6, 1.56]],
+                                       rotations=[0, 1.57], custom_values=[],
+                                       reshape_out=False),
+                 assigner_per_size=False, assign_per_class=False, diff_rad_by_sin=True,
+                 dir_offset=-np.pi / 2, dir_limit_offset=0,
+                 bbox_coder=dict(type='DeltaXYZWLHRBBoxCoder'),
+                 loss_cls=dict(type='CrossEntropyLoss', use_sigmoid=True, loss_weight=1.0),
+                 loss_bbox=dict(type='SmoothL1Loss', beta=1.0 / 9.0, loss_weight=2.0),
+                 loss_dir=dict(type='CrossEntropyLoss', loss_weight=0.2), loss_iou=None,
+                 init_cfg=None, conv_impl='auto'):
+        super().__init__()
+        self.in_channels, self.num_classes = in_channels, num_classes
+        self.feat_channels = feat_channels
+        self.diff_rad_by_sin = diff_rad_by_sin
+        self.use_direction_classifier = use_direction_classifier
+        self.train_cfg, self.test_cfg = train_cfg, test_cfg
+        self.assigner_per_size, self.assign_per_class = assigner_per_size, assign_per_class
+        self.dir_offset, self.dir_limit_offset = dir_offset, dir_limit_offset
+        self.init_cfg = init_cfg
+        self.extra_cfg = dict(anchor_generator=anchor_generator, bbox_coder=bbox_coder,
+                              loss_cls=loss_cls, loss_bbox=loss_bbox, loss_dir=loss_dir,
+                              loss_iou=loss_iou)
+        # Anchor3DRangeGenerator.num_base_anchors (core/anchor/anchor_3d_generator.py:78-82)
+        sizes = np.asarray(anchor_generator.get('sizes', [[3.9, 1.6, 1.56]])).reshape(-1, 3)
+        self.num_anchors = len(anchor_generator.get('rotations', [0, 1.5707963])) * len(sizes)
+        self.box_code_size = int(bbox_coder.get('code_size', 7))   # DeltaXYZWLHRBBoxCoder
+        self.use_sigmoid_cls = loss_cls.get('use_sigmoid', False)  # anchor3d_head.py:99-102
+        if not self.use_sigmoid_cls:
+            self.num_classes += 1
+        self.conv_impl = conv_impl
+        # _init_layers (:139-147): 1x1 convs on feat_channels (in_channels is not used)
+        self.cls_out_channels = self.num_anchors * self.num_classes
+        self.conv_cls = nn.Conv2d(feat_channels, self.cls_out_channels, 1)
+        self.conv_reg = nn.Conv2d(feat_channels, self.num_anchors * self.box_code_size, 1)
+        if use_direction_classifier:
+            self.conv_dir_cls = nn.Conv2d(feat_channels, self.num_anchors * 2, 1)
+        self._handle = None
+        self._key = None
+
+    def forward(self, feats):
+        outs = [self.forward_single(x) for x in feats]       # multi_apply (:166-185)
+        return tuple(map(list, zip(*outs)))
+
+    def forward_single(self, x):
+        _check_cuda(x, 'x')
+        self._forward_only(x)
+        b, c, ny, nx = x.shape
+        if c != self.feat_channels:
+            raise RuntimeError(f'Anchor3DHead: input has {c} channels, the convs take '
+                               f'feat_channels = {self.feat_channels}')
+        L = capi.lib()
+        nd = self.num_anchors * 2 if self.use_direction_classifier else 0
+        nr = self.num_anchors * self.box_code_size
+        key = (ny, nx, self.conv_impl)
+        if self._handle is None or key != self._key:
+            self.release()
+            desc = capi.Anchor3DHeadDesc(self.feat_channels, self.cls_out_channels, nr, nd,
+                                         ny, nx, _IMPL[self.conv_impl])
+            hd = ctypes.c_void_p()
+            capi.check(L.dfm_anchor3d_head_create(ctypes.byref(desc), ctypes.byref(hd)),
+                       'dfm_anchor3d_head_create')
+            self._handle, self._key = hd, key
+            self._sync = _ParamSync()
+        self._sync.sync(self, lambda k, p, m: capi.check(
+            L.dfm_anchor3d_head_set_param(self._handle, k, p, m),
+            f'dfm_anchor3d_head_set_param({k.decode()})'))
+        x = x.contiguous()
+        cls = torch.empty((b, self.cls_out_channels, ny, nx), device=x.device)
+        box = torch.empty((b, nr, ny, nx), device=x.device)
+        dirc = torch.empty((b, nd, ny, nx), device=x.device) if nd else None
+        for i in range(b):
+            capi.check(L.dfm_anchor3d_head_forward(
+                self._handle, _ptr(x[i]), _ptr(cls[i]), _ptr(box[i]),
+                _ptr(dirc[i]) if dirc is not None else None, _stream()),
+                'dfm_anchor3d_head_forward')
+        return cls, box, dirc
 
 
 def aligned_voxel_centers(n_voxels, voxel_range):

@@ -136,9 +136,9 @@ def register_into_mmdet():
                                  module=modules.DfMBackbone)
     MM_HEADS.register_module(name='DepthHead', force=True,
                              module=modules.DepthHead)
-    # (LIGAAnchor3DHead is NOT forced into mmdet's registry: the mirror implements forward
-    # only, the detector needs the reference class's loss / get_bboxes; BEVHourglass's
-    # forward is the whole module)
+    # (LIGAAnchor3DHead and Anchor3DHead are NOT forced into mmdet's registry: the mirrors
+    # implement forward only, the detector needs the reference class's loss / get_bboxes;
+    # BEVHourglass's forward is the whole module)
     MM_BACKBONES.register_module(name='BEVHourglassB200', force=True,
                                  module=modules.BEVHourglass)
     try:

@@ -318,3 +318,27 @@ def make_bev_case(seed=91, nz=5, ny=44, nx=36, cv=32):
     rng = np.random.RandomState(seed)
     vol = torch.from_numpy(rng.standard_normal((1, cv, nz, ny, nx)).astype(np.float32)).relu()
     return dict(volume=vol, bev=make_bev_params(rng, cv * nz), head=make_anchor_head_params(rng))
+
+
+# the Anchor3DHead fixture (tests/golden/anchor3d_head.npz): 37 x 29 = 1,073 cells, i.e. 8 full
+# 128-cell tiles of the 1x1-conv kernel plus a ragged tail of 49
+ANCHOR3D_HEAD_CASE = dict(seed=101, feat=256, ny=37, nx=29)
+
+
+def make_anchor3d_head_case(seed=101, feat=256, ny=37, nx=29, num_anchors=6, num_classes=3,
+                            box_code_size=7):
+    """Inputs of the Anchor3DHead fixture: random (not near-zero-init) parameters of the three
+    1x1 convs in the reference state_dict order (dense_heads/anchor3d_head.py:139-147), and a
+    non-negative BEV map x [1, feat, ny, nx] (the neck's output is a blend of ReLUs)."""
+    rng = np.random.RandomState(seed)
+    p = {}
+    for name, co in (('conv_cls', num_anchors * num_classes),
+                     ('conv_reg', num_anchors * box_code_size),
+                     ('conv_dir_cls', num_anchors * 2)):
+        p[name + '.weight'] = (rng.standard_normal((co, feat, 1, 1)) /
+                               np.sqrt(feat)).astype(np.float32)
+        p[name + '.bias'] = (0.1 * rng.standard_normal(co)).astype(np.float32)
+    a = np.maximum(rng.standard_normal((1, feat, ny, nx)), 0)
+    b = np.maximum(rng.standard_normal((1, feat, ny, nx)), 0)
+    x = torch.from_numpy((0.7 * a + 0.3 * b).astype(np.float32))
+    return x, {k: torch.from_numpy(v) for k, v in p.items()}

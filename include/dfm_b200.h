@@ -377,6 +377,37 @@ int dfm_anchor_head_debug_tensor(dfm_anchor_head_t* h, const char* name, float* 
                                  long long numel, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * Anchor3DHead's forward (mmdet3d/models/dense_heads/anchor3d_head.py:139-164), the box head
+ * of both MultiViewDfM (Waymo) configs: three 1x1 convs with bias on the BEV map that
+ * DfMNeck / OutdoorImVoxelNeck return.  All tensors NCHW fp32.  conv_impl AUTO / TC run the
+ * three convs as one wgmma GEMM when feat_channels % 16 == 0 and the shape fits the kernel
+ * (combined output channels <= 128 and its shared-memory image); SIMT, and AUTO on other
+ * shapes, run the fp32 CUDA-core 2-D conv; TC on a shape without the kernel fails at create
+ * with DFM_ERR_INVALID.
+ * ---------------------------------------------------------------------------------- */
+typedef struct dfm_anchor3d_head dfm_anchor3d_head_t;
+typedef struct dfm_anchor3d_head_desc {
+  int feat_channels;  /* input channels of the three convs (256)                       */
+  int cls_channels;   /* num_anchors * num_classes (18)                               */
+  int reg_channels;   /* num_anchors * box_code_size (42)                             */
+  int dir_channels;   /* num_anchors * 2 (12), 0 without direction classifier         */
+  int ny, nx;         /* BEV grid (300 x 220)                                         */
+  int conv_impl;      /* DFM_CONV_AUTO / DFM_CONV_SIMT / DFM_CONV_TC                  */
+} dfm_anchor3d_head_desc_t;
+int dfm_anchor3d_head_create(const dfm_anchor3d_head_desc_t* desc, dfm_anchor3d_head_t** out);
+int dfm_anchor3d_head_destroy(dfm_anchor3d_head_t* h);
+/* Keys: "conv_cls.{weight,bias}", "conv_reg.{weight,bias}", "conv_dir_cls.{weight,bias}"
+ * (weights (out, feat_channels, 1, 1)); a wrong numel fails with DFM_ERR_INVALID. */
+int dfm_anchor3d_head_set_param(dfm_anchor3d_head_t* h, const char* name, const float* h_data,
+                                long long numel);
+int dfm_anchor3d_head_missing_params(const dfm_anchor3d_head_t* h);
+/* forward_single: d_x [feat_channels][ny][nx] -> cls_score [cls_channels][ny][nx], bbox_pred
+ * [reg_channels][ny][nx], dir_cls_preds [dir_channels][ny][nx] (d_dir may be NULL when
+ * dir_channels == 0).  DFM_ERR_STATE while a parameter is missing. */
+int dfm_anchor3d_head_forward(dfm_anchor3d_head_t* h, const float* d_x, float* d_cls,
+                              float* d_bbox, float* d_dir, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * voxel_sample (mmdet3d/models/fusion_layers/point_fusion.py:324-410): frustum-from-voxel
  * resampling for an optional depth head of MultiViewDfM (detectors/multiview_dfm.py:220-256;
  * no shipped config enables it).  d_voxel [C][Nx][Ny][Nz] -> d_out [C][num_depths][out_h][out_w],
