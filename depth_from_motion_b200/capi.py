@@ -46,6 +46,8 @@ SYMBOLS = (
     'dfm_anchor_head_debug_tensor',
     'dfm_anchor3d_head_create', 'dfm_anchor3d_head_destroy', 'dfm_anchor3d_head_set_param',
     'dfm_anchor3d_head_missing_params', 'dfm_anchor3d_head_forward',
+    'dfm_spp_neck_create', 'dfm_spp_neck_destroy', 'dfm_spp_neck_set_param',
+    'dfm_spp_neck_missing_params', 'dfm_spp_neck_forward', 'dfm_spp_neck_debug_tensor',
 )
 
 
@@ -217,7 +219,12 @@ def lib():
     L.dfm_stereo_tail_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
     L.dfm_stereo_tail_missing_params.argtypes = [vp]
     L.dfm_stereo_tail_forward.argtypes = [vp, vp, vp, vp, vp]
-    for f in ('neck', 'frustum', 'bev_hourglass', 'anchor_head'):
+    L.dfm_spp_neck_create.argtypes = [c_int, c_int, c_int, POINTER(vp)]
+    L.dfm_spp_neck_destroy.argtypes = [vp]
+    L.dfm_spp_neck_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
+    L.dfm_spp_neck_missing_params.argtypes = [vp]
+    L.dfm_spp_neck_forward.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    for f in ('neck', 'frustum', 'bev_hourglass', 'anchor_head', 'spp_neck'):
         getattr(L, f'dfm_{f}_debug_tensor').argtypes = [vp, c_char_p, vp, c_longlong, vp]
     L.dfm_voxel_sample.argtypes = [POINTER(VoxelSampleDesc), vp, vp, POINTER(c_double), vp, vp]
     _lib = L

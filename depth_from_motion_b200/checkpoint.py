@@ -7,6 +7,7 @@ sub-module names of ``mmdet3d/models/detectors/dfm.py:54-76``:
     feature_transformation.*   -> FrustumToVoxel
     neck_3d.*                  -> DfMNeck / OutdoorImVoxelNeck (multiview_dfm.py)
     bbox_head_3d.*             -> Anchor3DHead (MultiViewDfM; mmdet3d-style keys only)
+    neck.*                     -> SPPUNetNeck (DfM's image neck, detectors/dfm.py:44)
 
 and the original LIGA-DfM release uses older names that the reference's
 ``tools/model_converters/convert_dfm_checkpoints.py:34-63`` renames (first matching
@@ -27,7 +28,8 @@ _LIGA_RENAMES = (
     ('backbone_3d', 'backbone_stereo'),
 )
 
-HOT_PATH_PREFIXES = ('backbone_stereo', 'feature_transformation', 'neck_3d', 'bbox_head_3d')
+HOT_PATH_PREFIXES = ('backbone_stereo', 'feature_transformation', 'neck_3d', 'bbox_head_3d',
+                     'neck')
 
 
 def convert_liga_key(key):
@@ -64,16 +66,18 @@ def hot_path_state_dicts(state_dict, liga=False):
 
 
 def load_hot_path(state_dict, backbone=None, frustum=None, neck=None, strict=True,
-                  liga=False, head=None):
+                  liga=False, head=None, img_neck=None):
     """Loads the matching sub-dicts into the given mirror modules
     (``DfMBackbone`` / ``FrustumToVoxel`` / ``DfMNeck`` or ``OutdoorImVoxelNeck`` /
-    ``Anchor3DHead``, the latter from mmdet3d-style ``bbox_head_3d.*`` keys).
+    ``Anchor3DHead``, the latter from mmdet3d-style ``bbox_head_3d.*`` keys).  ``neck`` is the
+    3-D neck (``neck_3d.*``); the image neck ``SPPUNetNeck`` (``neck.*``, LIGA
+    ``backbone_3d.feature_neck.*``) is passed as ``img_neck``.
     Returns the ``{prefix: load_state_dict result}`` dict."""
     parts = hot_path_state_dicts(state_dict, liga=liga)
     res = {}
     for prefix, module in (('backbone_stereo', backbone),
                            ('feature_transformation', frustum), ('neck_3d', neck),
-                           ('bbox_head_3d', head)):
+                           ('bbox_head_3d', head), ('neck', img_neck)):
         if module is None:
             continue
         if strict and not parts[prefix]:

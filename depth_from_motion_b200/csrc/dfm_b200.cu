@@ -20,6 +20,7 @@
 #include "tail_kernels.cuh"
 #include "logits_tc.cuh"
 #include "head1x1_tc.cuh"
+#include "spp_neck_kernels.cuh"
 
 namespace {
 
@@ -306,6 +307,12 @@ int conv_simt_dispatch(const L& ld, const ConvW& w, float* out, const dfm::ConvG
   CASE(128, 128);
   CASE(128, 256);
   CASE(256, 256);
+  if constexpr (std::is_same<L, dfm::SrcLoader>::value) {
+    // SPPUNetNeck's upconv_module.conv.0, rpnconv.0 and rpnconv.1 (2-D layer driver only)
+    CASE(512, 64);
+    CASE(512, 128);
+    CASE(128, 32);
+  }
 #undef CASE
   return fail(DFM_ERR_INVALID, "conv3d: unsupported (Cin, Cout) = (" + std::to_string(g.Cin) +
                                    ", " + std::to_string(g.Cout) + ")");
@@ -1584,3 +1591,4 @@ int dfm_depth_head_forward(const float* d_cost, const float* d_depth_samples, in
 #include "anchor3d_head_api.inc"
 #include "voxel_sample_api.inc"
 #include "stereo_tail_api.inc"
+#include "spp_neck_api.inc"

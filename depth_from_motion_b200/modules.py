@@ -12,6 +12,7 @@ of PyTorch ops:
     multiview_lift       mmdet3d/models/detectors/multiview_dfm.py:119-209
     FrustumToVoxel       mmdet3d/models/necks/feature_transformation.py:12-173
     Anchor3DHead         mmdet3d/models/dense_heads/anchor3d_head.py:139-185 (forward)
+    SPPUNetNeck          mmdet3d/models/necks/spp_unet_neck.py (shipped KITTI config)
 
 The ``nn.Conv3d`` / ``nn.GroupNorm`` / ``nn.BatchNorm3d`` children below are
 parameter containers only (they give the exact reference ``state_dict`` layout so
@@ -955,6 +956,123 @@ class SPPUNetNeckTail(_HandleMirror):
         if b == 1:
             out._dfm_cl = twins[0]
         return out
+
+
+class _ConvGN1x1(nn.Module):
+    """Parameter layout of mmcv ConvModule(Conv2d 1x1, norm=GN): .conv / .gn."""
+
+    def __init__(self, cin, cout):
+        super().__init__()
+        self.conv = nn.Conv2d(cin, cout, 1, bias=False)
+        self.gn = nn.GroupNorm(32, cout)
+
+
+def _convbn_bn(cin, cout):
+    """Parameter layout of models/utils/conv_modules.py:6-24 ``convbn`` (SyncBatchNorm: the
+    BatchNorm2d placeholder has the same state_dict, num_batches_tracked included)."""
+    return nn.Sequential(nn.Conv2d(cin, cout, 3, 1, 1, bias=False), nn.BatchNorm2d(cout))
+
+
+class _UpconvModule(nn.Module):
+    """Parameter layout of models/utils/conv_modules.py:46-60 ``upconv_module([512, 64, 3],
+    [64, 32])``."""
+
+    def __init__(self):
+        super().__init__()
+        self.conv = nn.ModuleList([_convbn_bn(512, 64), _convbn_bn(64, 32)])
+        self.redir = nn.ModuleList([_convbn_bn(64, 64), _convbn_bn(3, 32)])
+
+
+@NECKS.register_module()
+class SPPUNetNeck(_HandleMirror):
+    """The reference ``SPPUNetNeck`` (necks/spp_unet_neck.py) of the shipped KITTI config on
+    CUDA: SPP branches, concat, ``upconv_module``, ``lastconv`` and ``rpnconv``
+    (``csrc/spp_neck_api.inc``).  ``forward(feats) -> (stereo_feature [B, 32, H, W],
+    sem_feature [B, 32, H/4, W/4])`` for ``feats = [img, f1, f2, f3, f4]`` (NCHW, LIGAResNet34's
+    [3 @ H, 64 @ H/2, 128 @ H/4 x 3]).  The ``state_dict`` is the reference's (46 entries, BN
+    running statistics included); BatchNorm runs in eval form.  For B == 1 the stereo feature
+    carries a channels-last twin that our ``DfMBackbone`` consumes without transposes.
+    Patch: ``model.neck = SPPUNetNeck(**cfg.model.neck)``."""
+    _destroy = 'dfm_spp_neck_destroy'
+
+    def __init__(self, in_channels, start_level, sem_channels=[128, 32], stereo_channels=[32, 32],
+                 spp_channel=32, with_upconv=True, cat_img_feature=True, norm_cfg=None,
+                 conv_impl='auto'):
+        super().__init__()
+        assert list(in_channels) == [3, 64, 128, 128, 128] and start_level == 2, \
+            'only the shipped KITTI configuration is implemented'
+        assert list(sem_channels) == [128, 32] and list(stereo_channels) == [32, 32]
+        assert spp_channel == 32 and with_upconv and cat_img_feature
+        assert norm_cfg is not None and norm_cfg.get('type') == 'GN' and \
+            norm_cfg.get('num_groups', 32) == 32, 'only the GroupNorm(32) variant is implemented'
+        self.in_channels, self.start_level = list(in_channels), start_level
+        self.sem_channels, self.stereo_channels = list(sem_channels), list(stereo_channels)
+        self.spp_channel, self.with_upconv = spp_channel, with_upconv
+        self.cat_img_feature = cat_img_feature
+        self.conv_impl = conv_impl
+        self.spp_branches = nn.ModuleList([
+            nn.Sequential(nn.AvgPool2d(s, stride=s), _ConvGN1x1(128, 32))
+            for s in (64, 32, 16, 8)])
+        self.upconv_module = _UpconvModule()
+        self.lastconv = nn.Sequential(_ConvGN2d(32, 32), nn.Conv2d(32, 32, 1, bias=False))
+        self.rpnconv = nn.Sequential(_ConvGN2d(512, 128), _ConvGN2d(128, 32))
+        self._handle = None
+        self._key = None
+
+    @staticmethod
+    def check_shapes(feats):
+        """Raises ValueError on the inputs the reference rejects (or cannot add up)."""
+        if len(feats) != 5:
+            raise ValueError(f'SPPUNetNeck takes 5 feature maps, got {len(feats)}')
+        img, f1, f2, f3, f4 = feats
+        b, _, h, w = img.shape
+        want = ((b, 3, h, w), (b, 64, h // 2, w // 2)) + ((b, 128, h // 4, w // 4),) * 3
+        got = tuple(tuple(f.shape) for f in feats)
+        if h % 4 or w % 4 or got != want:
+            raise ValueError(f'SPPUNetNeck: feature shapes {got} do not double from f2 to img '
+                             '(expected [3, H, W], [64, H/2, W/2], [128, H/4, W/4] x 3)')
+        h4, w4 = h // 4, w // 4
+        if (h4 // 64) * (w4 // 64) < 2:
+            raise ValueError(f'SPPUNetNeck: the 64x64 average pool of f4 ({h4} x {w4}) leaves '
+                             f'{(h4 // 64) * (w4 // 64)} cells; the reference needs at least 2 '
+                             '(AvgPool2d / GroupNorm)')
+
+    def forward(self, feats):
+        self.check_shapes(feats)
+        for i, f in enumerate(feats):
+            _check_cuda(f, f'feats[{i}]')
+        self._forward_only(*feats)
+        b, _, h, w = feats[0].shape
+        L = capi.lib()
+        key = (h, w, self.conv_impl)
+        if self._handle is None or key != self._key:
+            self.release()
+            hd = ctypes.c_void_p()
+            capi.check(L.dfm_spp_neck_create(h, w, _IMPL[self.conv_impl], ctypes.byref(hd)),
+                       'dfm_spp_neck_create')
+            self._handle, self._key = hd, key
+            self._sync = _ParamSync()
+        self._sync.sync(self, lambda k, p, m: capi.check(
+            L.dfm_spp_neck_set_param(self._handle, k, p, m),
+            f'dfm_spp_neck_set_param({k.decode()})'))
+        feats = [f.contiguous() for f in feats]
+        dev = feats[0].device
+        stereo = torch.empty((b, 32, h, w), device=dev)
+        sem = torch.empty((b, 32, h // 4, w // 4), device=dev)
+        cl = torch.empty((h, w, 32), device=dev) if b == 1 else None
+        for i in range(b):
+            capi.check(L.dfm_spp_neck_forward(
+                self._handle, *[_ptr(f[i]) for f in feats], _ptr(cl), _ptr(stereo[i]),
+                _ptr(sem[i]), _stream()), 'dfm_spp_neck_forward')
+        if cl is not None:
+            stereo._dfm_cl = cl
+        return stereo, sem
+
+    def debug_tensor(self, name, shape):
+        """Channels-last intermediate of the last forward: raw conv outputs 'conv0', 'redir0',
+        'conv1', 'rpn0', 'rpn1', 'lastconv'; 'pool64' .. 'pool8', 'spp64' .. 'spp8', 'concat',
+        'x0', 'x1' (tests only)."""
+        return _debug_tensor(self._handle, 'dfm_spp_neck_debug_tensor', name, shape)
 
 
 @BACKBONES.register_module()

@@ -342,3 +342,54 @@ def make_anchor3d_head_case(seed=101, feat=256, ny=37, nx=29, num_anchors=6, num
     b = np.maximum(rng.standard_normal((1, feat, ny, nx)), 0)
     x = torch.from_numpy((0.7 * a + 0.3 * b).astype(np.float32))
     return x, {k: torch.from_numpy(v) for k, v in p.items()}
+
+
+# SPPUNetNeck of the shipped KITTI config (configs/dfm/dfm_r34_1x8_kitti-3d-3class.py `neck`):
+# state_dict entries in the reference order (necks/spp_unet_neck.py:35-91,
+# models/utils/conv_modules.py:46-60)
+def spp_neck_state_shapes():
+    shapes = []
+    for i in range(4):
+        p = f'spp_branches.{i}.1.'
+        shapes += [(p + 'conv.weight', (32, 128, 1, 1)), (p + 'gn.weight', (32,)),
+                   (p + 'gn.bias', (32,))]
+    for name, (co, ci) in (('conv.0', (64, 512)), ('conv.1', (32, 64)),
+                           ('redir.0', (64, 64)), ('redir.1', (32, 3))):
+        p = f'upconv_module.{name}.'
+        shapes.append((p + '0.weight', (co, ci, 3, 3)))
+        shapes += [(p + '1.' + f, (co,)) for f in ('weight', 'bias', 'running_mean',
+                                                   'running_var')]
+        shapes.append((p + '1.num_batches_tracked', ()))
+    shapes += [('lastconv.0.conv.weight', (32, 32, 3, 3)), ('lastconv.0.gn.weight', (32,)),
+               ('lastconv.0.gn.bias', (32,)), ('lastconv.1.weight', (32, 32, 1, 1))]
+    for i, (co, ci) in enumerate(((128, 512), (32, 128))):
+        p = f'rpnconv.{i}.'
+        shapes += [(p + 'conv.weight', (co, ci, 3, 3)), (p + 'gn.weight', (co,)),
+                   (p + 'gn.bias', (co,))]
+    return shapes
+
+
+def make_spp_neck_case(seed, H, W):
+    """Inputs of SPPUNetNeck at image size H x W: feats = [img, f1, f2, f3, f4] ([1, C, h, w]
+    smooth fields with LIGAResNet34's shapes: 3 @ H, 64 @ H/2, 128 @ H/4 three times) and a random
+    state_dict (reference keys and order): Kaiming weights, GN / BN affines around 1 / 0, BN
+    running statistics away from the identity, so every folded affine carries signal."""
+    rng = np.random.RandomState(seed)
+    feats = [smooth_field(rng, 3, H, W, cell=16),
+             smooth_field(rng, 64, H // 2, W // 2)]
+    feats += [torch.relu(smooth_field(rng, 128, H // 4, W // 4, cell=4)) for _ in range(3)]
+    sd = {}
+    for k, shape in spp_neck_state_shapes():
+        if k.endswith('num_batches_tracked'):
+            sd[k] = torch.tensor(0, dtype=torch.int64)
+        elif len(shape) == 4:
+            sd[k] = torch.from_numpy(_kaiming(rng, shape, shape[1] * shape[2] * shape[3]))
+        elif k.endswith('running_var'):
+            sd[k] = torch.from_numpy((0.5 + rng.random_sample(shape)).astype(np.float32))
+        elif k.endswith('running_mean'):
+            sd[k] = torch.from_numpy((0.2 * rng.standard_normal(shape)).astype(np.float32))
+        elif k.endswith('weight'):
+            sd[k] = torch.from_numpy((0.5 + rng.random_sample(shape)).astype(np.float32))
+        else:
+            sd[k] = torch.from_numpy((0.2 * rng.standard_normal(shape)).astype(np.float32))
+    return feats, sd

@@ -466,6 +466,40 @@ int dfm_stereo_tail_missing_params(const dfm_stereo_tail_t* t);
 int dfm_stereo_tail_forward(dfm_stereo_tail_t* t, const float* d_x, float* d_out_cl,
                             float* d_out_nchw, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * The whole SPPUNetNeck of the shipped KITTI config (mmdet3d/models/necks/spp_unet_neck.py;
+ * configs/dfm/dfm_r34_1x8_kitti-3d-3class.py `neck`: in_channels [3, 64, 128, 128, 128],
+ * start_level 2, spp_channel 32, with_upconv, cat_img_feature, GN(32)), one image per call.
+ * H x W is the image size: d_img [3][H][W], d_f1 [64][H/2][W/2], d_f2 / d_f3 / d_f4
+ * [128][H/4][W/4], all NCHW.  Outputs: stereo_feature as d_stereo_cl [H][W][32] (channels-last,
+ * for dfm_backbone_forward_cl) and / or d_stereo_nchw [32][H][W]; sem_feature d_sem
+ * [32][H/4][W/4] NCHW (required).
+ * create: H and W multiples of 4, and floor(H/256) * floor(W/256) >= 2 (the reference's
+ * GroupNorm of the 64x64 SPP branch needs two cells); else DFM_ERR_INVALID.
+ * Keys: the reference state_dict without num_batches_tracked (42 entries): spp_branches.{0..3}.1.
+ * {conv.weight, gn.weight, gn.bias}, upconv_module.{conv,redir}.{0,1}.0.weight and .1.{weight,
+ * bias, running_mean, running_var} (BatchNorm, folded), lastconv.*, rpnconv.{0,1}.{conv.weight,
+ * gn.weight, gn.bias}.
+ * ---------------------------------------------------------------------------------- */
+typedef struct dfm_spp_neck dfm_spp_neck_t;
+int dfm_spp_neck_create(int H, int W, int conv_impl, dfm_spp_neck_t** out);
+int dfm_spp_neck_destroy(dfm_spp_neck_t* n);
+int dfm_spp_neck_set_param(dfm_spp_neck_t* n, const char* name, const float* h_data,
+                           long long numel);
+int dfm_spp_neck_missing_params(const dfm_spp_neck_t* n);
+int dfm_spp_neck_forward(dfm_spp_neck_t* n, const float* d_img, const float* d_f1,
+                         const float* d_f2, const float* d_f3, const float* d_f4,
+                         float* d_stereo_cl, float* d_stereo_nchw, float* d_sem, void* stream);
+/* Test hook: channels-last copy of an intermediate of the last forward.  Names: the raw conv
+ * outputs "conv0" (upconv.conv.0, [H/4][W/4][64]), "redir0" ([H/2][W/2][64]), "conv1"
+ * ([H/2][W/2][32]), "rpn0" ([H/4][W/4][128]), "rpn1" ([H/4][W/4][32]), "lastconv" ([H][W][32]);
+ * the pooled f4 "pool64" .. "pool8" ([Ph][Pw][128]); the branch maps before upsampling
+ * "spp64" .. "spp8" ([Ph][Pw][32], after GroupNorm + ReLU); "concat" ([H/4][W/4][512]); "x0"
+ * ([H/2][W/2][64]); "x1" ([H][W][32]).  DFM_ERR_STATE if the last forward did not write it,
+ * DFM_ERR_INVALID on a wrong element count. */
+int dfm_spp_neck_debug_tensor(dfm_spp_neck_t* n, const char* name, float* d_out,
+                              long long numel, void* stream);
+
 /* Re-entrancy: handles may live on different devices and be driven from different host
  * threads only if each thread owns its device; per-device scratch (K-slice partial sums,
  * lifting staging, the host-copy side stream) and the profiling record are shared by all
