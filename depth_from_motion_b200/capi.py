@@ -48,6 +48,8 @@ SYMBOLS = (
     'dfm_anchor3d_head_missing_params', 'dfm_anchor3d_head_forward',
     'dfm_spp_neck_create', 'dfm_spp_neck_destroy', 'dfm_spp_neck_set_param',
     'dfm_spp_neck_missing_params', 'dfm_spp_neck_forward', 'dfm_spp_neck_debug_tensor',
+    'dfm_fpn_create', 'dfm_fpn_destroy', 'dfm_fpn_set_param', 'dfm_fpn_missing_params',
+    'dfm_fpn_forward', 'dfm_fpn_debug_tensor',
 )
 
 
@@ -112,6 +114,12 @@ class Anchor3DHeadDesc(ctypes.Structure):
     _fields_ = [(n, c_int) for n in
                 ('feat_channels', 'cls_channels', 'reg_channels', 'dir_channels', 'ny', 'nx',
                  'conv_impl')]
+
+
+class FpnDesc(ctypes.Structure):
+    """``dfm_fpn_desc_t``."""
+    _fields_ = [('in_channels', c_int * 4), ('out_channels', c_int), ('level_h', c_int * 4),
+                ('level_w', c_int * 4), ('num_images', c_int), ('conv_impl', c_int)]
 
 
 class VoxelSampleDesc(ctypes.Structure):
@@ -224,7 +232,12 @@ def lib():
     L.dfm_spp_neck_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
     L.dfm_spp_neck_missing_params.argtypes = [vp]
     L.dfm_spp_neck_forward.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
-    for f in ('neck', 'frustum', 'bev_hourglass', 'anchor_head', 'spp_neck'):
+    L.dfm_fpn_create.argtypes = [POINTER(FpnDesc), POINTER(vp)]
+    L.dfm_fpn_destroy.argtypes = [vp]
+    L.dfm_fpn_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
+    L.dfm_fpn_missing_params.argtypes = [vp]
+    L.dfm_fpn_forward.argtypes = [vp, POINTER(vp), POINTER(vp), vp]
+    for f in ('neck', 'frustum', 'bev_hourglass', 'anchor_head', 'spp_neck', 'fpn'):
         getattr(L, f'dfm_{f}_debug_tensor').argtypes = [vp, c_char_p, vp, c_longlong, vp]
     L.dfm_voxel_sample.argtypes = [POINTER(VoxelSampleDesc), vp, vp, POINTER(c_double), vp, vp]
     _lib = L

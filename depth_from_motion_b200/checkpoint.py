@@ -7,7 +7,8 @@ sub-module names of ``mmdet3d/models/detectors/dfm.py:54-76``:
     feature_transformation.*   -> FrustumToVoxel
     neck_3d.*                  -> DfMNeck / OutdoorImVoxelNeck (multiview_dfm.py)
     bbox_head_3d.*             -> Anchor3DHead (MultiViewDfM; mmdet3d-style keys only)
-    neck.*                     -> SPPUNetNeck (DfM's image neck, detectors/dfm.py:44)
+    neck.*                     -> SPPUNetNeck (DfM's image neck, detectors/dfm.py:44) or
+                                  FPN (MultiViewDfM's image neck)
 
 and the original LIGA-DfM release uses older names that the reference's
 ``tools/model_converters/convert_dfm_checkpoints.py:34-63`` renames (first matching
@@ -70,8 +71,9 @@ def load_hot_path(state_dict, backbone=None, frustum=None, neck=None, strict=Tru
     """Loads the matching sub-dicts into the given mirror modules
     (``DfMBackbone`` / ``FrustumToVoxel`` / ``DfMNeck`` or ``OutdoorImVoxelNeck`` /
     ``Anchor3DHead``, the latter from mmdet3d-style ``bbox_head_3d.*`` keys).  ``neck`` is the
-    3-D neck (``neck_3d.*``); the image neck ``SPPUNetNeck`` (``neck.*``, LIGA
-    ``backbone_3d.feature_neck.*``) is passed as ``img_neck``.
+    3-D neck (``neck_3d.*``); the image neck (``neck.*``) is passed as ``img_neck``:
+    DfM's ``SPPUNetNeck`` (also from LIGA ``backbone_3d.feature_neck.*``) or MultiViewDfM's
+    ``FPN`` (``neck.lateral_convs.*`` / ``neck.fpn_convs.*``).
     Returns the ``{prefix: load_state_dict result}`` dict."""
     parts = hot_path_state_dicts(state_dict, liga=liga)
     res = {}

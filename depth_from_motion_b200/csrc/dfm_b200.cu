@@ -21,6 +21,7 @@
 #include "logits_tc.cuh"
 #include "head1x1_tc.cuh"
 #include "spp_neck_kernels.cuh"
+#include "fpn_kernels.cuh"
 
 namespace {
 
@@ -1592,3 +1593,4 @@ int dfm_depth_head_forward(const float* d_cost, const float* d_depth_samples, in
 #include "voxel_sample_api.inc"
 #include "stereo_tail_api.inc"
 #include "spp_neck_api.inc"
+#include "fpn_api.inc"

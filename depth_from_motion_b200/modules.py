@@ -13,6 +13,7 @@ of PyTorch ops:
     FrustumToVoxel       mmdet3d/models/necks/feature_transformation.py:12-173
     Anchor3DHead         mmdet3d/models/dense_heads/anchor3d_head.py:139-185 (forward)
     SPPUNetNeck          mmdet3d/models/necks/spp_unet_neck.py (shipped KITTI config)
+    FPN                  mmdet's FPN as the Waymo configs' image neck (mmdet 2.24 semantics)
 
 The ``nn.Conv3d`` / ``nn.GroupNorm`` / ``nn.BatchNorm3d`` children below are
 parameter containers only (they give the exact reference ``state_dict`` layout so
@@ -1312,6 +1313,120 @@ class Anchor3DHead(_HandleMirror):
                 _ptr(dirc[i]) if dirc is not None else None, _stream()),
                 'dfm_anchor3d_head_forward')
         return cls, box, dirc
+
+
+class _ConvModuleConv(nn.Module):
+    """Parameter layout of mmcv ConvModule without norm or activation: .conv only."""
+
+    def __init__(self, cin, cout, k):
+        super().__init__()
+        self.conv = nn.Conv2d(cin, cout, k, padding=k // 2)
+
+
+@NECKS.register_module()
+class FPN(_HandleMirror):
+    """mmdet's ``FPN`` image neck in the configuration of both MultiViewDfM (Waymo) configs
+    (``neck``: in_channels [256, 512, 1024, 2048], out_channels 64, num_outs 4) on CUDA
+    (``csrc/fpn_api.inc``): lateral 1x1 convs with the nearest-upsampled top-down merge fused
+    into one tensor-core GEMM per level, then the 3x3 ``fpn_convs``.  ``forward(inputs) ->
+    tuple`` of 4 NCHW maps, for any batch size in one call.  The ``state_dict`` is mmdet's
+    (``lateral_convs.{0..3}.conv.*``, ``fpn_convs.{0..3}.conv.*``).  Only that configuration is
+    implemented: extra convs, norm, activation, non-nearest upsampling, ``start_level != 0`` and
+    ``num_outs`` other than the number of levels raise ``NotImplementedError``.  It is
+    registered in the local ``NECKS`` only: KITTI's ``neck_2d`` is also an mmdet ``FPN`` (with
+    extra convs) and must keep resolving to mmdet's class.
+    Patch: ``model.neck = FPN(**cfg.model.neck)``."""
+    _destroy = 'dfm_fpn_destroy'
+
+    def __init__(self, in_channels, out_channels, num_outs, start_level=0, end_level=-1,
+                 add_extra_convs=False, relu_before_extra_convs=False, no_norm_on_lateral=False,
+                 conv_cfg=None, norm_cfg=None, act_cfg=None, upsample_cfg=dict(mode='nearest'),
+                 init_cfg=None, conv_impl='auto'):
+        super().__init__()
+        in_channels = list(in_channels)
+        n = len(in_channels)
+        if n != 4:
+            raise NotImplementedError(f'FPN: {n} input levels; only 4 are implemented')
+        if start_level != 0 or end_level not in (-1, n - 1):
+            raise NotImplementedError('FPN: only start_level=0 and end_level=-1 are implemented')
+        if num_outs < n:
+            raise ValueError(f'FPN: num_outs = {num_outs} is below the {n} input levels')
+        if num_outs > n or add_extra_convs:
+            raise NotImplementedError('FPN: extra levels (num_outs > number of inputs, '
+                                      'add_extra_convs) are not implemented')
+        if conv_cfg is not None or norm_cfg is not None or act_cfg is not None:
+            raise NotImplementedError('FPN: conv_cfg, norm_cfg and act_cfg must be None')
+        up = dict(upsample_cfg or {})
+        if up.get('mode', 'nearest') != 'nearest' or set(up) - {'mode'}:
+            raise NotImplementedError("FPN: only upsample_cfg=dict(mode='nearest') is implemented")
+        if any(c % 16 for c in in_channels + [out_channels]):
+            raise NotImplementedError('FPN: channel counts must be multiples of 16')
+        if out_channels not in (32, 64):
+            raise NotImplementedError('FPN: out_channels must be 64 (tensor cores) or 32')
+        self.in_channels, self.out_channels = in_channels, out_channels
+        self.num_ins, self.num_outs = n, num_outs
+        self.start_level, self.backbone_end_level = 0, n
+        self.add_extra_convs = False
+        self.relu_before_extra_convs = relu_before_extra_convs
+        self.no_norm_on_lateral = no_norm_on_lateral
+        self.upsample_cfg = up
+        self.init_cfg = init_cfg
+        self.conv_impl = conv_impl
+        self.lateral_convs = nn.ModuleList(_ConvModuleConv(c, out_channels, 1)
+                                           for c in in_channels)
+        self.fpn_convs = nn.ModuleList(_ConvModuleConv(out_channels, out_channels, 3)
+                                       for _ in in_channels)
+        self._handle = None
+        self._key = None
+
+    def check_shapes(self, inputs):
+        """Raises ValueError on inputs that disagree with the constructor."""
+        if len(inputs) != self.num_ins:
+            raise ValueError(f'FPN takes {self.num_ins} feature maps, got {len(inputs)}')
+        for i, (x, c) in enumerate(zip(inputs, self.in_channels)):
+            if x.dim() != 4 or x.shape[1] != c or x.shape[0] != inputs[0].shape[0]:
+                raise ValueError(f'FPN: inputs[{i}] has shape {tuple(x.shape)}; expected '
+                                 f'[{inputs[0].shape[0]}, {c}, H, W]')
+
+    def forward(self, inputs):
+        self.check_shapes(inputs)
+        for i, x in enumerate(inputs):
+            _check_cuda(x, f'inputs[{i}]')
+        self._forward_only(*inputs)
+        b = inputs[0].shape[0]
+        sizes = [tuple(x.shape[2:]) for x in inputs]
+        dev = inputs[0].device
+        outs = tuple(torch.empty((b, self.out_channels) + s, device=dev) for s in sizes)
+        if b == 0:
+            return outs
+        L = capi.lib()
+        key = (b, tuple(sizes), self.conv_impl)
+        if self._handle is None or key != self._key:
+            self.release()
+            desc = capi.FpnDesc()
+            desc.in_channels[:] = self.in_channels
+            desc.out_channels = self.out_channels
+            desc.level_h[:] = [s[0] for s in sizes]
+            desc.level_w[:] = [s[1] for s in sizes]
+            desc.num_images, desc.conv_impl = b, _IMPL[self.conv_impl]
+            hd = ctypes.c_void_p()
+            capi.check(L.dfm_fpn_create(ctypes.byref(desc), ctypes.byref(hd)), 'dfm_fpn_create')
+            self._handle, self._key = hd, key
+            self._sync = _ParamSync()
+        self._sync.sync(self, lambda k, p, m: capi.check(
+            L.dfm_fpn_set_param(self._handle, k, p, m), f'dfm_fpn_set_param({k.decode()})'))
+        xs = [x.contiguous() for x in inputs]
+        arr = ctypes.c_void_p * 4
+        capi.check(L.dfm_fpn_forward(self._handle, arr(*[x.data_ptr() for x in xs]),
+                                     arr(*[o.data_ptr() for o in outs]), _stream()),
+                   'dfm_fpn_forward')
+        return outs
+
+    def debug_tensor(self, name, shape):
+        """Channels-last [B, H, W, C] intermediate of the last forward: the merged laterals
+        'merged0' .. 'merged3' and the raw fpn_conv outputs before the bias 'fpn0' .. 'fpn3'
+        (tests only)."""
+        return _debug_tensor(self._handle, 'dfm_fpn_debug_tensor', name, shape)
 
 
 def aligned_voxel_centers(n_voxels, voxel_range):

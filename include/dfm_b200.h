@@ -500,6 +500,44 @@ int dfm_spp_neck_forward(dfm_spp_neck_t* n, const float* d_img, const float* d_f
 int dfm_spp_neck_debug_tensor(dfm_spp_neck_t* n, const char* name, float* d_out,
                               long long numel, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * mmdet's FPN image neck as both MultiViewDfM (Waymo) configs use it (`neck`: in_channels
+ * [256, 512, 1024, 2048], out_channels 64, num_outs 4; start_level 0, no extra convs, no norm,
+ * no activation, nearest upsampling to the finer level's size), for num_images images per
+ * call.  merged_3 = lateral_3(x_3); merged_l = lateral_l(x_l) + up(merged_{l+1});
+ * out_l = fpn_conv_l(merged_l).  The lateral 1x1 convs run as one wgmma GEMM per level with
+ * the merge in its epilogue when out_channels == 64 (conv_impl AUTO / TC); SIMT, and AUTO with
+ * out_channels == 32, run them on fp32 CUDA cores.  TC with out_channels != 64 fails at
+ * create with DFM_ERR_INVALID, as do channel counts that are not multiples of 16, other
+ * out_channels, and levels with in_channels * h * w >= 2^31.
+ * ---------------------------------------------------------------------------------- */
+typedef struct dfm_fpn dfm_fpn_t;
+typedef struct dfm_fpn_desc {
+  int in_channels[4];  /* channels of C2..C5 (256, 512, 1024, 2048)                       */
+  int out_channels;    /* 64 (tensor cores) or 32                                         */
+  int level_h[4];      /* sizes of the four levels, finest first (208, 104, 52, 26)      */
+  int level_w[4];      /* (312, 156, 78, 39)                                              */
+  int num_images;      /* images per call (views x frames of a sample)                   */
+  int conv_impl;       /* DFM_CONV_AUTO / DFM_CONV_SIMT / DFM_CONV_TC                     */
+} dfm_fpn_desc_t;
+int dfm_fpn_create(const dfm_fpn_desc_t* desc, dfm_fpn_t** out);
+int dfm_fpn_destroy(dfm_fpn_t* f);
+/* Keys: "lateral_convs.{0..3}.conv.{weight,bias}" (weights (out, in_l, 1, 1)) and
+ * "fpn_convs.{0..3}.conv.{weight,bias}" (weights (out, out, 3, 3)); a wrong numel fails with
+ * DFM_ERR_INVALID. */
+int dfm_fpn_set_param(dfm_fpn_t* f, const char* name, const float* h_data, long long numel);
+int dfm_fpn_missing_params(const dfm_fpn_t* f);
+/* d_in[l]: [num_images][in_channels[l]][level_h[l]][level_w[l]] NCHW -> d_out[l]:
+ * [num_images][out_channels][level_h[l]][level_w[l]] NCHW.  DFM_ERR_STATE while a parameter
+ * is missing. */
+int dfm_fpn_forward(dfm_fpn_t* f, const float* const* d_in, float* const* d_out, void* stream);
+/* Test hook: channels-last copy of an intermediate of the last forward.  "merged0" ..
+ * "merged3": the merged laterals [num_images][h_l][w_l][out_channels]; "fpn0" .. "fpn3": the
+ * raw fpn_conv outputs before the bias, same layout.  DFM_ERR_STATE if the last forward did
+ * not write it, DFM_ERR_INVALID on a wrong element count. */
+int dfm_fpn_debug_tensor(dfm_fpn_t* f, const char* name, float* d_out, long long numel,
+                         void* stream);
+
 /* Re-entrancy: handles may live on different devices and be driven from different host
  * threads only if each thread owns its device; per-device scratch (K-slice partial sums,
  * lifting staging, the host-copy side stream) and the profiling record are shared by all
