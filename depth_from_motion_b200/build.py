@@ -10,7 +10,8 @@ OUT = os.path.join(HERE, 'libdfm_b200.so')
 DEPS = [os.path.join(HERE, 'csrc', f) for f in
         ('dfm_b200.cu', 'common.cuh', 'simt_kernels.cuh', 'conv_tc.cuh', 'conv_tc_neck.cuh',
          'neck_api.inc', 'frustum_api.inc', 'frustum_kernels.cuh', 'pipeline_api.inc', 'bev_api.inc', 'tail_kernels.cuh', 'voxel_sample_api.inc', 'stereo_tail_api.inc', 'logits_tc.cuh', 'wgmma.cuh', 'head1x1_tc.cuh', 'anchor3d_head_api.inc', 'spp_neck_kernels.cuh',
-         'spp_neck_api.inc', 'fpn_kernels.cuh', 'fpn_api.inc')] + [os.path.join(HERE, '..', 'include', 'dfm_b200.h')]
+         'spp_neck_api.inc', 'fpn_kernels.cuh', 'fpn_api.inc', 'resnet_kernels.cuh',
+         'liga_resnet_api.inc')] + [os.path.join(HERE, '..', 'include', 'dfm_b200.h')]
 
 
 def nvcc_path():

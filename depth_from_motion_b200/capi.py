@@ -50,6 +50,8 @@ SYMBOLS = (
     'dfm_spp_neck_missing_params', 'dfm_spp_neck_forward', 'dfm_spp_neck_debug_tensor',
     'dfm_fpn_create', 'dfm_fpn_destroy', 'dfm_fpn_set_param', 'dfm_fpn_missing_params',
     'dfm_fpn_forward', 'dfm_fpn_debug_tensor',
+    'dfm_liga_resnet_create', 'dfm_liga_resnet_destroy', 'dfm_liga_resnet_set_param',
+    'dfm_liga_resnet_missing_params', 'dfm_liga_resnet_forward', 'dfm_liga_resnet_debug_tensor',
 )
 
 
@@ -120,6 +122,11 @@ class FpnDesc(ctypes.Structure):
     """``dfm_fpn_desc_t``."""
     _fields_ = [('in_channels', c_int * 4), ('out_channels', c_int), ('level_h', c_int * 4),
                 ('level_w', c_int * 4), ('num_images', c_int), ('conv_impl', c_int)]
+
+
+class LigaResNetDesc(ctypes.Structure):
+    """``dfm_liga_resnet_desc_t``."""
+    _fields_ = [(n, c_int) for n in ('height', 'width', 'num_images', 'conv_impl')]
 
 
 class VoxelSampleDesc(ctypes.Structure):
@@ -237,7 +244,13 @@ def lib():
     L.dfm_fpn_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
     L.dfm_fpn_missing_params.argtypes = [vp]
     L.dfm_fpn_forward.argtypes = [vp, POINTER(vp), POINTER(vp), vp]
-    for f in ('neck', 'frustum', 'bev_hourglass', 'anchor_head', 'spp_neck', 'fpn'):
+    L.dfm_liga_resnet_create.argtypes = [POINTER(LigaResNetDesc), POINTER(vp)]
+    L.dfm_liga_resnet_destroy.argtypes = [vp]
+    L.dfm_liga_resnet_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
+    L.dfm_liga_resnet_missing_params.argtypes = [vp]
+    L.dfm_liga_resnet_forward.argtypes = [vp, vp, POINTER(vp), vp]
+    for f in ('neck', 'frustum', 'bev_hourglass', 'anchor_head', 'spp_neck', 'fpn',
+              'liga_resnet'):
         getattr(L, f'dfm_{f}_debug_tensor').argtypes = [vp, c_char_p, vp, c_longlong, vp]
     L.dfm_voxel_sample.argtypes = [POINTER(VoxelSampleDesc), vp, vp, POINTER(c_double), vp, vp]
     _lib = L

@@ -9,12 +9,13 @@ sub-module names of ``mmdet3d/models/detectors/dfm.py:54-76``:
     bbox_head_3d.*             -> Anchor3DHead (MultiViewDfM; mmdet3d-style keys only)
     neck.*                     -> SPPUNetNeck (DfM's image neck, detectors/dfm.py:44) or
                                   FPN (MultiViewDfM's image neck)
+    backbone.*                 -> LIGAResNet (DfM's image backbone, detectors/dfm.py:43)
 
 and the original LIGA-DfM release uses older names that the reference's
 ``tools/model_converters/convert_dfm_checkpoints.py:34-63`` renames (first matching
 prefix wins, ``:77-81``).  The subset of that table that decides where hot-path
 parameters end up is restated here so a LIGA-style ``model_state`` can be read
-directly; all other prefixes (2-D backbone, necks, heads) are left untouched because
+directly; all other prefixes (``neck_2d``, the heads' decoding) are left untouched because
 those modules stay PyTorch on the caller's side.
 """
 from collections import OrderedDict
@@ -29,8 +30,9 @@ _LIGA_RENAMES = (
     ('backbone_3d', 'backbone_stereo'),
 )
 
+# (a key matches a prefix only up to its '.': 'backbone.' never captures 'backbone_stereo.*')
 HOT_PATH_PREFIXES = ('backbone_stereo', 'feature_transformation', 'neck_3d', 'bbox_head_3d',
-                     'neck')
+                     'neck', 'backbone')
 
 
 def convert_liga_key(key):
@@ -67,19 +69,22 @@ def hot_path_state_dicts(state_dict, liga=False):
 
 
 def load_hot_path(state_dict, backbone=None, frustum=None, neck=None, strict=True,
-                  liga=False, head=None, img_neck=None):
+                  liga=False, head=None, img_neck=None, img_backbone=None):
     """Loads the matching sub-dicts into the given mirror modules
     (``DfMBackbone`` / ``FrustumToVoxel`` / ``DfMNeck`` or ``OutdoorImVoxelNeck`` /
     ``Anchor3DHead``, the latter from mmdet3d-style ``bbox_head_3d.*`` keys).  ``neck`` is the
     3-D neck (``neck_3d.*``); the image neck (``neck.*``) is passed as ``img_neck``:
     DfM's ``SPPUNetNeck`` (also from LIGA ``backbone_3d.feature_neck.*``) or MultiViewDfM's
-    ``FPN`` (``neck.lateral_convs.*`` / ``neck.fpn_convs.*``).
+    ``FPN`` (``neck.lateral_convs.*`` / ``neck.fpn_convs.*``).  The image backbone
+    (``backbone.*``, DfM's ``LIGAResNet``; LIGA ``backbone_3d.feature_backbone.*``) is passed as
+    ``img_backbone``.
     Returns the ``{prefix: load_state_dict result}`` dict."""
     parts = hot_path_state_dicts(state_dict, liga=liga)
     res = {}
     for prefix, module in (('backbone_stereo', backbone),
                            ('feature_transformation', frustum), ('neck_3d', neck),
-                           ('bbox_head_3d', head), ('neck', img_neck)):
+                           ('bbox_head_3d', head), ('neck', img_neck),
+                           ('backbone', img_backbone)):
         if module is None:
             continue
         if strict and not parts[prefix]:

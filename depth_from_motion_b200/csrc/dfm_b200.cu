@@ -22,6 +22,7 @@
 #include "head1x1_tc.cuh"
 #include "spp_neck_kernels.cuh"
 #include "fpn_kernels.cuh"
+#include "resnet_kernels.cuh"
 
 namespace {
 
@@ -1594,3 +1595,4 @@ int dfm_depth_head_forward(const float* d_cost, const float* d_depth_samples, in
 #include "stereo_tail_api.inc"
 #include "spp_neck_api.inc"
 #include "fpn_api.inc"
+#include "liga_resnet_api.inc"

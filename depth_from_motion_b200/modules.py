@@ -14,6 +14,7 @@ of PyTorch ops:
     Anchor3DHead         mmdet3d/models/dense_heads/anchor3d_head.py:139-185 (forward)
     SPPUNetNeck          mmdet3d/models/necks/spp_unet_neck.py (shipped KITTI config)
     FPN                  mmdet's FPN as the Waymo configs' image neck (mmdet 2.24 semantics)
+    LIGAResNet           mmdet3d/models/backbones/liga_resnet.py (shipped KITTI config)
 
 The ``nn.Conv3d`` / ``nn.GroupNorm`` / ``nn.BatchNorm3d`` children below are
 parameter containers only (they give the exact reference ``state_dict`` layout so
@@ -1427,6 +1428,146 @@ class FPN(_HandleMirror):
         'merged0' .. 'merged3' and the raw fpn_conv outputs before the bias 'fpn0' .. 'fpn3'
         (tests only)."""
         return _debug_tensor(self._handle, 'dfm_fpn_debug_tensor', name, shape)
+
+
+class _LigaBasicBlock(nn.Module):
+    """Parameter layout of the reference ``LigaBasicBlock`` (backbones/liga_resnet.py:11-54):
+    conv1 / bn1 / conv2 / bn2 and an optional ``downsample`` = (1x1 conv, BatchNorm)."""
+
+    def __init__(self, inplanes, planes, stride, dilation, downsample):
+        super().__init__()
+        self.conv1 = nn.Conv2d(inplanes, planes, 3, stride, dilation, dilation, bias=False)
+        self.bn1 = nn.BatchNorm2d(planes)
+        self.conv2 = nn.Conv2d(planes, planes, 3, 1, 1, bias=False)
+        self.bn2 = nn.BatchNorm2d(planes)
+        self.downsample = nn.Sequential(
+            nn.Conv2d(inplanes, planes, 1, stride, bias=False),
+            nn.BatchNorm2d(planes)) if downsample else None
+        self.stride, self.dilation = stride, dilation
+
+
+@BACKBONES.register_module()
+class LIGAResNet(_HandleMirror):
+    """The reference ``LIGAResNet`` (backbones/liga_resnet.py) in the configuration of the shipped
+    KITTI config's ``backbone`` on CUDA (``csrc/liga_resnet_api.inc``): depth 34, strides
+    (1, 2, 1, 1), dilations (1, 1, 2, 4), num_channels_factor (1, 2, 2, 2), no max-pool and no
+    ReLU after the residual adds.  ``forward(img [B, 3, H, W]) -> tuple`` of 4 NCHW maps
+    ([B, 64, H2, W2] and three [B, 128, H4, W4], H2 = ceil(H / 2), H4 = ceil(H2 / 2)) for any
+    batch size in one C call.  The ``state_dict`` is the reference's (204 entries, BatchNorm
+    running statistics included); BatchNorm runs in eval form.  Other depths, strides,
+    dilations or channel factors, ``with_max_pool``, ``block_with_final_relu``, ``deep_stem``,
+    ``avg_down``, ``dcn``, ``plugins`` and non-BN norms raise ``NotImplementedError``.  It is
+    registered in the local ``BACKBONES`` only (forward-only: training keeps mmdet3d's class).
+    Patch: ``model.backbone = LIGAResNet(**cfg.model.backbone)``."""
+    _destroy = 'dfm_liga_resnet_destroy'
+    STAGE_BLOCKS = (3, 4, 6, 3)
+
+    def __init__(self, depth, in_channels=3, stem_channels=None, base_channels=64, num_stages=4,
+                 strides=(1, 2, 2, 2), dilations=(1, 1, 1, 1), out_indices=(0, 1, 2, 3),
+                 style='pytorch', deep_stem=False, avg_down=False, frozen_stages=-1,
+                 conv_cfg=None, norm_cfg=dict(type='BN', requires_grad=True), norm_eval=True,
+                 dcn=None, stage_with_dcn=(False, False, False, False), plugins=None,
+                 with_cp=False, zero_init_residual=True, init_cfg=None, with_max_pool=True,
+                 block_with_final_relu=True, num_channels_factor=None, conv_impl='auto'):
+        super().__init__()
+        checks = (
+            (depth == 34, f'depth={depth}'),
+            (in_channels == 3 and stem_channels in (None, 64) and base_channels == 64,
+             'in_channels / stem_channels / base_channels other than 3 / 64 / 64'),
+            (num_stages == 4 and tuple(strides) == (1, 2, 1, 1) and
+             tuple(dilations) == (1, 1, 2, 4), f'strides={strides}, dilations={dilations}'),
+            (tuple(out_indices) == (0, 1, 2, 3), f'out_indices={out_indices}'),
+            (num_channels_factor is not None and tuple(num_channels_factor) == (1, 2, 2, 2),
+             f'num_channels_factor={num_channels_factor}'),
+            (style == 'pytorch', f'style={style!r}'),
+            (not deep_stem, 'deep_stem'), (not avg_down, 'avg_down'),
+            (dcn is None and not any(stage_with_dcn), 'dcn'), (plugins is None, 'plugins'),
+            (conv_cfg is None, 'conv_cfg'),
+            (norm_cfg is not None and norm_cfg.get('type') in ('BN', 'SyncBN'),
+             f'norm_cfg={norm_cfg}'),
+            (not with_max_pool, 'with_max_pool'),
+            (not block_with_final_relu, 'block_with_final_relu'))
+        for ok, what in checks:
+            if not ok:
+                raise NotImplementedError(
+                    f'LIGAResNet: {what} is not implemented (only the shipped KITTI backbone: '
+                    'depth 34, strides (1, 2, 1, 1), dilations (1, 1, 2, 4), channel factors '
+                    '(1, 2, 2, 2), no max-pool, no final block ReLU, BatchNorm)')
+        self.depth, self.num_stages = depth, num_stages
+        self.strides, self.dilations = tuple(strides), tuple(dilations)
+        self.out_indices, self.style = tuple(out_indices), style
+        self.frozen_stages, self.norm_cfg, self.norm_eval = frozen_stages, norm_cfg, norm_eval
+        self.with_cp, self.zero_init_residual, self.init_cfg = with_cp, zero_init_residual, init_cfg
+        self.with_max_pool, self.block_with_final_relu = False, False
+        self.num_channels_factor = tuple(num_channels_factor)
+        self.conv_impl = conv_impl
+        self.conv1 = nn.Conv2d(3, 64, 7, 2, 3, bias=False)
+        self.bn1 = nn.BatchNorm2d(64)
+        self.res_layers = []
+        inplanes = 64
+        for i, n in enumerate(self.STAGE_BLOCKS):
+            planes = 64 * self.num_channels_factor[i]
+            blocks = []
+            for j in range(n):
+                stride = self.strides[i] if j == 0 else 1
+                blocks.append(_LigaBasicBlock(inplanes, planes, stride, self.dilations[i],
+                                              j == 0 and (stride != 1 or inplanes != planes)))
+                inplanes = planes
+            self.add_module(f'layer{i + 1}', nn.Sequential(*blocks))
+            self.res_layers.append(f'layer{i + 1}')
+        self._handle = None
+        self._key = None
+
+    @staticmethod
+    def output_sizes(h, w):
+        """(H2, W2), (H4, W4): PyTorch's output-size rule of the stride-2 convs."""
+        h2, w2 = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+        return (h2, w2), ((h2 - 1) // 2 + 1, (w2 - 1) // 2 + 1)
+
+    @staticmethod
+    def check_shapes(img):
+        """Raises ValueError on an input that is not [B, 3, H, W] with a non-empty image."""
+        if not isinstance(img, torch.Tensor) or img.dim() != 4 or img.shape[1] != 3 or \
+                img.shape[2] < 1 or img.shape[3] < 1:
+            shape = tuple(img.shape) if isinstance(img, torch.Tensor) else type(img).__name__
+            raise ValueError(f'LIGAResNet takes an image batch [B, 3, H, W], got {shape}')
+
+    def forward(self, img):
+        self.check_shapes(img)
+        _check_cuda(img, 'img')
+        self._forward_only(img)
+        b, _, h, w = img.shape
+        (h2, w2), (h4, w4) = self.output_sizes(h, w)
+        dev = img.device
+        outs = (torch.empty((b, 64, h2, w2), device=dev),) + \
+            tuple(torch.empty((b, 128, h4, w4), device=dev) for _ in range(3))
+        if b == 0:
+            return outs
+        L = capi.lib()
+        key = (b, h, w, self.conv_impl)
+        if self._handle is None or key != self._key:
+            self.release()
+            desc = capi.LigaResNetDesc(h, w, b, _IMPL[self.conv_impl])
+            hd = ctypes.c_void_p()
+            capi.check(L.dfm_liga_resnet_create(ctypes.byref(desc), ctypes.byref(hd)),
+                       'dfm_liga_resnet_create')
+            self._handle, self._key = hd, key
+            self._sync = _ParamSync()
+        self._sync.sync(self, lambda k, p, m: capi.check(
+            L.dfm_liga_resnet_set_param(self._handle, k, p, m),
+            f'dfm_liga_resnet_set_param({k.decode()})'))
+        x = img.contiguous()
+        arr = ctypes.c_void_p * 4
+        capi.check(L.dfm_liga_resnet_forward(self._handle, _ptr(x),
+                                             arr(*[o.data_ptr() for o in outs]), _stream()),
+                   'dfm_liga_resnet_forward')
+        return outs
+
+    def debug_tensor(self, name, shape):
+        """Channels-last [B, h, w, C] intermediate of the last forward: 'stem' (raw conv1),
+        'layerI.J.conv1' / 'layerI.J.conv2' / 'layer2.0.downsample' (raw conv outputs) and the
+        block outputs 'layerI.J' (tests only)."""
+        return _debug_tensor(self._handle, 'dfm_liga_resnet_debug_tensor', name, shape)
 
 
 def aligned_voxel_centers(n_voxels, voxel_range):

@@ -393,3 +393,48 @@ def make_spp_neck_case(seed, H, W):
         else:
             sd[k] = torch.from_numpy((0.2 * rng.standard_normal(shape)).astype(np.float32))
     return feats, sd
+
+
+def liga_resnet_state_shapes():
+    """(key, shape) of the reference LIGAResNet-34 state_dict of the KITTI config, in order
+    (backbones/liga_resnet.py; mmdet ResLayer naming, BatchNorm statistics included)."""
+    def bn(prefix, c):
+        return [(prefix + f, (c,)) for f in ('.weight', '.bias', '.running_mean', '.running_var')] + \
+            [(prefix + '.num_batches_tracked', ())]
+    shapes = [('conv1.weight', (64, 3, 7, 7))] + bn('bn1', 64)
+    inplanes = 64
+    for s, (n, planes) in enumerate(zip((3, 4, 6, 3), (64, 128, 128, 128))):
+        for j in range(n):
+            p = f'layer{s + 1}.{j}.'
+            shapes += [(p + 'conv1.weight', (planes, inplanes, 3, 3))] + bn(p + 'bn1', planes)
+            shapes += [(p + 'conv2.weight', (planes, planes, 3, 3))] + bn(p + 'bn2', planes)
+            if j == 0 and inplanes != planes:
+                shapes += [(p + 'downsample.0.weight', (planes, inplanes, 1, 1))] + \
+                    bn(p + 'downsample.1', planes)
+            inplanes = planes
+    return shapes
+
+
+def make_liga_resnet_case(seed, H, W, B=1):
+    """Inputs of LIGAResNet at image size H x W: a normalised-image-like batch [B, 3, H, W]
+    (smooth fields) and a random state_dict (reference keys and order): Kaiming conv weights,
+    BatchNorm statistics away from the identity; bn2's gamma is kept below 1 so the 16-block
+    residual chain (no ReLU after the adds) stays O(1)."""
+    rng = np.random.RandomState(seed)
+    img = torch.cat([smooth_field(rng, 3, H, W, cell=4) for _ in range(B)], 0)
+    sd = {}
+    for k, shape in liga_resnet_state_shapes():
+        if k.endswith('num_batches_tracked'):
+            sd[k] = torch.tensor(0, dtype=torch.int64)
+        elif len(shape) == 4:
+            sd[k] = torch.from_numpy(_kaiming(rng, shape, shape[1] * shape[2] * shape[3]))
+        elif k.endswith('running_var'):
+            sd[k] = torch.from_numpy((0.5 + rng.random_sample(shape)).astype(np.float32))
+        elif k.endswith('running_mean'):
+            sd[k] = torch.from_numpy((0.2 * rng.standard_normal(shape)).astype(np.float32))
+        elif k.endswith('weight'):
+            lo, hi = (0.2, 0.6) if '.bn2.' in k or 'downsample.1' in k else (0.5, 1.5)
+            sd[k] = torch.from_numpy((lo + (hi - lo) * rng.random_sample(shape)).astype(np.float32))
+        else:
+            sd[k] = torch.from_numpy((0.2 * rng.standard_normal(shape)).astype(np.float32))
+    return img, sd

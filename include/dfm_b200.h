@@ -538,6 +538,44 @@ int dfm_fpn_forward(dfm_fpn_t* f, const float* const* d_in, float* const* d_out,
 int dfm_fpn_debug_tensor(dfm_fpn_t* f, const char* name, float* d_out, long long numel,
                          void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * DfM's LIGAResNet-34 image backbone as the shipped KITTI config builds it (`backbone`:
+ * depth 34, strides (1, 2, 1, 1), dilations (1, 1, 2, 4), num_channels_factor (1, 2, 2, 2),
+ * no max-pool, no ReLU after the residual add, BatchNorm in eval form), for num_images images
+ * per call.  Stem 7x7 / 2 (3 -> 64); layer1: 3 blocks at 64 channels, H2 = ceil(H / 2);
+ * layer2: 4 blocks at 128 channels, the first with stride 2 and a 1x1 / 2 downsample,
+ * H4 = ceil(H2 / 2); layer3: 6 blocks, dilation 2; layer4: 3 blocks, dilation 4.
+ * AUTO / TC run every 3x3 stride-1 conv on the wgmma implicit-GEMM kernel and the stem, the
+ * stride-2 conv and the downsample on fp32 CUDA cores; SIMT runs every conv on fp32 CUDA
+ * cores.  Fails at create with DFM_ERR_INVALID on an empty image or num_images < 1.
+ * ---------------------------------------------------------------------------------- */
+typedef struct dfm_liga_resnet dfm_liga_resnet_t;
+typedef struct dfm_liga_resnet_desc {
+  int height;          /* image size H x W (384 x 1248 in the KITTI test pipeline)        */
+  int width;
+  int num_images;      /* images per call (cur + prev of a frame: 2)                      */
+  int conv_impl;       /* DFM_CONV_AUTO / DFM_CONV_SIMT / DFM_CONV_TC                     */
+} dfm_liga_resnet_desc_t;
+int dfm_liga_resnet_create(const dfm_liga_resnet_desc_t* desc, dfm_liga_resnet_t** out);
+int dfm_liga_resnet_destroy(dfm_liga_resnet_t* r);
+/* Keys are the reference state_dict's: "conv1.weight", "bn1.{weight,bias,running_mean,
+ * running_var}", "layer{1..4}.{j}.conv{1,2}.weight", "layer{1..4}.{j}.bn{1,2}.*",
+ * "layer2.0.downsample.0.weight", "layer2.0.downsample.1.*" ("num_batches_tracked" is not
+ * needed); a wrong numel fails with DFM_ERR_INVALID. */
+int dfm_liga_resnet_set_param(dfm_liga_resnet_t* r, const char* name, const float* h_data,
+                              long long numel);
+int dfm_liga_resnet_missing_params(const dfm_liga_resnet_t* r);
+/* d_img: [num_images][3][H][W] NCHW -> d_out[0]: [num_images][64][H2][W2], d_out[1..3]:
+ * [num_images][128][H4][W4], NCHW.  DFM_ERR_STATE while a parameter is missing. */
+int dfm_liga_resnet_forward(dfm_liga_resnet_t* r, const float* d_img, float* const* d_out,
+                            void* stream);
+/* Test hook: channels-last [num_images][h][w][C] copy of an intermediate of the last forward:
+ * "stem" (raw conv1 output), "layerI.J.conv1" / "layerI.J.conv2" / "layer2.0.downsample" (raw
+ * conv outputs, before BatchNorm), "layerI.J" (block outputs).  DFM_ERR_STATE if the last
+ * forward did not write it, DFM_ERR_INVALID on a wrong element count. */
+int dfm_liga_resnet_debug_tensor(dfm_liga_resnet_t* r, const char* name, float* d_out,
+                                 long long numel, void* stream);
+
 /* Re-entrancy: handles may live on different devices and be driven from different host
  * threads only if each thread owns its device; per-device scratch (K-slice partial sums,
  * lifting staging, the host-copy side stream) and the profiling record are shared by all
