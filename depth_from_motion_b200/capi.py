@@ -52,6 +52,8 @@ SYMBOLS = (
     'dfm_fpn_forward', 'dfm_fpn_debug_tensor',
     'dfm_liga_resnet_create', 'dfm_liga_resnet_destroy', 'dfm_liga_resnet_set_param',
     'dfm_liga_resnet_missing_params', 'dfm_liga_resnet_forward', 'dfm_liga_resnet_debug_tensor',
+    'dfm_resnet101_create', 'dfm_resnet101_destroy', 'dfm_resnet101_set_param',
+    'dfm_resnet101_missing_params', 'dfm_resnet101_forward', 'dfm_resnet101_debug_tensor',
 )
 
 
@@ -126,6 +128,11 @@ class FpnDesc(ctypes.Structure):
 
 class LigaResNetDesc(ctypes.Structure):
     """``dfm_liga_resnet_desc_t``."""
+    _fields_ = [(n, c_int) for n in ('height', 'width', 'num_images', 'conv_impl')]
+
+
+class ResNet101Desc(ctypes.Structure):
+    """``dfm_resnet101_desc_t``."""
     _fields_ = [(n, c_int) for n in ('height', 'width', 'num_images', 'conv_impl')]
 
 
@@ -249,8 +256,13 @@ def lib():
     L.dfm_liga_resnet_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
     L.dfm_liga_resnet_missing_params.argtypes = [vp]
     L.dfm_liga_resnet_forward.argtypes = [vp, vp, POINTER(vp), vp]
+    L.dfm_resnet101_create.argtypes = [POINTER(ResNet101Desc), POINTER(vp)]
+    L.dfm_resnet101_destroy.argtypes = [vp]
+    L.dfm_resnet101_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
+    L.dfm_resnet101_missing_params.argtypes = [vp]
+    L.dfm_resnet101_forward.argtypes = [vp, vp, POINTER(vp), vp]
     for f in ('neck', 'frustum', 'bev_hourglass', 'anchor_head', 'spp_neck', 'fpn',
-              'liga_resnet'):
+              'liga_resnet', 'resnet101'):
         getattr(L, f'dfm_{f}_debug_tensor').argtypes = [vp, c_char_p, vp, c_longlong, vp]
     L.dfm_voxel_sample.argtypes = [POINTER(VoxelSampleDesc), vp, vp, POINTER(c_double), vp, vp]
     _lib = L

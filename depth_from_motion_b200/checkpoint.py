@@ -9,7 +9,8 @@ sub-module names of ``mmdet3d/models/detectors/dfm.py:54-76``:
     bbox_head_3d.*             -> Anchor3DHead (MultiViewDfM; mmdet3d-style keys only)
     neck.*                     -> SPPUNetNeck (DfM's image neck, detectors/dfm.py:44) or
                                   FPN (MultiViewDfM's image neck)
-    backbone.*                 -> LIGAResNet (DfM's image backbone, detectors/dfm.py:43)
+    backbone.*                 -> LIGAResNet (DfM's image backbone, detectors/dfm.py:43) or
+                                  ResNet (MultiViewDfM's ResNet-101 + DCNv2 image backbone)
 
 and the original LIGA-DfM release uses older names that the reference's
 ``tools/model_converters/convert_dfm_checkpoints.py:34-63`` renames (first matching
@@ -76,7 +77,8 @@ def load_hot_path(state_dict, backbone=None, frustum=None, neck=None, strict=Tru
     3-D neck (``neck_3d.*``); the image neck (``neck.*``) is passed as ``img_neck``:
     DfM's ``SPPUNetNeck`` (also from LIGA ``backbone_3d.feature_neck.*``) or MultiViewDfM's
     ``FPN`` (``neck.lateral_convs.*`` / ``neck.fpn_convs.*``).  The image backbone
-    (``backbone.*``, DfM's ``LIGAResNet``; LIGA ``backbone_3d.feature_backbone.*``) is passed as
+    (``backbone.*``: DfM's ``LIGAResNet``, also from LIGA ``backbone_3d.feature_backbone.*``, or
+    MultiViewDfM's ``ResNet``, ``conv2.conv_offset.*`` of layer3 / layer4 included) is passed as
     ``img_backbone``.
     Returns the ``{prefix: load_state_dict result}`` dict."""
     parts = hot_path_state_dicts(state_dict, liga=liga)

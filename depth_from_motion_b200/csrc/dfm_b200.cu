@@ -23,6 +23,7 @@
 #include "spp_neck_kernels.cuh"
 #include "fpn_kernels.cuh"
 #include "resnet_kernels.cuh"
+#include "resnet101_kernels.cuh"
 
 namespace {
 
@@ -1596,3 +1597,4 @@ int dfm_depth_head_forward(const float* d_cost, const float* d_depth_samples, in
 #include "spp_neck_api.inc"
 #include "fpn_api.inc"
 #include "liga_resnet_api.inc"
+#include "resnet101_api.inc"

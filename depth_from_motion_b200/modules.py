@@ -15,6 +15,7 @@ of PyTorch ops:
     SPPUNetNeck          mmdet3d/models/necks/spp_unet_neck.py (shipped KITTI config)
     FPN                  mmdet's FPN as the Waymo configs' image neck (mmdet 2.24 semantics)
     LIGAResNet           mmdet3d/models/backbones/liga_resnet.py (shipped KITTI config)
+    ResNet               mmdet's ResNet-101 with DCNv2 as the Waymo configs' image backbone
 
 The ``nn.Conv3d`` / ``nn.GroupNorm`` / ``nn.BatchNorm3d`` children below are
 parameter containers only (they give the exact reference ``state_dict`` layout so
@@ -1568,6 +1569,169 @@ class LIGAResNet(_HandleMirror):
         'layerI.J.conv1' / 'layerI.J.conv2' / 'layer2.0.downsample' (raw conv outputs) and the
         block outputs 'layerI.J' (tests only)."""
         return _debug_tensor(self._handle, 'dfm_liga_resnet_debug_tensor', name, shape)
+
+
+class _ModulatedDeformConv2dPack(nn.Module):
+    """Parameter layout of mmcv's ``ModulatedDeformConv2dPack`` as DCNv2 builds it (3x3, no bias,
+    deform_groups 1): ``weight`` and ``conv_offset`` (3x3 conv to 27 channels with a bias)."""
+
+    def __init__(self, inplanes, planes, stride):
+        super().__init__()
+        self.weight = nn.Parameter(torch.zeros(planes, inplanes, 3, 3))
+        self.conv_offset = nn.Conv2d(inplanes, 27, 3, stride, 1, bias=True)
+        self.stride = stride
+
+
+class _Bottleneck(nn.Module):
+    """Parameter layout of mmdet's ``Bottleneck`` (style 'pytorch'): conv1 / bn1 / conv2 / bn2 /
+    conv3 / bn3 and an optional ``downsample`` = (1x1 conv, BatchNorm)."""
+
+    def __init__(self, inplanes, planes, stride, dcn, downsample):
+        super().__init__()
+        self.conv1 = nn.Conv2d(inplanes, planes, 1, bias=False)
+        self.bn1 = nn.BatchNorm2d(planes)
+        self.conv2 = _ModulatedDeformConv2dPack(planes, planes, stride) if dcn else \
+            nn.Conv2d(planes, planes, 3, stride, 1, bias=False)
+        self.bn2 = nn.BatchNorm2d(planes)
+        self.conv3 = nn.Conv2d(planes, planes * 4, 1, bias=False)
+        self.bn3 = nn.BatchNorm2d(planes * 4)
+        self.downsample = nn.Sequential(
+            nn.Conv2d(inplanes, planes * 4, 1, stride, bias=False),
+            nn.BatchNorm2d(planes * 4)) if downsample else None
+        self.stride = stride
+
+
+@BACKBONES.register_module()
+class ResNet(_HandleMirror):
+    """mmdet's ``ResNet`` (mmdet/models/backbones/resnet.py, 2.x) in the configuration of both
+    MultiViewDfM (Waymo) configs' ``backbone`` on CUDA (``csrc/resnet101_api.inc``): depth 101,
+    style 'pytorch', the default strides (1, 2, 2, 2), dilations and out_indices, max-pool stem,
+    and ``dcn=dict(type='DCNv2', deform_groups=1, fallback_on_stride=False)`` in layer3 / layer4
+    (every conv2 there is a modulated deformable conv, the stride-2 ones included).
+    ``forward(img [B, 3, H, W]) -> tuple`` of 4 NCHW maps [B, 256, H/4, W/4], [B, 512, H/8, W/8],
+    [B, 1024, H/16, W/16], [B, 2048, H/32, W/32] (PyTorch's output sizes: each stride-2 step
+    rounds up) for any batch size in one C call.  The ``state_dict`` is mmdet's (676 entries,
+    BatchNorm running statistics and ``conv2.conv_offset`` included); BatchNorm runs in eval
+    form.  ``frozen_stages``, ``norm_eval``, ``init_cfg`` / ``pretrained``, ``with_cp`` and
+    ``zero_init_residual`` are accepted and ignored; any other setting (other depths, no DCN,
+    other DCN placement, caffe style, deep stem, plugins, non-BN norms, ...) raises
+    ``NotImplementedError``.  It is registered in the local ``BACKBONES`` only, never over
+    mmdet's global ``ResNet`` (forward-only: training keeps mmdet's class).
+    Patch: ``model.backbone = ResNet(**cfg.model.backbone)``."""
+    _destroy = 'dfm_resnet101_destroy'
+    STAGE_BLOCKS = (3, 4, 23, 3)
+    DCN = dict(type='DCNv2', deform_groups=1, fallback_on_stride=False)
+
+    def __init__(self, depth, in_channels=3, stem_channels=None, base_channels=64, num_stages=4,
+                 strides=(1, 2, 2, 2), dilations=(1, 1, 1, 1), out_indices=(0, 1, 2, 3),
+                 style='pytorch', deep_stem=False, avg_down=False, frozen_stages=-1,
+                 conv_cfg=None, norm_cfg=dict(type='BN', requires_grad=True), norm_eval=True,
+                 dcn=None, stage_with_dcn=(False, False, False, False), plugins=None,
+                 with_cp=False, zero_init_residual=True, pretrained=None, init_cfg=None,
+                 conv_impl='auto'):
+        super().__init__()
+        dcn_ok = isinstance(dcn, dict) and dict(dcn) == self.DCN
+        checks = (
+            (depth == 101, f'depth={depth}'),
+            (in_channels == 3 and stem_channels in (None, 64) and base_channels == 64,
+             'in_channels / stem_channels / base_channels other than 3 / 64 / 64'),
+            (num_stages == 4 and tuple(strides) == (1, 2, 2, 2) and
+             tuple(dilations) == (1, 1, 1, 1), f'strides={strides}, dilations={dilations}'),
+            (tuple(out_indices) == (0, 1, 2, 3), f'out_indices={out_indices}'),
+            (style == 'pytorch', f'style={style!r}'),
+            (not deep_stem, 'deep_stem'), (not avg_down, 'avg_down'),
+            (dcn_ok, f'dcn={dcn}'),
+            (tuple(stage_with_dcn) == (False, False, True, True),
+             f'stage_with_dcn={stage_with_dcn}'),
+            (plugins is None, 'plugins'), (conv_cfg is None, 'conv_cfg'),
+            (norm_cfg is not None and norm_cfg.get('type') in ('BN', 'SyncBN'),
+             f'norm_cfg={norm_cfg}'))
+        for ok, what in checks:
+            if not ok:
+                raise NotImplementedError(
+                    f'ResNet: {what} is not implemented (only the Waymo backbone: depth 101, '
+                    "style 'pytorch', default strides / dilations, DCNv2 (deform_groups 1, "
+                    'fallback_on_stride False) in layer3 / layer4, BatchNorm)')
+        self.depth, self.num_stages = depth, num_stages
+        self.strides, self.dilations = tuple(strides), tuple(dilations)
+        self.out_indices, self.style = tuple(out_indices), style
+        self.frozen_stages, self.norm_cfg, self.norm_eval = frozen_stages, norm_cfg, norm_eval
+        self.dcn, self.stage_with_dcn = dict(dcn), tuple(stage_with_dcn)
+        self.with_cp, self.zero_init_residual = with_cp, zero_init_residual
+        self.pretrained, self.init_cfg = pretrained, init_cfg
+        self.conv_impl = conv_impl
+        self.conv1 = nn.Conv2d(3, 64, 7, 2, 3, bias=False)
+        self.bn1 = nn.BatchNorm2d(64)
+        self.res_layers = []
+        inplanes = 64
+        for i, n in enumerate(self.STAGE_BLOCKS):
+            planes = 64 << i
+            blocks = []
+            for j in range(n):
+                stride = self.strides[i] if j == 0 else 1
+                blocks.append(_Bottleneck(inplanes, planes, stride, self.stage_with_dcn[i],
+                                          j == 0))
+                inplanes = planes * 4
+            self.add_module(f'layer{i + 1}', nn.Sequential(*blocks))
+            self.res_layers.append(f'layer{i + 1}')
+        self._handle = None
+        self._key = None
+
+    @staticmethod
+    def output_sizes(h, w):
+        """[(H2, W2) of the stem, (H4, W4), (H8, W8), (H16, W16), (H32, W32)]: PyTorch's
+        output-size rule of every stride-2 step (ceil(n / 2))."""
+        out = []
+        for _ in range(5):
+            h, w = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+            out.append((h, w))
+        return out
+
+    @staticmethod
+    def check_shapes(img):
+        """Raises ValueError on an input that is not [B, 3, H, W] with a non-empty image."""
+        if not isinstance(img, torch.Tensor) or img.dim() != 4 or img.shape[1] != 3 or \
+                img.shape[2] < 1 or img.shape[3] < 1:
+            shape = tuple(img.shape) if isinstance(img, torch.Tensor) else type(img).__name__
+            raise ValueError(f'ResNet takes an image batch [B, 3, H, W], got {shape}')
+
+    def forward(self, img):
+        self.check_shapes(img)
+        _check_cuda(img, 'img')
+        self._forward_only(img)
+        b, _, h, w = img.shape
+        sizes = self.output_sizes(h, w)[1:]
+        dev = img.device
+        outs = tuple(torch.empty((b, 256 << l) + sizes[l], device=dev) for l in range(4))
+        if b == 0:
+            return outs
+        L = capi.lib()
+        key = (b, h, w, self.conv_impl)
+        if self._handle is None or key != self._key:
+            self.release()
+            desc = capi.ResNet101Desc(h, w, b, _IMPL[self.conv_impl])
+            hd = ctypes.c_void_p()
+            capi.check(L.dfm_resnet101_create(ctypes.byref(desc), ctypes.byref(hd)),
+                       'dfm_resnet101_create')
+            self._handle, self._key = hd, key
+            self._sync = _ParamSync()
+        self._sync.sync(self, lambda k, p, m: capi.check(
+            L.dfm_resnet101_set_param(self._handle, k, p, m),
+            f'dfm_resnet101_set_param({k.decode()})'))
+        x = img.contiguous()
+        arr = ctypes.c_void_p * 4
+        capi.check(L.dfm_resnet101_forward(self._handle, _ptr(x),
+                                           arr(*[o.data_ptr() for o in outs]), _stream()),
+                   'dfm_resnet101_forward')
+        return outs
+
+    def debug_tensor(self, name, shape):
+        """Channels-last [B, h, w, C] intermediate of the last forward: 'stem' (raw conv1),
+        'pool', 'layerI.J.conv1' / '.conv2' / '.conv3' / 'layerI.0.downsample' (raw conv
+        outputs), 'layerI.J.conv2.conv_offset' (conv_offset + bias, 32 channels of which 27 are
+        real), 'layerI.J.conv2.offset_mask' (the same with the sigmoid on channels 18..26) and
+        the block outputs 'layerI.J' (tests only)."""
+        return _debug_tensor(self._handle, 'dfm_resnet101_debug_tensor', name, shape)
 
 
 def aligned_voxel_centers(n_voxels, voxel_range):

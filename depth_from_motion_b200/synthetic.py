@@ -438,3 +438,64 @@ def make_liga_resnet_case(seed, H, W, B=1):
         else:
             sd[k] = torch.from_numpy((0.2 * rng.standard_normal(shape)).astype(np.float32))
     return img, sd
+
+
+def resnet101_state_shapes():
+    """(key, shape) of mmdet's ResNet-101 state_dict with DCNv2 in layer3 / layer4 (the Waymo
+    configs' backbone), in order: 676 entries, BatchNorm statistics and conv_offset included."""
+    def bn(prefix, c):
+        return [(prefix + f, (c,)) for f in ('.weight', '.bias', '.running_mean', '.running_var')] + \
+            [(prefix + '.num_batches_tracked', ())]
+    shapes = [('conv1.weight', (64, 3, 7, 7))] + bn('bn1', 64)
+    inplanes = 64
+    for s, n in enumerate((3, 4, 23, 3)):
+        planes = 64 << s
+        for j in range(n):
+            p = f'layer{s + 1}.{j}.'
+            shapes += [(p + 'conv1.weight', (planes, inplanes, 1, 1))] + bn(p + 'bn1', planes)
+            shapes.append((p + 'conv2.weight', (planes, planes, 3, 3)))
+            if s >= 2:
+                shapes += [(p + 'conv2.conv_offset.weight', (27, planes, 3, 3)),
+                           (p + 'conv2.conv_offset.bias', (27,))]
+            shapes += bn(p + 'bn2', planes)
+            shapes += [(p + 'conv3.weight', (4 * planes, planes, 1, 1))] + bn(p + 'bn3', 4 * planes)
+            if j == 0:
+                shapes += [(p + 'downsample.0.weight', (4 * planes, inplanes, 1, 1))] + \
+                    bn(p + 'downsample.1', 4 * planes)
+            inplanes = 4 * planes
+    return shapes
+
+
+def make_resnet101_case(seed, H, W, B=1):
+    """Inputs of the Waymo ResNet-101 + DCNv2 backbone at image size H x W: a
+    normalised-image-like batch [B, 3, H, W] (smooth fields) and a random state_dict (mmdet's
+    keys and order).  Kaiming conv weights; BatchNorm statistics away from the identity; bn3 and
+    the downsample's gamma small (0.1 - 0.3) so the 33-block residual chain stays O(1).  mmcv
+    zero-initialises conv_offset, which would reduce every DCN to a plain conv times 0.5; here
+    its weights give offsets of several pixels (samples leave the map, a few land near integer
+    positions) and its bias spreads the masks over (0, 1)."""
+    rng = np.random.RandomState(seed)
+    img = torch.cat([smooth_field(rng, 3, H, W, cell=4) for _ in range(B)], 0)
+    sd = {}
+    for k, shape in resnet101_state_shapes():
+        if k.endswith('num_batches_tracked'):
+            sd[k] = torch.tensor(0, dtype=torch.int64)
+        elif 'conv_offset' in k:
+            # the input of conv_offset is a ReLU'd, BN'd activation of O(1): offsets of a few
+            # pixels for gain ~3 (the 27 channels of a tap share no scale)
+            a = _kaiming(rng, shape, shape[1] * 9, gain=2.0) if len(shape) == 4 else \
+                (np.concatenate([1.5 * rng.standard_normal(18),
+                                 rng.standard_normal(9)]).astype(np.float32))
+            sd[k] = torch.from_numpy(a)
+        elif len(shape) == 4:
+            sd[k] = torch.from_numpy(_kaiming(rng, shape, shape[1] * shape[2] * shape[3]))
+        elif k.endswith('running_var'):
+            sd[k] = torch.from_numpy((0.5 + rng.random_sample(shape)).astype(np.float32))
+        elif k.endswith('running_mean'):
+            sd[k] = torch.from_numpy((0.2 * rng.standard_normal(shape)).astype(np.float32))
+        elif k.endswith('weight'):
+            lo, hi = (0.1, 0.3) if '.bn3.' in k or 'downsample.1' in k else (0.5, 1.5)
+            sd[k] = torch.from_numpy((lo + (hi - lo) * rng.random_sample(shape)).astype(np.float32))
+        else:
+            sd[k] = torch.from_numpy((0.2 * rng.standard_normal(shape)).astype(np.float32))
+    return img, sd

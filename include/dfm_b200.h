@@ -576,6 +576,49 @@ int dfm_liga_resnet_forward(dfm_liga_resnet_t* r, const float* d_img, float* con
 int dfm_liga_resnet_debug_tensor(dfm_liga_resnet_t* r, const char* name, float* d_out,
                                  long long numel, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * mmdet's ResNet-101 with DCNv2 as both MultiViewDfM (Waymo) configs build it (`backbone`:
+ * depth 101, style pytorch, BatchNorm in eval form, dcn DCNv2 with deform_groups 1 and
+ * fallback_on_stride False in layer3 / layer4), for num_images images per call.  Stem 7x7 / 2
+ * (3 -> 64), BN, ReLU, max-pool 3x3 / 2 / 1; Bottleneck stages of 3, 4, 23, 3 blocks at
+ * 256, 512, 1024, 2048 output channels; H_l = ceil(H_{l-1} / 2) at every stride-2 step.  The
+ * conv2 of layer3 / layer4 is a modulated deformable conv whose offsets and masks come from its
+ * conv_offset (3x3, 27 channels, bias).  AUTO / TC run every conv but the stem on wgmma kernels;
+ * SIMT runs every conv on fp32 CUDA cores.  Fails at create with DFM_ERR_INVALID on an empty
+ * image, num_images < 1 or num_images * ceil(H / 2) * ceil(W / 2) >= 2^31.
+ * ---------------------------------------------------------------------------------- */
+typedef struct dfm_resnet101 dfm_resnet101_t;
+typedef struct dfm_resnet101_desc {
+  int height;          /* image size H x W (832 x 1248 in the Waymo test pipeline)         */
+  int width;
+  int num_images;      /* images per call (views x frames of a sample)                    */
+  int conv_impl;       /* DFM_CONV_AUTO / DFM_CONV_SIMT / DFM_CONV_TC                     */
+} dfm_resnet101_desc_t;
+int dfm_resnet101_create(const dfm_resnet101_desc_t* desc, dfm_resnet101_t** out);
+int dfm_resnet101_destroy(dfm_resnet101_t* r);
+/* Keys are mmdet's state_dict's: "conv1.weight", "bn1.{weight,bias,running_mean,running_var}",
+ * "layer{1..4}.{j}.conv{1,2,3}.weight", "layer{1..4}.{j}.bn{1,2,3}.*",
+ * "layer{3,4}.{j}.conv2.conv_offset.{weight,bias}", "layer{1..4}.0.downsample.0.weight",
+ * "layer{1..4}.0.downsample.1.*" ("num_batches_tracked" is not needed); a wrong numel fails
+ * with DFM_ERR_INVALID. */
+int dfm_resnet101_set_param(dfm_resnet101_t* r, const char* name, const float* h_data,
+                            long long numel);
+int dfm_resnet101_missing_params(const dfm_resnet101_t* r);
+/* d_img: [num_images][3][H][W] NCHW -> d_out[l]: [num_images][256 << l][H_{l+2}][W_{l+2}]
+ * NCHW (H_2 = H / 4 .. H_5 = H / 32, rounded up).  DFM_ERR_STATE while a parameter is
+ * missing. */
+int dfm_resnet101_forward(dfm_resnet101_t* r, const float* d_img, float* const* d_out,
+                          void* stream);
+/* Test hook: channels-last [num_images][h][w][C] copy of an intermediate of the last forward:
+ * "stem" (raw conv1 output), "pool" (the max-pooled activation), "layerI.J.conv{1,2,3}" and
+ * "layerI.0.downsample" (raw conv outputs, before BatchNorm), "layerI.J.conv2.conv_offset"
+ * (conv_offset + bias, 27 channels padded to 32), "layerI.J.conv2.offset_mask" (the same with
+ * the sigmoid applied to channels 18..26: what the deformable conv reads), "layerI.J" (block
+ * outputs).  DFM_ERR_STATE if the last forward did not write it, DFM_ERR_INVALID on a wrong
+ * element count. */
+int dfm_resnet101_debug_tensor(dfm_resnet101_t* r, const char* name, float* d_out,
+                               long long numel, void* stream);
+
 /* Re-entrancy: handles may live on different devices and be driven from different host
  * threads only if each thread owns its device; per-device scratch (K-slice partial sums,
  * lifting staging, the host-copy side stream) and the profiling record are shared by all
