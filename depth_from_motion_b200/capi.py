@@ -54,6 +54,8 @@ SYMBOLS = (
     'dfm_liga_resnet_missing_params', 'dfm_liga_resnet_forward', 'dfm_liga_resnet_debug_tensor',
     'dfm_resnet101_create', 'dfm_resnet101_destroy', 'dfm_resnet101_set_param',
     'dfm_resnet101_missing_params', 'dfm_resnet101_forward', 'dfm_resnet101_debug_tensor',
+    'dfm_box_post_create', 'dfm_box_post_destroy', 'dfm_box_post_forward',
+    'dfm_box_post_debug_tensor',
 )
 
 
@@ -134,6 +136,13 @@ class LigaResNetDesc(ctypes.Structure):
 class ResNet101Desc(ctypes.Structure):
     """``dfm_resnet101_desc_t``."""
     _fields_ = [(n, c_int) for n in ('height', 'width', 'num_images', 'conv_impl')]
+
+
+class BoxPostDesc(ctypes.Structure):
+    """``dfm_box_post_desc_t``."""
+    _fields_ = [(n, c_int) for n in ('num_classes', 'num_anchors', 'ny', 'nx', 'batch',
+                                     'use_sigmoid', 'nms_pre', 'max_num')] + \
+               [(n, c_float) for n in ('score_thr', 'nms_thr', 'dir_offset', 'dir_limit_offset')]
 
 
 class VoxelSampleDesc(ctypes.Structure):
@@ -264,6 +273,10 @@ def lib():
     for f in ('neck', 'frustum', 'bev_hourglass', 'anchor_head', 'spp_neck', 'fpn',
               'liga_resnet', 'resnet101'):
         getattr(L, f'dfm_{f}_debug_tensor').argtypes = [vp, c_char_p, vp, c_longlong, vp]
+    L.dfm_box_post_create.argtypes = [POINTER(BoxPostDesc), vp, POINTER(vp)]
+    L.dfm_box_post_destroy.argtypes = [vp]
+    L.dfm_box_post_forward.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.dfm_box_post_debug_tensor.argtypes = [vp, c_char_p, vp, c_longlong, vp]
     L.dfm_voxel_sample.argtypes = [POINTER(VoxelSampleDesc), vp, vp, POINTER(c_double), vp, vp]
     _lib = L
     return L

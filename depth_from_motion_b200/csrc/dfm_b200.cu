@@ -24,6 +24,7 @@
 #include "fpn_kernels.cuh"
 #include "resnet_kernels.cuh"
 #include "resnet101_kernels.cuh"
+#include "box_post_kernels.cuh"
 
 namespace {
 
@@ -1598,3 +1599,4 @@ int dfm_depth_head_forward(const float* d_cost, const float* d_depth_samples, in
 #include "fpn_api.inc"
 #include "liga_resnet_api.inc"
 #include "resnet101_api.inc"
+#include "box_post_api.inc"

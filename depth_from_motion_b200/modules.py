@@ -11,7 +11,8 @@ of PyTorch ops:
     OutdoorImVoxelNeck   mmdet3d/models/necks/imvoxel_neck.py:8-68
     multiview_lift       mmdet3d/models/detectors/multiview_dfm.py:119-209
     FrustumToVoxel       mmdet3d/models/necks/feature_transformation.py:12-173
-    Anchor3DHead         mmdet3d/models/dense_heads/anchor3d_head.py:139-185 (forward)
+    Anchor3DHead         mmdet3d/models/dense_heads/anchor3d_head.py:139-185, 407-547
+                         (forward, get_bboxes; LIGAAnchor3DHead inherits the latter)
     SPPUNetNeck          mmdet3d/models/necks/spp_unet_neck.py (shipped KITTI config)
     FPN                  mmdet's FPN as the Waymo configs' image neck (mmdet 2.24 semantics)
     LIGAResNet           mmdet3d/models/backbones/liga_resnet.py (shipped KITTI config)
@@ -1135,13 +1136,156 @@ class BEVHourglass(_HandleMirror):
         return _debug_tensor(self._handle, 'dfm_bev_hourglass_debug_tensor', name, shape)
 
 
+def grid_anchors(anchor_generator, ny, nx, device):
+    """Anchor table ``[ny * nx * A, 7]`` of one feature level, built with the same
+    ``torch.linspace`` / ``torch.tensor`` calls as the reference generators
+    (core/anchor/anchor_3d_generator.py): ``Anchor3DRangeGenerator`` spaces ``n`` centres from
+    min to max; ``AlignedAnchor3DRangeGenerator`` spaces ``n + 1`` and shifts them by half a
+    cell.  Row ``(y * nx + x) * A + s * n_rots + r`` for range / size ``s`` and rotation ``r``,
+    as ``grid_anchors(...)[0].reshape(-1, 7)``.  Anchors are copies of those values, so the
+    table is the reference's bit for bit on the same device."""
+    g = dict(anchor_generator)
+    kind = g.get('type', 'Anchor3DRangeGenerator')
+    if kind not in ('Anchor3DRangeGenerator', 'AlignedAnchor3DRangeGenerator'):
+        raise NotImplementedError(f'anchor generator {kind}')
+    if g.get('custom_values') or not g.get('size_per_range', True) or \
+            g.get('align_corner', False):
+        raise NotImplementedError('custom_values, size_per_range=False and align_corner=True '
+                                  'are not implemented')
+    aligned = kind == 'AlignedAnchor3DRangeGenerator'
+    ranges, sizes = g['ranges'], g.get('sizes', [[3.9, 1.6, 1.56]])
+    rotations = g.get('rotations', [0, 1.5707963])
+    scale = g.get('scales', [1])[0]
+    if len(sizes) != len(ranges):
+        assert len(ranges) == 1
+        ranges = ranges * len(sizes)
+    extra = 1 if aligned else 0
+    per_range = []
+    for rng, size in zip(ranges, sizes):
+        rng = torch.tensor(rng, device=device)
+        axes = []
+        for lo, hi, n in ((rng[2], rng[5], 1), (rng[1], rng[4], ny), (rng[0], rng[3], nx)):
+            c = torch.linspace(lo, hi, n + extra, device=device)
+            if aligned:
+                c += (c[1] - c[0]) / 2
+            axes.append(c[:n])
+        z, y, x = axes
+        sz = torch.tensor(size, device=device).reshape(-1, 3) * scale       # [S, 3]
+        rot = torch.tensor(rotations, device=device)
+        S, R = sz.shape[0], rot.shape[0]
+        t = torch.empty((ny, nx, S, R, 7), device=device)
+        t[..., 0] = x.view(1, nx, 1, 1)
+        t[..., 1] = y.view(ny, 1, 1, 1)
+        t[..., 2] = z[0]
+        t[..., 3:6] = sz.view(1, 1, S, 1, 3)
+        t[..., 6] = rot.view(1, 1, 1, R)
+        per_range.append(t)
+    return torch.cat(per_range, dim=2).reshape(-1, 7)
+
+
+class _BoxPost:
+    """``get_bboxes`` of both anchor heads through ``dfm_box_post_*``: one handle and anchor
+    table per (feature map size, batch, device, test_cfg), kept until the key changes."""
+
+    def __init__(self):
+        self.handle, self.key = None, None
+
+    def release(self):
+        if self.handle is not None:
+            capi.lib().dfm_box_post_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
+
+    def run(self, head, cls_scores, bbox_preds, dir_cls_preds, input_metas, cfg, num_classes,
+            use_sigmoid, dir_offset, dir_limit_offset):
+        cfg = head.test_cfg if cfg is None else cfg
+        if dir_cls_preds is None or any(d is None for d in dir_cls_preds):
+            raise NotImplementedError('get_bboxes needs the direction classifier '
+                                      '(use_direction_classifier=True)')
+        if not cfg['use_rotate_nms']:
+            raise NotImplementedError('use_rotate_nms=False (axis-aligned BEV NMS)')
+        if len(cls_scores) != 1 or len(bbox_preds) != 1 or len(dir_cls_preds) != 1:
+            raise NotImplementedError('get_bboxes takes one feature level')
+        for meta in input_metas:
+            bt = meta.get('box_type_3d')
+            if bt is not None and getattr(bt, '__name__', '') != 'LiDARInstance3DBoxes':
+                raise NotImplementedError('NMS on the BEV of LiDARInstance3DBoxes only, got '
+                                          f'{bt!r}')
+        B = len(input_metas)
+        cls, box, dirc = (t[:B].detach().contiguous() for t in
+                          (cls_scores[0], bbox_preds[0], dir_cls_preds[0]))
+        for name, t in (('cls_score', cls), ('bbox_pred', box), ('dir_cls_pred', dirc)):
+            _check_cuda(t, name)
+        ny, nx = cls.shape[-2:]
+        A, ncol = head.num_anchors, num_classes + (0 if use_sigmoid else 1)
+        if cls.shape != (B, A * ncol, ny, nx) or box.shape != (B, A * 7, ny, nx) or \
+                dirc.shape != (B, A * 2, ny, nx):
+            raise RuntimeError(f'get_bboxes: unexpected head output shapes {tuple(cls.shape)}, '
+                               f'{tuple(box.shape)}, {tuple(dirc.shape)}')
+        max_num = int(cfg['max_num'])
+        desc_args = (num_classes, A, ny, nx, B, int(use_sigmoid), int(cfg.get('nms_pre', -1)),
+                     max_num, float(cfg.get('score_thr', 0)), float(cfg['nms_thr']),
+                     float(dir_offset), float(dir_limit_offset))
+        key = desc_args + (str(cls.device),)
+        L = capi.lib()
+        if self.handle is None or key != self.key:
+            self.release()
+            with torch.cuda.device(cls.device):
+                anchors = grid_anchors(head.extra_cfg['anchor_generator'], ny, nx, cls.device)
+            anchors = anchors.cpu().contiguous()
+            if anchors.shape[0] != ny * nx * A:
+                raise RuntimeError(f'anchor generator gives {anchors.shape[0] // (ny * nx)} '
+                                   f'anchors per cell, the head has {A}')
+            hd = ctypes.c_void_p()
+            capi.check(L.dfm_box_post_create(ctypes.byref(capi.BoxPostDesc(*desc_args)),
+                                             _ptr(anchors), ctypes.byref(hd)),
+                       'dfm_box_post_create')
+            self.handle, self.key = hd, key
+            n, nms_pre = ny * nx * A, desc_args[6]
+            self.batch, self.k = B, nms_pre if 0 < nms_pre < n else n
+        dev = cls.device
+        boxes = torch.empty((B, max_num, 7), device=dev)
+        scores = torch.empty((B, max_num), device=dev)
+        labels = torch.empty((B, max_num), device=dev, dtype=torch.int32)
+        count = torch.empty((B,), device=dev, dtype=torch.int32)
+        with torch.cuda.device(dev):
+            capi.check(L.dfm_box_post_forward(self.handle, _ptr(cls), _ptr(box), _ptr(dirc),
+                                              _ptr(boxes), _ptr(scores), _ptr(labels),
+                                              _ptr(count), _stream()), 'dfm_box_post_forward')
+        counts = count.cpu().tolist()
+        out = []
+        for b, meta in enumerate(input_metas):
+            k = counts[b]
+            bb = boxes[b, :k]
+            if meta.get('box_type_3d') is not None:
+                bb = meta['box_type_3d'](bb, box_dim=7)
+            out.append((bb, scores[b, :k], labels[b, :k].long()))
+        return out
+
+    def debug_tensor(self, name):
+        """int32 ``[batch, K]`` stage output of the last call (tests only): 'topk_index',
+        'cls<c>_candidates', 'cls<c>_keep'; -1 past each sample's count."""
+        if self.handle is None:
+            raise RuntimeError('dfm_box_post_debug_tensor: no get_bboxes call has run')
+        out = torch.empty((self.batch, self.k), device='cuda', dtype=torch.int32)
+        capi.check(capi.lib().dfm_box_post_debug_tensor(self.handle, name.encode(), _ptr(out),
+                                                         out.numel(), _stream()),
+                   f'dfm_box_post_debug_tensor({name})')
+        return out
+
+
 @HEADS.register_module()
 class LIGAAnchor3DHead(_HandleMirror):
     """Forward of the reference ``LIGAAnchor3DHead`` (dense_heads/liga_anchor3d_head.py:
-    12-128): ``forward(feats) -> ([cls_score], [bbox_pred], [dir_cls_preds])``.  Anchor
-    generation, target assignment, losses and ``get_bboxes`` (NMS) stay with the reference's
-    PyTorch code (SURVEY.md section 2.1: heads only consume the hot path's output); the
-    constructor keeps their arguments so the config block builds unchanged."""
+    12-128): ``forward(feats) -> ([cls_score], [bbox_pred], [dir_cls_preds])``, and the
+    inherited ``get_bboxes`` (anchors, decode, rotated BEV NMS) on CUDA.  Target assignment
+    and losses stay with the reference's PyTorch code; the constructor keeps their arguments
+    so the config block builds unchanged."""
     _destroy = 'dfm_anchor_head_destroy'
 
     def __init__(self, num_classes, in_channels, feat_channels=256, num_convs=2,
@@ -1223,15 +1367,32 @@ class LIGAAnchor3DHead(_HandleMirror):
         (cls + dir channels) / 'reg_out', at their widths padded to 32 (tests only)."""
         return _debug_tensor(self._handle, 'dfm_anchor_head_debug_tensor', name, shape)
 
+    def get_bboxes(self, cls_scores, bbox_preds, dir_cls_preds, input_metas, cfg=None,
+                   rescale=False):
+        """Anchor3DHead.get_bboxes (anchor3d_head.py:407-547), which LIGAAnchor3DHead inherits:
+        ``[(boxes [K, 7], scores [K], labels [K] int64)]`` per sample, on CUDA
+        (``dfm_box_post_*``).  Reads ``test_cfg`` (or ``cfg``) as the reference does; sigmoid
+        scores only, one feature level, rotated NMS only."""
+        loss_cls = self.extra_cfg.get('loss_cls', dict(use_sigmoid=True))
+        if not loss_cls.get('use_sigmoid', False):
+            raise NotImplementedError('LIGAAnchor3DHead.get_bboxes: softmax scores')
+        if not hasattr(self, '_box_post'):
+            self._box_post = _BoxPost()
+        return self._box_post.run(self, cls_scores, bbox_preds, dir_cls_preds, input_metas, cfg,
+                                  self.num_classes, True,
+                                  self.extra_cfg.get('dir_offset', -np.pi / 2),
+                                  self.extra_cfg.get('dir_limit_offset', 0))
+
 
 @HEADS.register_module()
 class Anchor3DHead(_HandleMirror):
     """Forward of the reference ``Anchor3DHead`` (dense_heads/anchor3d_head.py:15-185), the
     ``bbox_head_3d`` of both MultiViewDfM (Waymo) configs: ``forward(feats) -> ([cls_score],
     [bbox_pred], [dir_cls_preds or None])``.  The three 1x1 convs run as one tensor-core GEMM
-    that reads the BEV map once (``csrc/head1x1_tc.cuh``).  Anchor generation, target
-    assignment, losses and ``get_bboxes`` (NMS) stay with the reference's PyTorch code; the
-    constructor keeps their arguments so the config block builds unchanged, and the
+    that reads the BEV map once (``csrc/head1x1_tc.cuh``); ``get_bboxes`` (anchors, decode,
+    rotated BEV NMS) runs on CUDA too.  Target assignment and losses stay with the reference's
+    PyTorch code; the constructor keeps their arguments so the config block builds unchanged,
+    and the
     ``state_dict`` (``conv_cls`` / ``conv_reg`` / ``conv_dir_cls``) is the reference's."""
     _destroy = 'dfm_anchor3d_head_destroy'
 
@@ -1315,6 +1476,18 @@ class Anchor3DHead(_HandleMirror):
                 _ptr(dirc[i]) if dirc is not None else None, _stream()),
                 'dfm_anchor3d_head_forward')
         return cls, box, dirc
+
+    def get_bboxes(self, cls_scores, bbox_preds, dir_cls_preds, input_metas, cfg=None,
+                   rescale=False):
+        """Reference ``get_bboxes`` (anchor3d_head.py:407-547): ``[(boxes [K, 7], scores [K],
+        labels [K] int64)]`` per sample, on CUDA (``dfm_box_post_*``).  Reads ``test_cfg`` (or
+        ``cfg``) as the reference does; one feature level, rotated NMS only."""
+        if not hasattr(self, '_box_post'):
+            self._box_post = _BoxPost()
+        fg = self.num_classes if self.use_sigmoid_cls else self.num_classes - 1
+        return self._box_post.run(self, cls_scores, bbox_preds, dir_cls_preds, input_metas, cfg,
+                                  fg, self.use_sigmoid_cls, self.dir_offset,
+                                  self.dir_limit_offset)
 
 
 class _ConvModuleConv(nn.Module):

@@ -499,3 +499,68 @@ def make_resnet101_case(seed, H, W, B=1):
         else:
             sd[k] = torch.from_numpy((0.2 * rng.standard_normal(shape)).astype(np.float32))
     return img, sd
+
+
+# ---- anchor-head post-processing (get_bboxes) ----
+
+KITTI_ANCHOR_GENERATOR = dict(   # configs/dfm/dfm_r34_1x8_kitti-3d-3class.py:160-167
+    type='Anchor3DRangeGenerator',
+    ranges=[[2, -30.4, -1.78, 59.6, 30.4, -1.78], [2, -30.4, -0.6, 59.6, 30.4, -0.6],
+            [2, -30.4, -0.6, 59.6, 30.4, -0.6]],
+    sizes=[[3.9, 1.6, 1.56], [0.8, 0.6, 1.73], [1.76, 0.6, 1.73]],
+    rotations=[0, 1.57], reshape_out=False)
+WAYMO_ANCHOR_GENERATOR = dict(   # configs/dfm/multiview-dfm_r101_dcn_2x16_waymoD5-*.py:41-53
+    type='AlignedAnchor3DRangeGenerator',
+    ranges=[[-35.0, -75.0, 0, 75.0, 75.0, 0], [-35.0, -75.0, -0.1188, 75.0, 75.0, -0.1188],
+            [-35.0, -75.0, -0.0345, 75.0, 75.0, -0.0345]],
+    sizes=[[0.91, 0.84, 1.74], [1.81, 0.84, 1.77], [4.73, 2.08, 1.77]],
+    rotations=[0, 1.57], reshape_out=False)
+KITTI_TEST_CFG = dict(use_rotate_nms=True, nms_across_levels=False, nms_thr=0.25,
+                      score_thr=0.1, min_bbox_size=0, nms_pre=4096, max_num=500)
+WAYMO_TEST_CFG = dict(use_rotate_nms=True, nms_across_levels=False, nms_thr=0.05,
+                      score_thr=0.001, min_bbox_size=0, nms_pre=4096, max_num=500)
+KITTI_DIR_OFFSET, WAYMO_DIR_OFFSET = 0.7854, -0.7854
+
+
+def make_box_post_case(seed, ny, nx, num_anchors=6, ncol=3, num_objects=50, empty_class=None):
+    """Synthetic head outputs (cls_score [A * ncol, ny, nx], bbox_pred [A * 7, ny, nx],
+    dir_cls_preds [A * 2, ny, nx]) with `num_objects` planted objects: a 3 x 3-cell cluster whose
+    anchors of one class carry logits of 1 .. 4 (kept below sigmoid saturation so scores rarely
+    tie) and small varied deltas with an oblique yaw offset, so neighbouring boxes overlap and
+    NMS suppresses heavily; on top of a background of logits around -4.  `empty_class` gets
+    logits of -8 everywhere (no candidate at any shipped score_thr)."""
+    rng = np.random.RandomState(seed)
+    A = num_anchors
+    cls = (-4.0 + 1.2 * rng.standard_normal((A, ncol, ny, nx))).astype(np.float32)
+    box = (0.15 * rng.standard_normal((A, 7, ny, nx))).astype(np.float32)
+    box[:, 6] = (0.4 * rng.standard_normal((A, ny, nx))).astype(np.float32)
+    dirc = rng.standard_normal((A * 2, ny, nx)).astype(np.float32)
+    for _ in range(num_objects):
+        y, x = rng.randint(1, ny - 1), rng.randint(1, nx - 1)
+        c = rng.randint(ncol if ncol < 4 else ncol - 1)
+        yaw = rng.uniform(0.3, 1.3) * rng.choice([-1, 1])
+        for dy in (-1, 0, 1):
+            for dx in (-1, 0, 1):
+                for j in range(A):
+                    cls[j, c, y + dy, x + dx] = rng.uniform(1.0, 4.0) - 0.3 * (abs(dx) + abs(dy))
+                    box[j, :6, y + dy, x + dx] = 0.05 * rng.standard_normal(6)
+                    box[j, 6, y + dy, x + dx] = yaw + 0.05 * rng.standard_normal()
+    if empty_class is not None:
+        cls[:, empty_class] = -8.0
+    return (torch.from_numpy(cls.reshape(A * ncol, ny, nx)),
+            torch.from_numpy(box.reshape(A * 7, ny, nx)), torch.from_numpy(dirc))
+
+
+# name -> (generator, ny, nx, test_cfg, use_sigmoid, dir_offset, seed, extra case arguments)
+BOX_POST_CASES = {
+    'kitti_topk': (KITTI_ANCHOR_GENERATOR, 32, 24, dict(KITTI_TEST_CFG, nms_pre=2048), True,
+                   KITTI_DIR_OFFSET, 301, dict(num_objects=12)),
+    'waymo_no_topk': (WAYMO_ANCHOR_GENERATOR, 20, 16, WAYMO_TEST_CFG, True, WAYMO_DIR_OFFSET,
+                      302, dict(num_objects=8)),
+    'kitti_max_num_empty_class': (KITTI_ANCHOR_GENERATOR, 24, 20,
+                                  dict(KITTI_TEST_CFG, nms_pre=1500, max_num=20), True,
+                                  KITTI_DIR_OFFSET, 303, dict(num_objects=14, empty_class=2)),
+    'waymo_softmax': (WAYMO_ANCHOR_GENERATOR, 16, 12, dict(WAYMO_TEST_CFG, nms_pre=600,
+                                                           score_thr=0.05), False,
+                      WAYMO_DIR_OFFSET, 304, dict(num_objects=6, ncol=4)),
+}

@@ -619,6 +619,51 @@ int dfm_resnet101_forward(dfm_resnet101_t* r, const float* d_img, float* const* 
 int dfm_resnet101_debug_tensor(dfm_resnet101_t* r, const char* name, float* d_out,
                                long long numel, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * get_bboxes of Anchor3DHead and LIGAAnchor3DHead (one feature level) for `batch` samples per
+ * call: class scores (sigmoid, or softmax with the background column last), the top nms_pre
+ * anchors by their best class score (skipped when the grid has no more than nms_pre anchors),
+ * DeltaXYZWLHRBBoxCoder decode, per-class score_thr filter and rotated BEV NMS, the cut to
+ * max_num by score, and the direction-classifier yaw fix.  Anchor index (y * nx + x) *
+ * num_anchors + j; class channel j * ncol + c, box channel j * 7 + k, direction channel
+ * j * 2 + k.  No host synchronisation inside forward.  Create fails with DFM_ERR_INVALID when a
+ * class could receive more than 4096 NMS candidates (min(nms_pre, anchors), or all anchors when
+ * nms_pre <= 0) or num_classes > 16.
+ * ---------------------------------------------------------------------------------- */
+typedef struct dfm_box_post dfm_box_post_t;
+typedef struct dfm_box_post_desc {
+  int num_classes;        /* C foreground classes                                          */
+  int num_anchors;        /* anchors per cell (sizes x rotations), 6 in the shipped configs */
+  int ny;                 /* feature map H                                                 */
+  int nx;                 /* feature map W                                                 */
+  int batch;              /* samples per call                                              */
+  int use_sigmoid;        /* 1: C sigmoid columns; 0: C + 1 softmax columns               */
+  int nms_pre;            /* test_cfg.nms_pre (<= 0: no pre-NMS top-k)                    */
+  int max_num;            /* test_cfg.max_num                                              */
+  float score_thr;        /* test_cfg.score_thr (strict, in fp32)                          */
+  float nms_thr;          /* test_cfg.nms_thr (a box is suppressed when IoU > nms_thr)     */
+  float dir_offset;       /* head dir_offset                                               */
+  float dir_limit_offset; /* head dir_limit_offset                                         */
+} dfm_box_post_desc_t;
+/* h_anchors: host [ny * nx * num_anchors][7] fp32 (x, y, z, w, l, h, yaw), copied at create. */
+int dfm_box_post_create(const dfm_box_post_desc_t* desc, const float* h_anchors,
+                        dfm_box_post_t** out);
+int dfm_box_post_destroy(dfm_box_post_t* h);
+/* d_cls [batch][num_anchors * ncol][ny][nx], d_bbox [batch][num_anchors * 7][ny][nx],
+ * d_dir [batch][num_anchors * 2][ny][nx] (NCHW) -> d_boxes [batch][max_num][7],
+ * d_scores [batch][max_num], d_labels [batch][max_num] (int32), d_count [batch].  Entries
+ * at and past d_count[b] are not written. */
+int dfm_box_post_forward(dfm_box_post_t* h, const float* d_cls, const float* d_bbox,
+                         const float* d_dir, float* d_boxes, float* d_scores, int* d_labels,
+                         int* d_count, void* stream);
+/* Test hook: int32 [batch][K] (K = anchors that enter decoding) from the last forward:
+ * "topk_index" (selected anchors by score descending, anchor index ascending; DFM_ERR_STATE
+ * when the grid skipped the top-k), "cls<c>_candidates" (anchors passing score_thr for class c,
+ * in NMS processing order), "cls<c>_keep" (anchors kept by class c's NMS, in order); -1 past
+ * each sample's count.  DFM_ERR_INVALID on a wrong element count. */
+int dfm_box_post_debug_tensor(dfm_box_post_t* h, const char* name, int* d_out, long long numel,
+                              void* stream);
+
 /* Re-entrancy: handles may live on different devices and be driven from different host
  * threads only if each thread owns its device; per-device scratch (K-slice partial sums,
  * lifting staging, the host-copy side stream) and the profiling record are shared by all
