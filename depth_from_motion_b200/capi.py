@@ -55,7 +55,7 @@ SYMBOLS = (
     'dfm_resnet101_create', 'dfm_resnet101_destroy', 'dfm_resnet101_set_param',
     'dfm_resnet101_missing_params', 'dfm_resnet101_forward', 'dfm_resnet101_debug_tensor',
     'dfm_box_post_create', 'dfm_box_post_destroy', 'dfm_box_post_forward',
-    'dfm_box_post_debug_tensor',
+    'dfm_box_post_debug_tensor', 'dfm_op_rotated_iou',
 )
 
 
@@ -277,6 +277,7 @@ def lib():
     L.dfm_box_post_destroy.argtypes = [vp]
     L.dfm_box_post_forward.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.dfm_box_post_debug_tensor.argtypes = [vp, c_char_p, vp, c_longlong, vp]
+    L.dfm_op_rotated_iou.argtypes = [vp, vp, c_int, vp, vp]
     L.dfm_voxel_sample.argtypes = [POINTER(VoxelSampleDesc), vp, vp, POINTER(c_double), vp, vp]
     _lib = L
     return L

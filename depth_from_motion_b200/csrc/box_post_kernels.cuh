@@ -302,36 +302,43 @@ __device__ __forceinline__ float bp_cross(float ax, float ay, float bx, float by
   return __fsub_rn(__fmul_rn(ax, by), __fmul_rn(ay, bx));
 }
 
-// 2 x the signed area swept by the parts of P's edges inside Q (Green's theorem).  An edge lying
-// on one of Q's edge lines counts only if `keep_on_line` and both run the same way, so a
-// boundary shared by the two polygons is counted once (from P) and an edge touching from
-// outside is counted by neither.
-__device__ __forceinline__ float bp_clip_edges(const float (&px)[4], const float (&py)[4],
-                                               const float (&qx)[4], const float (&qy)[4],
-                                               bool keep_on_line) {
-  float acc = 0.f;
-#pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    const float x0 = px[e], y0 = py[e];
-    const float dx = __fsub_rn(px[(e + 1) & 3], x0), dy = __fsub_rn(py[(e + 1) & 3], y0);
-    float t0 = 0.f, t1 = 1.f;
-    bool ok = true;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float ex = __fsub_rn(qx[(k + 1) & 3], qx[k]), ey = __fsub_rn(qy[(k + 1) & 3], qy[k]);
-      const float den = bp_cross(ex, ey, dx, dy);
-      const float num = bp_cross(ex, ey, __fsub_rn(x0, qx[k]), __fsub_rn(y0, qy[k]));
-      if (den == 0.f) {
-        if (num < 0.f || (num == 0.f && !(keep_on_line && ex * dx + ey * dy > 0.f))) ok = false;
-      } else {
-        const float t = -num / den;
-        if (den > 0.f) t0 = fmaxf(t0, t);
-        else t1 = fminf(t1, t);
-      }
+// Vertex slots of the intersection polygon.  Clipping an n-gon by one half-plane keeps its i
+// inside vertices and adds one per sign change of the side values, of which there are at most
+// 2 min(i, n - i): at most floor(3 n / 2) vertices whatever the rounding.  From the 4 corners
+// that is 6, 9, 13, then 19 after the fourth line, so no vertex is ever dropped (exactly, a
+// convex quadrilateral needs at most 8; rounding adds vertices where several lie within
+// rounding of one clip line, as on near-duplicate boxes).  The polygon lives in local memory.
+constexpr int BP_POLY = 19;
+
+// One Sutherland-Hodgman step: the polygon (x, y)[0..n) clipped to the closed half-plane left of
+// the line through (qx, qy) along (ex, ey).  Each vertex's side is computed once and an edge
+// that crosses the line gives one point at t = s0 / (s0 - s1), which lies in [0, 1] however
+// the side values round, so the clipped area is continuous in the corners: an edge of P lying
+// on one of Q's edge lines is kept or cut by its two end vertices alone, never counted twice.
+__device__ __forceinline__ int bp_clip(const float* x, const float* y, int n, float qx, float qy,
+                                       float ex, float ey, float* ox, float* oy) {
+  if (n == 0) return 0;
+  const float sf = bp_cross(ex, ey, __fsub_rn(x[0], qx), __fsub_rn(y[0], qy));
+  float s0 = sf;
+  int m = 0;
+  for (int i = 0; i < n; ++i) {
+    const int k = i + 1 == n ? 0 : i + 1;
+    const float s1 = k == 0 ? sf : bp_cross(ex, ey, __fsub_rn(x[k], qx), __fsub_rn(y[k], qy));
+    const bool in0 = s0 >= 0.f, in1 = s1 >= 0.f;
+    if (in0) {
+      ox[m] = x[i];
+      oy[m] = y[i];
+      ++m;
     }
-    if (ok && t1 > t0) acc += (t1 - t0) * bp_cross(x0, y0, dx, dy);
+    if (in0 != in1) {
+      const float t = __fdiv_rn(s0, __fsub_rn(s0, s1));
+      ox[m] = __fadd_rn(x[i], __fmul_rn(t, __fsub_rn(x[k], x[i])));
+      oy[m] = __fadd_rn(y[i], __fmul_rn(t, __fsub_rn(y[k], y[i])));
+      ++m;
+    }
+    s0 = s1;
   }
-  return acc;
+  return m;
 }
 
 __device__ __forceinline__ float bp_iou(const BpRect& a, const BpRect& b) {
@@ -340,16 +347,30 @@ __device__ __forceinline__ float bp_iou(const BpRect& a, const BpRect& b) {
   const float cx = __fmul_rn(__fadd_rn(a.x, b.x), 0.5f), cy = __fmul_rn(__fadd_rn(a.y, b.y), 0.5f);
   const float ax = __fsub_rn(a.x, cx), ay = __fsub_rn(a.y, cy);
   const float bx = __fsub_rn(b.x, cx), by = __fsub_rn(b.y, cy);
-  float pax[4], pay[4], pbx[4], pby[4];
+  float px[BP_POLY], py[BP_POLY], tx[BP_POLY], ty[BP_POLY], qx[4], qy[4];
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
-    pax[k] = __fadd_rn(ax, a.ox[k]);
-    pay[k] = __fadd_rn(ay, a.oy[k]);
-    pbx[k] = __fadd_rn(bx, b.ox[k]);
-    pby[k] = __fadd_rn(by, b.oy[k]);
+    px[k] = __fadd_rn(ax, a.ox[k]);
+    py[k] = __fadd_rn(ay, a.oy[k]);
+    qx[k] = __fadd_rn(bx, b.ox[k]);
+    qy[k] = __fadd_rn(by, b.oy[k]);
   }
-  float inter = 0.5f * (bp_clip_edges(pax, pay, pbx, pby, true) +
-                        bp_clip_edges(pbx, pby, pax, pay, false));
+  // P (box a) clipped by Q's four edge lines in turn, ping-ponging between p and t
+  int n = 4;
+#pragma unroll
+  for (int k = 0; k < 4; k += 2) {
+    const float ex0 = __fsub_rn(qx[k + 1], qx[k]), ey0 = __fsub_rn(qy[k + 1], qy[k]);
+    const float ex1 = __fsub_rn(qx[(k + 2) & 3], qx[k + 1]);
+    const float ey1 = __fsub_rn(qy[(k + 2) & 3], qy[k + 1]);
+    n = bp_clip(px, py, n, qx[k], qy[k], ex0, ey0, tx, ty);
+    n = bp_clip(tx, ty, n, qx[k + 1], qy[k + 1], ex1, ey1, px, py);
+  }
+  // shoelace as a fan from vertex 0 (short difference vectors for a small polygon)
+  float a2 = 0.f;
+  for (int i = 1; i + 1 < n; ++i)
+    a2 = __fadd_rn(a2, bp_cross(__fsub_rn(px[i], px[0]), __fsub_rn(py[i], py[0]),
+                                __fsub_rn(px[i + 1], px[0]), __fsub_rn(py[i + 1], py[0])));
+  float inter = 0.5f * a2;
   inter = fminf(fmaxf(inter, 0.f), fminf(a.area, b.area));
   const float uni = a.area + b.area - inter;
   return uni > 0.f ? inter / uni : 0.f;

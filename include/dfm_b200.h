@@ -663,6 +663,10 @@ int dfm_box_post_forward(dfm_box_post_t* h, const float* d_cls, const float* d_b
  * each sample's count.  DFM_ERR_INVALID on a wrong element count. */
 int dfm_box_post_debug_tensor(dfm_box_post_t* h, const char* name, int* d_out, long long numel,
                               void* stream);
+/* Test hook: the fp32 rotated IoU the NMS of dfm_box_post_forward decides with, pair by pair.
+ * d_a, d_b: device [n][5] (x, y, w, h, yaw), the NMS box of the earlier and of the later
+ * candidate; d_iou: device [n].  DFM_ERR_INVALID on n <= 0 or a null pointer. */
+int dfm_op_rotated_iou(const float* d_a, const float* d_b, int n, float* d_iou, void* stream);
 
 /* Re-entrancy: handles may live on different devices and be driven from different host
  * threads only if each thread owns its device; per-device scratch (K-slice partial sums,

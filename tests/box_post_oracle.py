@@ -9,8 +9,9 @@ order open (ties of ``topk`` and of the unstable sorts) the restatement fixes it
 kernels do: score descending, then anchor index ascending; the final ``max_num`` cut keeps
 class-major order among equal scores.
 
-mmcv's ``nms_rotated`` is not in the reference tree.  ``rotated_iou`` restates it with an exact
-fp64 polygon intersection under ``NMS_ROTATED_ROT_SIGN``: corners at
+mmcv's ``nms_rotated`` is not in the reference tree.  ``rotated_iou`` restates it with an fp64
+polygon intersection (Sutherland-Hodgman clip, shoelace area; within 1e-12 of exact rational
+arithmetic, ``tests/test_rotated_iou.py``) under ``NMS_ROTATED_ROT_SIGN``: corners at
 ``centre + R(NMS_ROTATED_ROT_SIGN * theta) (+-w/2, +-h/2)``, i.e. vertex 0 at
 ``(x + s h/2 + c w/2, y + c h/2 - s w/2)`` (mmcv-full 1.6.0 box_iou_rotated_utils.hpp, its
 ``clockwise=True`` default; box3d_nms.py:264 passes no flag).  IoU = inter / (w1 h1 + w2 h2 -
@@ -35,31 +36,49 @@ def corners(boxes):
     return torch.stack((px, py), -1)
 
 
-def _clip_edges(P, Q, keep_on_line):
-    """2 x signed area swept by the parts of P's edges inside Q (Green's theorem), batched over
-    the leading dims.  An edge on one of Q's edge lines counts only with `keep_on_line` and the
-    same direction, so a shared boundary is counted once and a touching one not at all."""
-    acc = torch.zeros(P.shape[:-2], dtype=torch.float64, device=P.device)
-    for e in range(4):
-        p0, d = P[..., e, :], P[..., (e + 1) % 4, :] - P[..., e, :]
-        t0 = torch.zeros_like(acc)
-        t1 = torch.ones_like(acc)
-        ok = torch.ones_like(acc, dtype=torch.bool)
-        for k in range(4):
-            q0 = Q[..., k, :]
-            ed = Q[..., (k + 1) % 4, :] - q0
-            den = ed[..., 0] * d[..., 1] - ed[..., 1] * d[..., 0]
-            rel = p0 - q0
-            num = ed[..., 0] * rel[..., 1] - ed[..., 1] * rel[..., 0]
-            par = den == 0
-            same = (ed * d).sum(-1) > 0
-            ok &= ~(par & ((num < 0) | ((num == 0) & ~(same & keep_on_line))))
-            t = torch.where(par, torch.zeros_like(num), -num / torch.where(par, 1.0, den))
-            t0 = torch.where(~par & (den > 0), torch.maximum(t0, t), t0)
-            t1 = torch.where(~par & (den < 0), torch.minimum(t1, t), t1)
-        cr = p0[..., 0] * d[..., 1] - p0[..., 1] * d[..., 0]
-        acc = acc + torch.where(ok & (t1 > t0), (t1 - t0) * cr, torch.zeros_like(acc))
-    return acc
+def _clip_half_plane(V, n, q0, e):
+    """One Sutherland-Hodgman step, batched over the leading dims: the polygons V [..., S, 2]
+    (first n [...] vertices valid) clipped to the closed half-plane left of the line through
+    q0 [..., 2] along e [..., 2].  A crossing edge gives one point at t = s0 / (s0 - s1) in
+    [0, 1], so the area stays continuous in the corners where edges are (nearly) collinear.
+    The result keeps the i inside vertices and one per sign change of the side values (at most
+    2 min(i, S - i)), so S * 3 // 2 slots always suffice: 6, 9, 13, 19 from a quadrilateral.
+    Returns the clipped polygons [..., S * 3 // 2, 2] and their vertex counts."""
+    S = V.shape[-2]
+    idx = torch.arange(S, device=V.device)
+    valid = idx < n[..., None]
+    nxt = torch.where(idx + 1 < n[..., None], idx + 1, torch.zeros_like(idx))
+    V1 = torch.gather(V, -2, nxt[..., None].expand(V.shape))
+    rel = V - q0[..., None, :]
+    side = e[..., None, 0] * rel[..., 1] - e[..., None, 1] * rel[..., 0]
+    side1 = torch.gather(side, -1, nxt)
+    in0, in1 = side >= 0, side1 >= 0
+    cross = valid & (in0 != in1)
+    t = side / torch.where(cross, side - side1, torch.ones_like(side))
+    cut = V + t[..., None] * (V1 - V)
+    cand = torch.stack((V, cut), -2).flatten(-3, -2)                  # [..., 2 S, 2]
+    take = torch.stack((valid & in0, cross), -1).flatten(-2)          # [..., 2 S]
+    slots = S * 3 // 2
+    pos = torch.cumsum(take.long(), -1) - 1
+    pos = torch.where(take, pos, torch.full_like(pos, slots))
+    out = V.new_zeros(V.shape[:-2] + (slots + 1, 2))
+    out.scatter_(-2, pos[..., None].expand(cand.shape), cand)
+    return out[..., :slots, :], take.sum(-1)
+
+
+def _intersection_area(P, Q):
+    """Area of the intersection of the counter-clockwise quadrilaterals P, Q [..., 4, 2]: P
+    clipped by Q's four edge lines (Sutherland-Hodgman), then the shoelace formula as a fan from
+    vertex 0."""
+    V = P
+    n = torch.full(P.shape[:-2], 4, dtype=torch.long, device=P.device)
+    for k in range(4):
+        V, n = _clip_half_plane(V, n, Q[..., k, :], Q[..., (k + 1) % 4, :] - Q[..., k, :])
+    d = V[..., 1:, :] - V[..., :1, :]
+    tri = d[..., :-1, 0] * d[..., 1:, 1] - d[..., :-1, 1] * d[..., 1:, 0]
+    idx = torch.arange(1, V.shape[-2] - 1, device=V.device)
+    tri = torch.where(idx + 1 < n[..., None], tri, torch.zeros_like(tri))
+    return 0.5 * tri.sum(-1)
 
 
 def rotated_iou(a, b):
@@ -70,8 +89,7 @@ def rotated_iou(a, b):
     cy = (a[..., 1] + b[..., 1]) / 2
     shift = torch.stack((cx, cy, torch.zeros_like(cx), torch.zeros_like(cx),
                          torch.zeros_like(cx)), -1)
-    A, B = corners(a - shift), corners(b - shift)
-    inter = 0.5 * (_clip_edges(A, B, True) + _clip_edges(B, A, False))
+    inter = _intersection_area(corners(a - shift), corners(b - shift))
     area_a, area_b = a[..., 2] * a[..., 3], b[..., 2] * b[..., 3]
     inter = torch.minimum(inter.clamp(min=0), torch.minimum(area_a, area_b))
     union = area_a + area_b - inter

@@ -331,6 +331,318 @@ def test_c_api_canaries_and_errors():
         L.dfm_box_post_destroy(hd)
 
 
+# Designed grids through the C entry point: one anchor per cell on a 1 x N grid, an anchor table
+# of chosen boxes and zero box deltas, so the decoded boxes are the anchors and the exact IoU of
+# every pair is known.
+
+def _c_run(anchors, cls, C=1, nms_thr=0.25, max_num=4096, nms_pre=4096, sigmoid=1, dirc=None,
+           dir_offset=0.0, dir_limit_offset=0.0):
+    """dfm_box_post_forward on cls [B, ncol, 1, N] (zero box deltas, dirc [B, 2, 1, N] or zero
+    direction logits); returns the outputs per sample with the candidate / keep lists per
+    (sample, class) and 'topk' when the grid takes the top-k."""
+    L, p, s = capi.lib(), modules._ptr, modules._stream()
+    B, N = cls.shape[0], anchors.shape[0]
+    reg = torch.zeros((B, 7, 1, N), device='cuda')
+    if dirc is None:
+        dirc = torch.zeros((B, 2, 1, N), device='cuda')
+    desc = _desc(num_classes=C, num_anchors=1, ny=1, nx=N, batch=B, use_sigmoid=sigmoid,
+                 nms_pre=nms_pre, max_num=max_num, score_thr=0.1, nms_thr=nms_thr,
+                 dir_offset=dir_offset, dir_limit_offset=dir_limit_offset)
+    hd = ctypes.c_void_p()
+    host_anchors = anchors.cpu().contiguous()     # alive until create has copied it
+    capi.check(L.dfm_box_post_create(ctypes.byref(desc), p(host_anchors), ctypes.byref(hd)),
+               'create')
+    try:
+        boxes = torch.empty((B, max_num, 7), device='cuda')
+        scores = torch.empty((B, max_num), device='cuda')
+        labels = torch.empty((B, max_num), device='cuda', dtype=torch.int32)
+        count = torch.empty((B,), device='cuda', dtype=torch.int32)
+        capi.check(L.dfm_box_post_forward(hd, p(cls), p(reg), p(dirc), p(boxes), p(scores),
+                                          p(labels), p(count), s), 'forward')
+        K = min(N, nms_pre)
+        names = [(c, kind) for c in range(C) for kind in ('candidates', 'keep')]
+        names += ['topk'] if N > nms_pre else []
+        dbg = {}
+        for key in names:
+            t = torch.empty((B, K), device='cuda', dtype=torch.int32)
+            name = 'topk_index' if key == 'topk' else f'cls{key[0]}_{key[1]}'
+            capi.check(L.dfm_box_post_debug_tensor(hd, name.encode(), p(t), t.numel(), s),
+                       'debug')
+            dbg[key] = t
+        capi.sync_check()
+    finally:
+        L.dfm_box_post_destroy(hd)
+    out = []
+    for b in range(B):
+        k = int(count[b])
+        st = {key: v[b][v[b] >= 0].long() for key, v in dbg.items()}
+        out.append((boxes[b, :k], scores[b, :k], labels[b, :k].long(), st))
+    return out, reg, dirc
+
+
+def _c_vs_oracle(anchors, cls, C=1, nms_thr=0.25, sigmoid=True, exact_scores=True, **kw):
+    """Every sample's top-k and candidates equal the restatement's; so do its keep lists and
+    outputs unless a decision lies within EPS of nms_thr, where both keep lists must be valid
+    greedy NMS.  Softmax scores (exact_scores=False) may differ from torch's in the last bit.
+    Returns the C results and the number of such decisions."""
+    res, reg, dirc = _c_run(anchors, cls, C, nms_thr, sigmoid=int(sigmoid), **kw)
+    cfg = dict(nms_pre=kw.get('nms_pre', 4096), score_thr=0.1, nms_thr=nms_thr,
+               max_num=kw.get('max_num', 4096))
+    with torch.no_grad():
+        bev = BP.nms_box(BP.decode(anchors, torch.zeros_like(anchors)))
+    band = 0
+    for b, (boxes, scores, labels, st) in enumerate(res):
+        with torch.no_grad():
+            r = BP.get_bboxes_single(cls[b], reg[b], dirc[b], anchors, cfg, C, sigmoid,
+                                     kw.get('dir_offset', 0.0), kw.get('dir_limit_offset', 0.0))
+        if 'topk' in st:
+            assert torch.equal(st['topk'], r['topk']), b
+        same = True
+        for c in range(C):
+            cand, keep = st[c, 'candidates'], st[c, 'keep']
+            assert torch.equal(cand, r['candidates'][c]), (b, c)
+            near = _nms_validity(bev[cand], cand, keep, nms_thr)
+            band += near
+            if near == 0:
+                assert torch.equal(keep, r['keep'][c]), (b, c, len(keep), len(r['keep'][c]))
+            same &= torch.equal(keep, r['keep'][c])
+        if same:
+            assert torch.equal(labels, r['labels'])
+            if exact_scores:
+                assert torch.equal(scores, r['scores'])
+            else:
+                torch.testing.assert_close(scores, r['scores'], rtol=1e-6, atol=1e-7)
+            bad = torch.nonzero(~torch.isclose(boxes, r['boxes'], rtol=2.4e-7,
+                                               atol=1e-6).all(1)).flatten()
+            assert len(bad) == 0, (bad[:4].tolist(), boxes[bad[:4]].tolist(),
+                                   r['boxes'][bad[:4]].tolist())
+    return res, band
+
+
+def _along(yaw, du, dv):
+    """(du, dv) in a box's (w, h) axes under the NMS corner convention, as an (x, y) offset."""
+    c, s = math.cos(yaw), BP.NMS_ROTATED_ROT_SIGN * math.sin(yaw)
+    return du * c - dv * s, du * s + dv * c
+
+
+_ULP_STEPS = np.array([(i, j) for i in range(-8, 9) for j in range(-8, 9)], dtype=np.int32)
+
+
+def _collinear_grid(thr):
+    """Anchors [N, 7] and logits [N] of equal boxes offset along their own axis, so their long or
+    short edges lie on one line: pairs with exact IoU (side - s) / (side + s) between 0.0002
+    and 0.005 below or above nms_thr, and greedy chains A, B, C with IoU(A, B), IoU(B, C) above
+    nms_thr and IoU(A, C) below it (A suppresses B, so C is kept).  Each later box takes,
+    among the fp32 centres within 8 ulp of its offset, the one whose NMS box lies closest to
+    the first box's axis: the edges are collinear to within the corners' rounding.  900 groups 14 m apart, out
+    to 203 m; groups[g] lists each group's rows."""
+    rng = np.random.RandomState(int(thr * 100))
+    rows, logits, groups = [], [], []
+    gx = np.linspace(-203.0, 203.0, 30)
+    centres = [(x, y) for x in gx for y in gx]
+    rng.shuffle(centres)
+    for g, (x0, y0) in enumerate(centres):
+        yaw = float(rng.choice([0.0, math.pi / 2, math.pi / 4, -math.pi / 2]) if g % 4 == 0
+                    else rng.uniform(-6.0, 6.0))
+        w, l = rng.uniform(1.5, 2.2), rng.uniform(3.5, 5.0)
+        axis = rng.randint(2)
+        side = (w, l)[axis]
+        if g % 5 == 4:   # chain: step with IoU thr + 0.1 twice, two steps apart fall below thr
+            t = thr + 0.1
+            steps = (0.0, 1.0, 2.0)
+        else:
+            t = thr + rng.choice([-1.0, 1.0]) * rng.uniform(0.0002, 0.005)
+            steps = (0.0, 1.0)
+        sft = side * (1 - t) / (1 + t)
+        groups.append(list(range(len(rows), len(rows) + len(steps))))
+        ux, uy = _along(yaw, 1.0, 0.0) if axis == 0 else _along(yaw, 0.0, 1.0)
+        for k, m in enumerate(steps):
+            row = np.array([x0 + m * sft * ux, y0 + m * sft * uy, -1.0, w, l, 1.6, yaw],
+                           dtype=np.float32)
+            if k > 0:    # the fp32 centre whose NMS box lies closest to the first box's axis
+                cand = np.repeat(row[None], len(_ULP_STEPS), 0)
+                cand[:, :2] = (row[:2].view(np.int32) + _ULP_STEPS).view(np.float32)
+                bev = BP.nms_box(torch.from_numpy(cand)).double().numpy()
+                first = BP.nms_box(torch.from_numpy(np.array(rows[groups[-1][0]],
+                                                             dtype=np.float32)[None]))
+                d = bev[:, :2] - first.double().numpy()[:, :2]
+                row = cand[np.argmin(np.abs(d[:, 0] * uy - d[:, 1] * ux))]
+            rows.append(tuple(row.tolist()))
+            logits.append(3.0 - 0.5 * k - 1e-3 * g)
+    return (torch.tensor(rows, dtype=torch.float32), torch.tensor(logits, dtype=torch.float32),
+            groups)
+
+
+@pytest.mark.skipif(shutil.which('g++') is None, reason='no C++ compiler')
+@pytest.mark.parametrize('thr', [0.05, 0.25])
+def test_collinear_grid_flips_the_edge_clipping_iou(thr, tmp_path):
+    """The collinear grid below is one an fp32 edge-clipping (Green's theorem) IoU gets wrong:
+    on its NMS boxes (after the fp32 round trip) that IoU decides some pair the other way from
+    the exact IoU, so the GPU test can tell the two forms apart."""
+    from tests import test_rotated_iou as R
+    anchors, _, groups = _collinear_grid(thr)
+    bev = BP.nms_box(BP.decode(anchors, torch.zeros_like(anchors))).numpy()
+    pairs = [(g[0], g[1]) for g in groups if len(g) == 2]
+    a = np.ascontiguousarray(bev[[i for i, _ in pairs]])
+    b = np.ascontiguousarray(bev[[j for _, j in pairs]])
+    old = R.green_iou(a, b, tmp_path)
+    ex = np.array([R.exact_iou(x, y) for x, y in zip(a, b)])
+    assert bool((np.abs(ex - thr) >= 1.5e-4).all())
+    flips = int(((old > thr) != (ex > thr)).sum())
+    print('pairs', len(pairs), 'decisions flipped by the edge-clipping IoU', flips)
+    assert flips >= 2
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('thr', [0.05, 0.25])
+def test_collinear_duplicates_and_chains_vs_oracle(thr):
+    """The collinear grid through dfm_box_post_*: the keep lists must equal the
+    restatement's, with no decision within EPS of nms_thr."""
+    anchors, logits, groups = _collinear_grid(thr)
+    anchors, cls = anchors.cuda(), logits.cuda().view(1, 1, 1, -1)
+    ((_, _, _, st),), band = _c_vs_oracle(anchors, cls, nms_thr=thr)
+    assert band == 0
+    assert len(groups) < len(st[0, 'keep']) < len(anchors)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('n,nms_pre', [(300, 100), (101, 100), (100, 100)])
+def test_topk_ties_take_the_lowest_anchors(n, nms_pre):
+    """All logits equal: the top-k is the first nms_pre anchors by index (N = nms_pre + 1 drops
+    the last one; N = nms_pre takes no top-k at all)."""
+    rng = np.random.RandomState(n)
+    a = np.stack([rng.uniform(-60, 60, n), rng.uniform(-60, 60, n), np.full(n, -1.0),
+                  rng.uniform(1.5, 2.2, n), rng.uniform(3.5, 5.0, n), np.full(n, 1.6),
+                  rng.uniform(-math.pi, math.pi, n)], 1)
+    anchors = torch.tensor(a, dtype=torch.float32, device='cuda')
+    cls = torch.full((1, 1, 1, n), 1.5, device='cuda')
+    ((_, _, _, st),), _ = _c_vs_oracle(anchors, cls, nms_pre=nms_pre, max_num=500)
+    assert ('topk' in st) == (n > nms_pre)
+    if n > nms_pre:
+        assert torch.equal(st['topk'], torch.arange(nms_pre, device='cuda'))
+    assert torch.equal(st[0, 'candidates'], torch.arange(min(n, nms_pre), device='cuda'))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('sigmoid', [True, False])
+def test_sixteen_classes_vs_oracle(sigmoid):
+    """num_classes = 16 with sigmoid (16 columns) and with softmax (ncol = 17, background last)
+    on a crowded grid with top-k."""
+    rng = np.random.RandomState(16 + sigmoid)
+    n, C = 200, 16
+    a = np.stack([rng.uniform(-20, 20, n), rng.uniform(-20, 20, n), np.full(n, -1.0),
+                  rng.uniform(1.5, 2.2, n), rng.uniform(3.5, 5.0, n), np.full(n, 1.6),
+                  rng.uniform(-math.pi, math.pi, n)], 1)
+    anchors = torch.tensor(a, dtype=torch.float32, device='cuda')
+    ncol = C if sigmoid else C + 1
+    logits = rng.uniform(-4.0, 4.0, (ncol, n))
+    if not sigmoid:
+        logits[C] -= 2.0       # background: leave foreground scores above score_thr
+    cls = torch.tensor(logits, dtype=torch.float32, device='cuda').view(1, ncol, 1, n)
+    ((_, _, labels, st),), band = _c_vs_oracle(anchors, cls, C=C, sigmoid=sigmoid,
+                                               exact_scores=sigmoid, nms_pre=150, max_num=1000)
+    assert 'topk' in st
+    assert len(set(labels.tolist())) == C
+    print('sigmoid' if sigmoid else 'softmax', 'boxes', len(labels), 'band', band)
+
+
+@pytest.mark.gpu
+def test_max_num_cut_through_scores_equal_across_classes():
+    """Three classes with bit-equal scores on runs of anchors (the same logit in every class
+    column): the cut at max_num falls inside such a run, and the tie order (score descending,
+    then class, then keep rank) must equal the restatement's stable sort of the class-major
+    list."""
+    n, C = 120, 3
+    gx = np.arange(n) * 8.0 - 480.0           # 8 m apart: every box is kept in every class
+    a = np.stack([gx, np.zeros(n), np.full(n, -1.0), np.full(n, 1.8), np.full(n, 4.0),
+                  np.full(n, 1.6), np.zeros(n)], 1)
+    anchors = torch.tensor(a, dtype=torch.float32, device='cuda')
+    base = np.repeat(np.linspace(3.0, 1.0, 12), 10)          # runs of 10 equal logits
+    cls = torch.tensor(np.stack([base] * C), dtype=torch.float32,
+                       device='cuda').view(1, C, 1, n)
+    for max_num in (45, 95, 200):                             # 45, 95: inside a run of ties
+        ((_, scores, labels, st),), _ = _c_vs_oracle(anchors, cls, C=C, max_num=max_num)
+        assert len(labels) == min(max_num, n * C)
+        assert len(st[0, 'keep']) == n
+    assert int((scores == scores[0]).sum()) == C * 10
+
+
+@pytest.mark.gpu
+def test_yaw_fix_at_period_boundaries():
+    """Decoded yaws within a few ulp of dir_offset + k pi, where (yaw - dir_offset) / pi +
+    dir_limit_offset is within about one ulp of an integer, with both direction labels: the
+    boxes equal those of the restatement run on the CPU bit for bit (the kernel's yaw fix
+    divides by pi as torch's CPU path does)."""
+    off = syn.KITTI_DIR_OFFSET
+    yaws = []
+    for k in np.arange(-3.0, 3.5, 0.5):     # boundaries of dir_limit_offset 0 / 1 and 0.5
+        y = np.float32(off + k * math.pi)
+        for d in range(-3, 4):
+            yaws.append((y.view(np.int32) + d).view(np.float32) if y != 0 else y)
+    n = len(yaws)
+    a = np.stack([np.arange(n) * 8.0 - 4.0 * n, np.zeros(n), np.full(n, -1.0),
+                  np.full(n, 1.8), np.full(n, 4.0), np.full(n, 1.6), np.array(yaws)], 1)
+    anchors = torch.tensor(a, dtype=torch.float32)
+    logits = torch.linspace(3.0, 1.0, n).view(1, 1, 1, n)    # well apart: same order anywhere
+    dirc = torch.zeros((1, 2, 1, n))
+    dirc[0, 1, 0, 1::2] = 1.0                                  # label 1 on odd anchors
+    for limit in (0.0, 0.5, 1.0):
+        (got,), reg, _ = _c_run(anchors.cuda(), logits.cuda(), dirc=dirc.cuda(),
+                                dir_offset=off, dir_limit_offset=limit, max_num=500)
+        cfg = dict(nms_pre=4096, score_thr=0.1, nms_thr=0.25, max_num=500)
+        with torch.no_grad():
+            r = BP.get_bboxes_single(logits[0], reg[0].cpu(), dirc[0], anchors, cfg, 1, True,
+                                     off, limit)
+        assert torch.equal(got[2].cpu(), r['labels'])
+        assert torch.equal(got[0].cpu(), r['boxes']), (limit, (got[0].cpu() - r['boxes'])
+                                                       .abs().max(0)[0].tolist())
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('n', [1, 63, 64, 65, 127, 128, 4095, 4096])
+def test_candidate_counts_vs_oracle(n):
+    """n candidates of one class in a crowded 40 m square: the diagonal IoU tile, the row and
+    column blocks of the mask and the later words of the greedy sweep at the block edges.  Half
+    the anchors score below score_thr."""
+    rng = np.random.RandomState(n)
+    N = 2 * n
+    side = 40.0 * math.sqrt(N / 8192)
+    a = np.stack([rng.uniform(-side, side, N), rng.uniform(-side, side, N), np.full(N, -1.0),
+                  rng.uniform(1.5, 2.2, N), rng.uniform(3.5, 5.0, N), np.full(N, 1.6),
+                  rng.uniform(-math.pi, math.pi, N)], 1)
+    logits = rng.uniform(-1.0, 4.0, N)
+    logits[rng.permutation(N)[:n]] = -5.0
+    anchors = torch.tensor(a, dtype=torch.float32, device='cuda')
+    cls = torch.tensor(logits, dtype=torch.float32, device='cuda').view(1, 1, 1, -1)
+    ((_, _, _, st),), band = _c_vs_oracle(anchors, cls, nms_thr=0.25, nms_pre=min(N, 4096),
+                                          max_num=4096)
+    assert len(st[0, 'candidates']) == n
+    print('candidates', n, 'kept', len(st[0, 'keep']), 'decisions within EPS of nms_thr', band)
+
+
+@pytest.mark.gpu
+def test_batch_with_an_empty_sample_equals_single_samples():
+    """B = 2: sample 0 has no candidate, sample 1 has 4096; each equals its B = 1 run."""
+    rng = np.random.RandomState(5)
+    N = 4096
+    a = np.stack([rng.uniform(-40, 40, N), rng.uniform(-40, 40, N), np.full(N, -1.0),
+                  rng.uniform(1.5, 2.2, N), rng.uniform(3.5, 5.0, N), np.full(N, 1.6),
+                  rng.uniform(-math.pi, math.pi, N)], 1)
+    anchors = torch.tensor(a, dtype=torch.float32, device='cuda')
+    cls = torch.stack([torch.full((1, 1, N), -5.0),
+                       torch.tensor(rng.uniform(-1.0, 4.0, N), dtype=torch.float32)
+                       .view(1, 1, N)]).cuda()
+    both, _, _ = _c_run(anchors, cls, max_num=500)
+    assert len(both[0][0]) == 0 and len(both[1][3][0, 'candidates']) == N
+    for b in range(2):
+        (one,), _, _ = _c_run(anchors, cls[b:b + 1].contiguous(), max_num=500)
+        for u, v in zip(both[b][:3], one[:3]):
+            assert torch.equal(u, v)
+        for key in one[3]:
+            assert torch.equal(both[b][3][key], one[3][key])
+    _c_vs_oracle(anchors, cls[1:2].contiguous(), max_num=500)
+
+
 @pytest.mark.gpu
 def test_kitti_chain_end_to_end():
     """The real regressions of test_box_regression_parity_end_to_end's all-CUDA KITTI chain

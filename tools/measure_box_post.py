@@ -87,10 +87,15 @@ def main():
             n = [len(o[0]) for o in out]
             print(f'{name} {ny}x{nx} B={B}: C entry {c_ms:.3f} ms ({c_ms / B:.3f} ms/sample), '
                   f'module {m_ms:.3f} ms{o_txt}; boxes {n}', flush=True)
-    capi.profile_enable(True)
-    head.get_bboxes([cls], [box], [dirc], metas)
-    torch.cuda.synchronize()
-    print('per-stage (last shape):', capi.profile_report())
+            capi.profile_enable(True)
+            capi.profile_report()
+            for _ in range(args.iters):
+                c_call()
+            torch.cuda.synchronize()
+            rep = capi.profile_report()
+            capi.profile_enable(False)
+            print('  per-stage ms/call:', {k.split('@')[0]: round(v['ms'] / v['launches'], 4)
+                                           for k, v in rep.items()}, flush=True)
 
 
 if __name__ == '__main__':
