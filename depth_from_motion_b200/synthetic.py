@@ -75,6 +75,36 @@ def make_img_meta(h, w, sweep=2, flip=False, crop_offset=(0, 0), scale=1.0,
         scale_factor=[scale, scale, scale, scale])
 
 
+def kitti_p2_for_width(w):
+    """KITTI P2 with its focal lengths and principal point rescaled to an image w pixels wide
+    (w = 1248 keeps the whole lattice of a w-wide feature map inside the original field of
+    view at the demo sample's scale)."""
+    p = KITTI_P2.copy()
+    p[:2] *= w / 1248.0
+    return p
+
+
+def cur2prev_pose(yaw=0.0, pitch=0.0, t=(0.0, 0.0, 0.0)):
+    """A cur -> prev camera transform [4, 4] (camera axes: x right, y down, z forward):
+    rotation by `yaw` about y, then `pitch` about x (radians), then translation t (metres)."""
+    cy, sy = math.cos(yaw), math.sin(yaw)
+    cp, sp = math.cos(pitch), math.sin(pitch)
+    r_yaw = np.array([[cy, 0, sy], [0, 1, 0], [-sy, 0, cy]])
+    r_pitch = np.array([[1, 0, 0], [0, cp, -sp], [0, sp, cp]])
+    m = np.eye(4)
+    m[:3, :3] = r_pitch @ r_yaw
+    m[:3, 3] = t
+    return m
+
+
+def white_noise_pair(seed, c, h, w):
+    """relu(N(0, 1)) (cur, prev) feature maps [1, c, h, w] fp32: neighbouring pixels differ by
+    O(1), so a sample-coordinate error shows up undamped."""
+    rng = np.random.RandomState(seed)
+    return tuple(torch.from_numpy(rng.standard_normal((1, c, h, w)).astype(np.float32)).relu()
+                 for _ in range(2))
+
+
 def _kaiming(rng, shape, fan_in, gain=1.0):
     std = gain * math.sqrt(2.0 / fan_in)
     return (rng.standard_normal(shape) * std).astype(np.float32)
