@@ -181,10 +181,7 @@ def lib():
     L.dfm_profile_enable.argtypes = [c_int]
     L.dfm_profile_report.argtypes = [c_char_p, c_int]
     L.dfm_backbone_create.argtypes = [POINTER(BackboneDesc), POINTER(vp)]
-    L.dfm_backbone_destroy.argtypes = [vp]
-    L.dfm_backbone_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
     L.dfm_backbone_set_depths.argtypes = [vp, vp, c_int]
-    L.dfm_backbone_missing_params.argtypes = [vp]
     L.dfm_backbone_workspace_bytes.argtypes = [vp]
     L.dfm_backbone_workspace_bytes.restype = c_longlong
     L.dfm_backbone_forward.argtypes = [vp, vp, vp, POINTER(Geometry), vp, vp,
@@ -197,7 +194,6 @@ def lib():
     L.dfm_backbone_cost_device.restype = vp
     L.dfm_backbone_stereo_feat_device.argtypes = [vp]
     L.dfm_backbone_stereo_feat_device.restype = vp
-    L.dfm_backbone_debug_tensor.argtypes = [vp, c_char_p, vp, c_longlong, vp]
     L.dfm_op_build_cost_volume.argtypes = [vp, vp, c_int, c_int, c_int, vp,
                                            c_int, c_int, c_int,
                                            POINTER(Geometry), vp, vp]
@@ -211,16 +207,10 @@ def lib():
     L.dfm_multiview_lift_cl.argtypes = [POINTER(LiftDesc), vp, vp, vp, vp, vp, vp,
                                      vp, vp]
     L.dfm_neck_create.argtypes = [POINTER(NeckDesc), POINTER(vp)]
-    L.dfm_neck_destroy.argtypes = [vp]
-    L.dfm_neck_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
-    L.dfm_neck_missing_params.argtypes = [vp]
     L.dfm_neck_forward.argtypes = [vp, vp, vp, vp]
     L.dfm_neck_forward_cl.argtypes = [vp, vp, vp, vp]
     L.dfm_frustum_create.argtypes = [POINTER(FrustumDesc), vp, vp, vp,
                                      POINTER(vp)]
-    L.dfm_frustum_destroy.argtypes = [vp]
-    L.dfm_frustum_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
-    L.dfm_frustum_missing_params.argtypes = [vp]
     L.dfm_frustum_forward.argtypes = [vp, vp, c_int, vp, vp, vp, vp, vp,
                                       POINTER(c_double), c_int, c_int, vp, vp]
     L.dfm_pipeline_forward_host.argtypes = [vp, vp, vp, vp, vp, POINTER(Geometry),
@@ -230,53 +220,34 @@ def lib():
                                            POINTER(c_double), c_int, c_int, vp, vp, vp, vp]
     L.dfm_pipeline_wait.argtypes = [vp]
     L.dfm_bev_hourglass_create.argtypes = [POINTER(BevDesc), POINTER(vp)]
-    L.dfm_bev_hourglass_destroy.argtypes = [vp]
-    L.dfm_bev_hourglass_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
-    L.dfm_bev_hourglass_missing_params.argtypes = [vp]
     L.dfm_bev_hourglass_forward.argtypes = [vp, vp, vp, vp, vp]
     L.dfm_anchor_head_create.argtypes = [POINTER(AnchorHeadDesc), POINTER(vp)]
-    L.dfm_anchor_head_destroy.argtypes = [vp]
-    L.dfm_anchor_head_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
-    L.dfm_anchor_head_missing_params.argtypes = [vp]
     L.dfm_anchor_head_forward.argtypes = [vp, vp, vp, vp, vp, vp]
     L.dfm_anchor3d_head_create.argtypes = [POINTER(Anchor3DHeadDesc), POINTER(vp)]
-    L.dfm_anchor3d_head_destroy.argtypes = [vp]
-    L.dfm_anchor3d_head_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
-    L.dfm_anchor3d_head_missing_params.argtypes = [vp]
     L.dfm_anchor3d_head_forward.argtypes = [vp, vp, vp, vp, vp, vp]
     L.dfm_backbone_forward_cl.argtypes = [vp, vp, vp, POINTER(Geometry), vp, vp, vp, vp]
     L.dfm_stereo_tail_create.argtypes = [c_int, c_int, c_int, POINTER(vp)]
-    L.dfm_stereo_tail_destroy.argtypes = [vp]
-    L.dfm_stereo_tail_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
-    L.dfm_stereo_tail_missing_params.argtypes = [vp]
     L.dfm_stereo_tail_forward.argtypes = [vp, vp, vp, vp, vp]
     L.dfm_spp_neck_create.argtypes = [c_int, c_int, c_int, POINTER(vp)]
-    L.dfm_spp_neck_destroy.argtypes = [vp]
-    L.dfm_spp_neck_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
-    L.dfm_spp_neck_missing_params.argtypes = [vp]
     L.dfm_spp_neck_forward.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.dfm_fpn_create.argtypes = [POINTER(FpnDesc), POINTER(vp)]
-    L.dfm_fpn_destroy.argtypes = [vp]
-    L.dfm_fpn_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
-    L.dfm_fpn_missing_params.argtypes = [vp]
     L.dfm_fpn_forward.argtypes = [vp, POINTER(vp), POINTER(vp), vp]
     L.dfm_liga_resnet_create.argtypes = [POINTER(LigaResNetDesc), POINTER(vp)]
-    L.dfm_liga_resnet_destroy.argtypes = [vp]
-    L.dfm_liga_resnet_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
-    L.dfm_liga_resnet_missing_params.argtypes = [vp]
     L.dfm_liga_resnet_forward.argtypes = [vp, vp, POINTER(vp), vp]
     L.dfm_resnet101_create.argtypes = [POINTER(ResNet101Desc), POINTER(vp)]
-    L.dfm_resnet101_destroy.argtypes = [vp]
-    L.dfm_resnet101_set_param.argtypes = [vp, c_char_p, vp, c_longlong]
-    L.dfm_resnet101_missing_params.argtypes = [vp]
     L.dfm_resnet101_forward.argtypes = [vp, vp, POINTER(vp), vp]
-    for f in ('neck', 'frustum', 'bev_hourglass', 'anchor_head', 'spp_neck', 'fpn',
-              'liga_resnet', 'resnet101'):
+    # the parameterised handle families share destroy / set_param / missing_params
+    for f in ('backbone', 'neck', 'frustum', 'bev_hourglass', 'anchor_head', 'anchor3d_head',
+              'stereo_tail', 'spp_neck', 'fpn', 'liga_resnet', 'resnet101'):
+        getattr(L, f'dfm_{f}_destroy').argtypes = [vp]
+        getattr(L, f'dfm_{f}_set_param').argtypes = [vp, c_char_p, vp, c_longlong]
+        getattr(L, f'dfm_{f}_missing_params').argtypes = [vp]
+    for f in ('backbone', 'neck', 'frustum', 'bev_hourglass', 'anchor_head', 'spp_neck', 'fpn',
+              'liga_resnet', 'resnet101', 'box_post'):
         getattr(L, f'dfm_{f}_debug_tensor').argtypes = [vp, c_char_p, vp, c_longlong, vp]
     L.dfm_box_post_create.argtypes = [POINTER(BoxPostDesc), vp, POINTER(vp)]
     L.dfm_box_post_destroy.argtypes = [vp]
     L.dfm_box_post_forward.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp]
-    L.dfm_box_post_debug_tensor.argtypes = [vp, c_char_p, vp, c_longlong, vp]
     L.dfm_op_rotated_iou.argtypes = [vp, vp, c_int, vp, vp]
     L.dfm_voxel_sample.argtypes = [POINTER(VoxelSampleDesc), vp, vp, POINTER(c_double), vp, vp]
     _lib = L

@@ -16,11 +16,63 @@ inline int cur_device() {
   cudaGetDevice(&dev);
   return dev >= 0 && dev < kMaxDevices ? dev : 0;
 }
+// The slots are never destroyed: freeing device memory during static destruction could run
+// after the CUDA runtime has torn down its context.
 template <class T, int TAG = 0>
 inline T& per_device() {
-  static T slots[kMaxDevices];
+  static T* slots = new T[kMaxDevices]();  // value-initialised, as a static array would be
   return slots[cur_device()];
 }
+
+// Sole owner of one device allocation of n elements: move-only, freed by the destructor.
+// alloc is grow-only: it keeps the allocation when that already holds `count` elements.
+template <class T>
+struct DevArray {
+  T* p = nullptr;
+  size_t n = 0;
+
+  DevArray() = default;
+  DevArray(const DevArray&) = delete;
+  DevArray& operator=(const DevArray&) = delete;
+  DevArray(DevArray&& o) noexcept : p(o.p), n(o.n) {
+    o.p = nullptr;
+    o.n = 0;
+  }
+  DevArray& operator=(DevArray&& o) noexcept {
+    if (this != &o) {
+      release();
+      p = o.p;
+      n = o.n;
+      o.p = nullptr;
+      o.n = 0;
+    }
+    return *this;
+  }
+  ~DevArray() { release(); }
+
+  cudaError_t alloc(size_t count) {
+    if (p && n >= count) return cudaSuccess;
+    release();
+    const cudaError_t e = cudaMalloc(&p, count * sizeof(T));
+    if (e != cudaSuccess) {
+      p = nullptr;
+      return e;
+    }
+    n = count;
+    return cudaSuccess;
+  }
+  // alloc + a synchronous copy of `count` host elements
+  cudaError_t upload(const T* h, size_t count) {
+    cudaError_t e = alloc(count);
+    if (e == cudaSuccess) e = cudaMemcpy(p, h, count * sizeof(T), cudaMemcpyHostToDevice);
+    return e;
+  }
+  void release() {
+    if (p) cudaFree(p);
+    p = nullptr;
+    n = 0;
+  }
+};
 
 // One additive term of a layer input, read from a channels-last fp32 tensor
 // [D][H][W][C]:  term(c) = act(x * scale[c] + shift[c]).  scale == nullptr means the

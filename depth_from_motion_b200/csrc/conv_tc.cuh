@@ -238,16 +238,13 @@ inline void tc_build_program(int ptype, int Cin, int ncta, uint32_t* w_cursor, T
 }
 
 struct TcWeights {
-  uint8_t* dev = nullptr;  // [nsplit][image bytes]
+  DevArray<uint8_t> dev;  // [nsplit][image bytes]
   int Cin = 0, Cout = 0, ncta = 0, nsplit = 0, mode = -1, kslice = 0;
   uint32_t image_bytes = 0, hi_bytes = 0;
   TcProgram prog[2];
 
-  bool ready() const { return dev != nullptr; }
-  void release() {
-    if (dev) cudaFree(dev);
-    dev = nullptr;
-  }
+  bool ready() const { return dev.p != nullptr; }
+  void release() { dev.release(); }
   // packed: [27][Cin][Cout] fp32 (tap = kz*9 + ky*3 + kx; transposed weights are
   // already in "o = 2i - 1 + k" orientation)
   // kslice: the CTA groups split the *input* channels (16 per group) and each covers all
@@ -290,8 +287,7 @@ struct TcWeights {
                   img[off + hi_bytes / 2] = lo;
                 }
         }
-    if (cudaMalloc(&dev, img.size() * 2) != cudaSuccess ||
-        cudaMemcpy(dev, img.data(), img.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) {
+    if (dev.upload(reinterpret_cast<const uint8_t*>(img.data()), img.size() * 2) != cudaSuccess) {
       if (err) *err = "TcWeights: device upload failed";
       release();
       return false;
@@ -1326,7 +1322,7 @@ bool tc_launch(const Loader& ld, const TcWeights& w, float* out, double* stats,
   }
   const int sms = tc_sm_count();
   TcParams p{};
-  p.wimg = w.dev;
+  p.wimg = w.dev.p;
   p.out = out;
   p.stats = stats;
   p.store1 = opt.store1;

@@ -64,14 +64,11 @@ inline int nk_zmode(const ConvGeom& g) {
 }
 
 struct NeckTcWeights {
-  uint8_t* dev = nullptr;  // [nsplit][ncg][NK_W_BYTES]
+  DevArray<uint8_t> dev;   // [nsplit][ncg][NK_W_BYTES]
   int Cin = 0, Cout = 0, zmode = -1;
   int cg = 32;             // input channels per group (32 -> NCTA 32, 16 -> NCTA 64)
-  bool ready() const { return dev != nullptr; }
-  void release() {
-    if (dev) cudaFree(dev);
-    dev = nullptr;
-  }
+  bool ready() const { return dev.p != nullptr; }
+  void release() { dev.release(); }
   // packed: [27][Cin][Cout] fp32, tap = kz*9 + ky*3 + kx with (kz,ky,kx) over (Nz, Ny, Nx)...
   // NOTE the conv dims are (D,H,W) = (Nx, Ny, Nz): the packed tap index is kd*9 + kh*3 + kw,
   // i.e. kd over Nx, kh over Ny, kw over Nz (the short, marched axis).
@@ -113,8 +110,7 @@ struct NeckTcWeights {
                 img[off + NK_WHI_BYTES / 2] = lo;
               }
         }
-    if (cudaMalloc(&dev, img.size() * 2) != cudaSuccess ||
-        cudaMemcpy(dev, img.data(), img.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) {
+    if (dev.upload(reinterpret_cast<const uint8_t*>(img.data()), img.size() * 2) != cudaSuccess) {
       if (err) *err = "NeckTcWeights: device upload failed";
       release();
       return false;
@@ -543,7 +539,7 @@ inline int neck_group_for(int cin, int cout, int planes, bool windowed = false) 
 inline bool neck_tc_conv(const Src& s, const NeckTcWeights& w, float* out, const ConvGeom& g,
                          cudaStream_t st, std::string* err) {
   NeckParams p{};
-  p.wimg = w.dev;
+  p.wimg = w.dev.p;
   p.out = out;
   p.src = s;
   p.Nx = g.Di; p.Ny = g.Hi; p.Zi = g.Wi; p.Zo = g.Wo;
@@ -631,7 +627,7 @@ inline bool neck_tc_conv_dhw(const Src& s, const NeckTcWeights& w, float* out, c
                              double* stats, int zw_lo, int zw_hi, float zw, cudaStream_t st,
                              std::string* err) {
   NeckParams p{};
-  p.wimg = w.dev;
+  p.wimg = w.dev.p;
   p.out = out;
   p.src = s;
   p.Nx = g.Hi; p.Ny = g.Wi; p.Zi = g.Di; p.Zo = g.Do;

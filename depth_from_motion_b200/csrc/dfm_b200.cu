@@ -8,6 +8,7 @@
 #include <cmath>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <set>
 #include <string>
 #include <vector>
@@ -113,24 +114,35 @@ std::string neck_class(const char* kind, const dfm::ConvGeom& g, const dfm::Neck
          std::to_string(g.Ho) + "x" + std::to_string(g.Wo);
 }
 
-struct DevBuf {
-  float* p = nullptr;
-  size_t n = 0;
+// Grow-only fp32 device buffer of the handles.  Its alloc returns a DFM_* code (a failure is
+// DFM_ERR_CUDA with the message set), unlike DevArray::alloc / upload, which return the
+// cudaError_t; upload() below is the DFM_* counterpart of DevArray::upload.
+struct DevBuf : dfm::DevArray<float> {
   int alloc(size_t count) {
-    if (p && n >= count) return DFM_OK;
-    if (p) cudaFree(p);
-    p = nullptr;
-    n = 0;
-    CU_TRY(cudaMalloc(&p, count * sizeof(float)));
-    n = count;
+    CU_TRY(DevArray::alloc(count));
     return DFM_OK;
   }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    n = 0;
-  }
 };
+
+// every handle's create: the kernels are built for sm_90a only
+int require_sm90() {
+  int maj = 0;
+  DFM_TRY(dfm_device_info(nullptr, &maj, nullptr, nullptr));
+  if (maj != 9) return fail(DFM_ERR_NOGPU, "this library is built for sm_90a only");
+  return DFM_OK;
+}
+
+// every handle's forward: refuse to run after a tensor-core kernel timed out, or with
+// parameters missing (the message names the first missing key in sorted order)
+int forward_prologue(const std::set<std::string>& missing) {
+  if (dfm::tc_consume_error())
+    return fail(DFM_ERR_CUDA, "an earlier tensor-core conv kernel timed out on an mbarrier "
+                              "hand-over: its outputs were invalid");
+  if (!missing.empty())
+    return fail(DFM_ERR_STATE, "missing parameter: " + *missing.begin() + " (+" +
+                                   std::to_string(missing.size() - 1) + " more)");
+  return DFM_OK;
+}
 
 // Test hooks of the downstream handles (dfm_neck_debug_tensor, ...): copies the `written`
 // floats the last forward left in `b`.  written == 0: that forward did not write the tensor.
@@ -149,11 +161,11 @@ int debug_copy(const DevBuf& b, long long written, const std::string& name, floa
 struct Norm {  // GroupNorm (statistics computed per frame) or folded BatchNorm (static)
   int C = 0;
   DevBuf gamma, beta, scale, shift;
-  double* sums = nullptr;
+  dfm::DevArray<double> sums;
   bool sums_clean = false;  // gn_finalize_kernel left the sums zeroed and nothing touched them since
   // call before launching kernels that accumulate into `sums`
   int begin_stats(cudaStream_t st) {
-    if (!sums_clean) CU_TRY(cudaMemsetAsync(sums, 0, 2 * C * sizeof(double), st));
+    if (!sums_clean) CU_TRY(cudaMemsetAsync(sums.p, 0, 2 * C * sizeof(double), st));
     sums_clean = false;
     return DFM_OK;
   }
@@ -163,16 +175,8 @@ struct Norm {  // GroupNorm (statistics computed per frame) or folded BatchNorm 
     DFM_TRY(beta.alloc(c));
     DFM_TRY(scale.alloc(c));
     DFM_TRY(shift.alloc(c));
-    CU_TRY(cudaMalloc(&sums, 2 * c * sizeof(double)));
+    CU_TRY(sums.alloc(2 * c));
     return DFM_OK;
-  }
-  void release() {
-    gamma.release();
-    beta.release();
-    scale.release();
-    shift.release();
-    if (sums) cudaFree(sums);
-    sums = nullptr;
   }
 };
 
@@ -323,8 +327,8 @@ int conv_simt_dispatch(const L& ld, const ConvW& w, float* out, const dfm::ConvG
 }
 
 int gn_finalize(Norm& n, long long V, int groups, cudaStream_t st) {
-  dfm::gn_finalize_kernel<<<1, 256, 0, st>>>(n.sums, n.gamma.p, n.beta.p, n.C, groups, (double)V,
-                                           1e-5f, n.scale.p, n.shift.p);
+  dfm::gn_finalize_kernel<<<1, 256, 0, st>>>(n.sums.p, n.gamma.p, n.beta.p, n.C, groups,
+                                           (double)V, 1e-5f, n.scale.p, n.shift.p);
   LAUNCH_CHECK();
   n.sums_clean = true;
   return DFM_OK;
@@ -334,9 +338,9 @@ int run_gn(const float* raw, long long V, Norm& n, int groups, cudaStream_t st) 
   DFM_TRY(n.begin_stats(st));
   const int blocks = (int)std::min<long long>(8LL * dfm::tc_sm_count(), (V * n.C + 255) / 256);
   if (n.C == 32)
-    dfm::channel_stats_kernel<32><<<blocks, 256, 0, st>>>(raw, V, n.sums);
+    dfm::channel_stats_kernel<32><<<blocks, 256, 0, st>>>(raw, V, n.sums.p);
   else if (n.C == 64)
-    dfm::channel_stats_kernel<64><<<blocks, 256, 0, st>>>(raw, V, n.sums);
+    dfm::channel_stats_kernel<64><<<blocks, 256, 0, st>>>(raw, V, n.sums.p);
   else
     return fail(DFM_ERR_INVALID, "GroupNorm: unsupported channel count");
   LAUNCH_CHECK();
@@ -368,7 +372,7 @@ int run_conv_impl(const L& simt_loader, TCFN tc_fn, const char* loader_name, con
       // K-sliced launches carry their own tag: they also run the slice-reduce kernel
       ProfScope ps(conv_class(w.tc.kslice ? "conv_tc_ks" : "conv_tc", g, loader_name),
                    conv_flops(g), st);
-      if (!tc_fn(gn ? gn->sums : nullptr, &err)) return fail(DFM_ERR_CUDA, err);
+      if (!tc_fn(gn ? gn->sums.p : nullptr, &err)) return fail(DFM_ERR_CUDA, err);
     }
     g_launches.fetch_add(w.tc.kslice ? 2 : 1);  // K-slice convs run a slice-reduce kernel too
     g_tc_launches.fetch_add(1);
@@ -396,7 +400,7 @@ int run_conv(const dfm::Src& s, const ConvW& w, float* out, const dfm::ConvGeom&
     {
       std::string err;
       ProfScope ps(conv_class("conv_tck", g, "src"), conv_flops(g), st);
-      if (!dfm::neck_tc_conv_dhw(s, w.ntk, out, g, gn ? gn->sums : nullptr, zw.lo, zw.hi, zw.w,
+      if (!dfm::neck_tc_conv_dhw(s, w.ntk, out, g, gn ? gn->sums.p : nullptr, zw.lo, zw.hi, zw.w,
                                  st, &err))
         return fail(DFM_ERR_CUDA, err);
     }
@@ -438,7 +442,7 @@ int run_conv_presplit(const dfm::Src& s, DevBuf& ps, const ConvW& w, float* out,
     o.zw_hi = zw.hi;
     o.zw = zw.w;
     if (!dfm::tc_conv_presplit(reinterpret_cast<const uint4*>(ps.p), g.Cin, w.tc, out,
-                               gn ? gn->sums : nullptr, g, st, &err, o))
+                               gn ? gn->sums.p : nullptr, g, st, &err, o))
       return fail(DFM_ERR_CUDA, err);
   }
   g_launches.fetch_add(2);  // conv + slice reduce
@@ -598,6 +602,10 @@ struct dfm_backbone {
     cudaEvent_t consumed = nullptr;  // recorded after the last kernel that reads this slot
                                      // (asynchronous pipeline: a later prefetch waits for it)
     unsigned long long tick = 0;
+    ~HostStage() {
+      if (ready) cudaEventDestroy(ready);
+      if (consumed) cudaEventDestroy(consumed);
+    }
   } stage[2];
   unsigned long long stage_tick = 0;
   // grow-only device scratch of the host-buffer entry points (no cudaMalloc per call)
@@ -655,21 +663,6 @@ int tower_alloc(Tower& t, int D, int Ho, int Wo, int cv) {
   DFM_TRY(t.gc6.init(cv));
   DFM_TRY(t.gp0.init(cv));
   return DFM_OK;
-}
-
-void tower_release(Tower& t) {
-  for (DevBuf* b : {&t.raw0, &t.raw1, &t.b1, &t.b2, &t.b3, &t.b4, &t.b5, &t.b6, &t.cur, &t.p0b,
-                    &t.logit, &t.p1w, &t.cls5, &t.cls3, &t.ps0, &t.ps2})
-    b->release();
-  for (Norm* n : {&t.g0, &t.g1, &t.gc1, &t.gc2, &t.gc3, &t.gc4, &t.gc5, &t.gc6, &t.gp0})
-    n->release();
-  for (ConvW* c : {&t.dres0, &t.dres1, &t.c1, &t.c2, &t.c3, &t.c4, &t.c5, &t.c6, &t.p0, &t.p1tc,
-                   &t.d0cur, &t.d0prev}) {
-    c->simt.release();
-    c->tc.release();
-    c->ntk.release();
-  }
-  t.p1q.release();
 }
 
 std::vector<std::string> tower_param_names(bool mono) {
@@ -831,7 +824,7 @@ int tower_forward(dfm_backbone* bb, Tower& t, bool mono, const dfm::WarpLoader& 
       // three planes 1 : Dfull-2 : 1
       DFM_TRY(t.g0.begin_stats(st));
       dfm::channel_stats_zcls_kernel<32><<<dim3(296, 3), 256, 0, st>>>(t.cls3.p, Ho * Wo, Dfull,
-                                                                    t.g0.sums);
+                                                                    t.g0.sums.p);
       LAUNCH_CHECK();
       DFM_TRY(gn_finalize(t.g0, (long long)Dfull * Ho * Wo, 32, st));
       T0 = term(t.cls3, &t.g0, 1, D);  // first / interior / last plane of the computed volume
@@ -1039,28 +1032,20 @@ int dfm_backbone_create(const dfm_backbone_desc_t* desc, dfm_backbone_t** out) {
                 "adds conv5 output to conv2 output, conv_modules.py:145)");
   if ((Ho - 1) * csf > desc->feat_h - 1 || (Wo - 1) * csf > desc->feat_w - 1)
     return fail(DFM_ERR_INVALID, "feature size not compatible with cost_sample_factor");
-  int sm = 0, maj = 0, mnr = 0;
-  DFM_TRY(dfm_device_info(&sm, &maj, &mnr, nullptr));
-  if (maj != 9) return fail(DFM_ERR_NOGPU, "this library is built for sm_90a only");
-  dfm_backbone* bb = new dfm_backbone();
+  DFM_TRY(require_sm90());
+  std::unique_ptr<dfm_backbone> bb(new dfm_backbone());
   bb->d = *desc;
   bb->D = D;
   bb->Ho = Ho;
   bb->Wo = Wo;
   const size_t HW = (size_t)desc->feat_h * desc->feat_w;
-  int rc = DFM_OK;
-  auto chk = [&](int r) { if (rc == DFM_OK) rc = r; };
-  chk(bb->cur_nhwc.alloc(HW * desc->in_channels));
-  chk(bb->prev_nhwc.alloc(HW * desc->in_channels));
-  chk(bb->depths.alloc(D));
-  chk(bb->wagg.alloc((size_t)D * 2 * D));
-  chk(bb->cost.alloc((size_t)D * Ho * Wo));
-  chk(tower_alloc(bb->st, D, Ho, Wo, desc->cv_channels));
-  chk(tower_alloc(bb->mo, D, Ho, Wo, desc->cv_channels));
-  if (rc != DFM_OK) {
-    dfm_backbone_destroy(bb);
-    return rc;
-  }
+  DFM_TRY(bb->cur_nhwc.alloc(HW * desc->in_channels));
+  DFM_TRY(bb->prev_nhwc.alloc(HW * desc->in_channels));
+  DFM_TRY(bb->depths.alloc(D));
+  DFM_TRY(bb->wagg.alloc((size_t)D * 2 * D));
+  DFM_TRY(bb->cost.alloc((size_t)D * Ho * Wo));
+  DFM_TRY(tower_alloc(bb->st, D, Ho, Wo, desc->cv_channels));
+  DFM_TRY(tower_alloc(bb->mo, D, Ho, Wo, desc->cv_channels));
   for (bool mono : {false, true})
     for (const std::string& n : tower_param_names(mono)) bb->missing.insert(n);
   bb->missing.insert("aggregate_cost.weight");
@@ -1080,7 +1065,7 @@ int dfm_backbone_create(const dfm_backbone_desc_t* desc, dfm_backbone_t** out) {
     bb->dbg["p0" + s] = {&t.p0b, nullptr};
     bb->dbg["logit" + s] = {&t.logit, nullptr};
   }
-  *out = bb;
+  *out = bb.release();
   return DFM_OK;
 }
 
@@ -1088,17 +1073,6 @@ void pipeline_forget(const dfm_backbone* bb);  // pipeline_api.inc
 int dfm_backbone_destroy(dfm_backbone_t* bb) {
   if (!bb) return DFM_OK;
   pipeline_forget(bb);
-  tower_release(bb->st);
-  tower_release(bb->mo);
-  for (DevBuf* b : {&bb->cur_nhwc, &bb->prev_nhwc, &bb->depths, &bb->wagg, &bb->waggT, &bb->cost,
-                    &bb->volume_dbg, &bb->stage[0].cur, &bb->stage[0].prev, &bb->stage[1].cur,
-                    &bb->stage[1].prev, &bb->out_st, &bb->out_mo, &bb->pipe_sem, &bb->pipe_vox,
-                    &bb->pipe_preds, &bb->pipe_samples})
-    b->release();
-  for (auto& hs : bb->stage) {
-    if (hs.ready) cudaEventDestroy(hs.ready);
-    if (hs.consumed) cudaEventDestroy(hs.consumed);
-  }
   delete bb;
   return DFM_OK;
 }
@@ -1164,12 +1138,7 @@ int backbone_forward_impl(dfm_backbone_t* bb, const float* d_cur, const float* d
                           float* d_mono, void* stream, cudaEvent_t prev_ready,
                           bool channels_last = false) {
   if (!bb || !d_cur || !d_prev || !geom) return fail(DFM_ERR_INVALID, "null argument");
-  if (dfm::tc_consume_error())
-    return fail(DFM_ERR_CUDA, "an earlier tensor-core conv kernel timed out on an mbarrier "
-                              "hand-over: its outputs were invalid");
-  if (!bb->missing.empty())
-    return fail(DFM_ERR_STATE, "missing parameter: " + *bb->missing.begin() + " (+" +
-                                   std::to_string(bb->missing.size() - 1) + " more)");
+  DFM_TRY(forward_prologue(bb->missing));
   if (!bb->depths_set) return fail(DFM_ERR_STATE, "downsampled_depth not set");
   cudaStream_t st = (cudaStream_t)stream;
   ProfScope ps_all("backbone_forward_total", 0.0, st);
@@ -1501,9 +1470,6 @@ int dfm_op_build_cost_volume(const float* d_cur, const float* d_prev, int C, int
   dfm::cost_volume_kernel<<<grid, 256, 0, st>>>(wl, D, Ho, Wo, d_volume);
   LAUNCH_CHECK();
   CU_TRY(cudaStreamSynchronize(st));
-  cur.release();
-  prev.release();
-  dep.release();
   return DFM_OK;
 }
 
@@ -1562,12 +1528,6 @@ int dfm_op_conv3d(const float* d_x, int Cin, int Di, int Hi, int Wi, const float
   }
   if (rc == DFM_OK) rc = to_ncdhw(yout.p, d_y, Cout, Vo, st);
   cudaError_t e = cudaStreamSynchronize(st);
-  xin.release();
-  yout.release();
-  w.simt.release();
-  w.tc.release();
-  w.ntc.release();
-  w.ntk.release();
   if (rc == DFM_OK && e != cudaSuccess) rc = fail(DFM_ERR_CUDA, cudaGetErrorString(e));
   if (rc == DFM_OK && dfm::tc_consume_error())
     rc = fail(DFM_ERR_CUDA, "tensor-core conv kernel: mbarrier hand-over timed out");

@@ -237,19 +237,14 @@ head1x1_tc_kernel(const __grid_constant__ Head1x1Params p) {
 
 // Device images of the combined 1x1 conv: hi + lo bf16 weights and the fp32 bias.
 struct Head1x1Weights {
-  uint8_t* wimg = nullptr;
-  float* bias = nullptr;
+  DevArray<uint8_t> wimg;
+  DevArray<float> bias;
   int cin = 0, n = 0, np = 0;
-  bool ready() const { return wimg != nullptr; }
-  void release() {
-    if (wimg) cudaFree(wimg);
-    if (bias) cudaFree(bias);
-    wimg = nullptr;
-    bias = nullptr;
-  }
+  bool ready() const { return wimg.p != nullptr; }
   // w: [n][cin] rows (cls | dir | reg), b: [n]
   bool build(const float* w, const float* b, int cin_, int n_, std::string* err) {
-    release();
+    wimg.release();
+    bias.release();
     cin = cin_;
     n = n_;
     np = head1x1_np(n);
@@ -267,13 +262,13 @@ struct Head1x1Weights {
       }
     std::vector<float> bp(np, 0.f);
     std::copy(b, b + n, bp.begin());
-    if (cudaMalloc(&wimg, img.size() * 2) != cudaSuccess ||
-        cudaMemcpy(wimg, img.data(), img.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess ||
-        cudaMalloc(&bias, np * sizeof(float)) != cudaSuccess ||
-        cudaMemcpy(bias, bp.data(), np * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) {
+    if (wimg.upload(reinterpret_cast<const uint8_t*>(img.data()), img.size() * 2) !=
+            cudaSuccess ||
+        bias.upload(bp.data(), np) != cudaSuccess) {
       cudaGetLastError();
       if (err) *err = "head1x1_tc: weight upload failed";
-      release();
+      wimg.release();
+      bias.release();
       return false;
     }
     return true;
@@ -290,8 +285,8 @@ inline bool head1x1_tc_launch(const Head1x1Weights& w, const float* x, long long
   }
   Head1x1Params p{};
   p.x = x;
-  p.wimg = w.wimg;
-  p.bias = w.bias;
+  p.wimg = w.wimg.p;
+  p.bias = w.bias.p;
   for (int o = 0; o < 3; ++o) {
     p.out[o] = out[o];
     p.rows[o] = rows[o];

@@ -223,18 +223,13 @@ logits_tc_kernel(const __grid_constant__ LogitsTcParams p, const SrcLoader8<1> l
 }
 
 struct LogitsTcWeights {
-  uint8_t* dev = nullptr;
-  bool ready() const { return dev != nullptr; }
-  void release() {
-    if (dev) cudaFree(dev);
-    dev = nullptr;
-  }
+  DevArray<uint8_t> dev;
+  bool ready() const { return dev.p != nullptr; }
   bool build(const float* w /*[27][32]*/) {
-    release();
+    dev.release();
     std::vector<uint16_t> img;
     logits_tc_pack(w, img);
-    return cudaMalloc(&dev, LT_W_BYTES) == cudaSuccess &&
-           cudaMemcpy(dev, img.data(), LT_W_BYTES, cudaMemcpyHostToDevice) == cudaSuccess;
+    return dev.upload(reinterpret_cast<const uint8_t*>(img.data()), LT_W_BYTES) == cudaSuccess;
   }
 };
 
@@ -242,7 +237,7 @@ inline bool logits_tc_launch(const Src& s, const LogitsTcWeights& w, float* out,
                              int W, cudaStream_t st) {
   if (s.n != 1 || s.outer_relu || !w.ready()) return false;
   LogitsTcParams p{};
-  p.wimg = w.dev;
+  p.wimg = w.dev.p;
   p.out = out;
   p.D = D; p.H = H; p.W = W;
   p.tiles_x = (W + LT_OX - 1) / LT_OX;
