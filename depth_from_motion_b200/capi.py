@@ -55,8 +55,10 @@ SYMBOLS = (
     'dfm_resnet101_create', 'dfm_resnet101_destroy', 'dfm_resnet101_set_param',
     'dfm_resnet101_missing_params', 'dfm_resnet101_forward', 'dfm_resnet101_debug_tensor',
     'dfm_box_post_create', 'dfm_box_post_destroy', 'dfm_box_post_forward',
-    'dfm_box_post_debug_tensor', 'dfm_op_rotated_iou',
+    'dfm_box_post_debug_tensor', 'dfm_op_rotated_iou', 'dfm_image_prep',
 )
+
+DFM_IMAGE_PREP_CROP, DFM_IMAGE_PREP_RESCALE = 0, 1
 
 
 class Geometry(ctypes.Structure):
@@ -143,6 +145,13 @@ class BoxPostDesc(ctypes.Structure):
     _fields_ = [(n, c_int) for n in ('num_classes', 'num_anchors', 'ny', 'nx', 'batch',
                                      'use_sigmoid', 'nms_pre', 'max_num')] + \
                [(n, c_float) for n in ('score_thr', 'nms_thr', 'dir_offset', 'dir_limit_offset')]
+
+
+class ImagePrepDesc(ctypes.Structure):
+    """``dfm_image_prep_desc_t``."""
+    _fields_ = [(n, c_int) for n in ('mode', 'num_views', 'src_h', 'src_w', 'crop_x', 'crop_y',
+                                     'out_h', 'out_w', 'pad_divisor', 'to_rgb')] + \
+               [('mean', c_double * 3), ('std', c_double * 3)]
 
 
 class VoxelSampleDesc(ctypes.Structure):
@@ -250,6 +259,7 @@ def lib():
     L.dfm_box_post_forward.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.dfm_op_rotated_iou.argtypes = [vp, vp, c_int, vp, vp]
     L.dfm_voxel_sample.argtypes = [POINTER(VoxelSampleDesc), vp, vp, POINTER(c_double), vp, vp]
+    L.dfm_image_prep.argtypes = [POINTER(ImagePrepDesc), vp, vp, vp]
     _lib = L
     return L
 

@@ -21,31 +21,57 @@ those modules stay PyTorch on the caller's side.
 """
 from collections import OrderedDict
 
-# (old substring, new substring), in the reference's matching order for the keys that
-# contain 'backbone_3d' (convert_dfm_checkpoints.py:49-53)
+# (old substring, new substring), in the reference's matching order
+# (convert_dfm_checkpoints.py:49-63, without the lidar teacher's rows).  The first five rows
+# cover the keys that contain 'backbone_3d'; they are all ``load_hot_path`` applies.
 _LIGA_RENAMES = (
     ('backbone_3d.feature_backbone', 'backbone'),
     ('backbone_3d.feature_neck', 'neck'),
     ('backbone_3d.sem_neck', 'neck_2d'),
     ('backbone_3d.rpn3d_convs', 'feature_transformation.voxel_convs'),
     ('backbone_3d', 'backbone_stereo'),
+    ('backbone_2d.rpn3d_conv2', 'backbone_3d.compress_conv'),
+    ('backbone_2d.rpn3d_conv3', 'backbone_3d.bev_hourglass'),
+    ('dense_head_2d.bbox_head', 'bbox_head_2d'),
+    ('dense_head.rpn3d_cls_convs', 'bbox_head_3d.cls_convs'),
+    ('dense_head.rpn3d_bbox_convs', 'bbox_head_3d.reg_convs'),
+    ('dense_head.conv_cls', 'bbox_head_3d.conv_cls'),
+    ('dense_head.conv_box', 'bbox_head_3d.conv_reg'),
+    ('dense_head.conv_dir_cls', 'bbox_head_3d.conv_dir_cls'),
+    ('dense_head.norm_imitation', 'norm_imitation'),
+    ('dense_head.conv_imitation', 'conv_imitation'),
 )
+_LIGA_HOT_PATH_RENAMES = _LIGA_RENAMES[:5]
+
+# detector entries that only training builds (the LiDAR teacher, the 2-D head and neck, the
+# imitation layers): load_detector skips and reports them
+TRAINING_ONLY_PREFIXES = ('lidar_model.', 'neck_2d.', 'bbox_head_2d.', 'conv_imitation.',
+                          'norm_imitation.')
 
 # (a key matches a prefix only up to its '.': 'backbone.' never captures 'backbone_stereo.*')
 HOT_PATH_PREFIXES = ('backbone_stereo', 'feature_transformation', 'neck_3d', 'bbox_head_3d',
                      'neck', 'backbone')
 
 
-def convert_liga_key(key):
-    """mmdet3d-style name of a LIGA-DfM ``model_state`` key, for the prefixes that
-    involve the hot path; keys of the lidar teacher (``lidar_model.*``) and of other
-    modules are returned unchanged."""
+def convert_liga_key(key, renames=_LIGA_HOT_PATH_RENAMES):
+    """mmdet3d-style name of a LIGA-DfM ``model_state`` key.  By default only the rows for the
+    keys that contain 'backbone_3d' apply; ``renames=_LIGA_RENAMES`` applies the converter's whole
+    table.  Keys of the lidar teacher (``lidar_model.*``) and unmatched keys are returned
+    unchanged."""
     if key.startswith('lidar_model.'):
         return key
-    for old, new in _LIGA_RENAMES:
+    for old, new in renames:
         if old in key:
             return key.replace(old, new)
     return key
+
+
+def _unwrap(state_dict, liga):
+    if 'state_dict' in state_dict and isinstance(state_dict['state_dict'], dict):
+        return state_dict['state_dict'], bool(liga)
+    if 'model_state' in state_dict and isinstance(state_dict['model_state'], dict):
+        return state_dict['model_state'], True
+    return state_dict, bool(liga)
 
 
 def hot_path_state_dicts(state_dict, liga=False):
@@ -53,10 +79,7 @@ def hot_path_state_dicts(state_dict, liga=False):
     hot-path modules, with the prefix stripped and the checkpoint's key order kept.
     ``liga=True`` first applies :func:`convert_liga_key` (drops ``global_step`` keys
     like the reference converter, ``:65-71``)."""
-    if 'state_dict' in state_dict and isinstance(state_dict['state_dict'], dict):
-        state_dict = state_dict['state_dict']
-    elif 'model_state' in state_dict and isinstance(state_dict['model_state'], dict):
-        state_dict, liga = state_dict['model_state'], True
+    state_dict, liga = _unwrap(state_dict, liga)
     out = {p: OrderedDict() for p in HOT_PATH_PREFIXES}
     for key, value in state_dict.items():
         if liga:
@@ -93,3 +116,32 @@ def load_hot_path(state_dict, backbone=None, frustum=None, neck=None, strict=Tru
             raise KeyError(f'checkpoint has no "{prefix}." parameters')
         res[prefix] = module.load_state_dict(parts[prefix], strict=strict)
     return res
+
+
+def load_detector(ckpt, detector, liga=None):
+    """Strictly loads a whole-detector checkpoint into ``modules.DfM`` / ``modules.MultiViewDfM``:
+    every key of ``detector.state_dict()`` must be present (``backbone_3d.*`` included), the
+    training-only entries (``TRAINING_ONLY_PREFIXES``) are skipped, and any other key the
+    detector does not have raises ``KeyError``.  ``ckpt`` is a state_dict, an mmdet3d checkpoint
+    (``state_dict``) or a LIGA-DfM one (``model_state``, renamed by the converter's whole table;
+    ``liga=True`` applies the renames to a bare state_dict too).  Returns the sorted skipped
+    keys."""
+    state, liga = _unwrap(ckpt, liga)
+    own = detector.state_dict()
+    keep, skipped, unknown = OrderedDict(), [], []
+    for key, value in state.items():
+        if liga:
+            if 'global_step' in key:
+                continue
+            key = convert_liga_key(key, _LIGA_RENAMES)
+        if key.startswith(TRAINING_ONLY_PREFIXES):
+            skipped.append(key)
+        elif key in own:
+            keep[key] = value
+        else:
+            unknown.append(key)
+    if unknown:
+        raise KeyError(f'checkpoint keys the detector does not have: {sorted(unknown)[:8]}'
+                       f'{" ..." if len(unknown) > 8 else ""} ({len(unknown)} in all)')
+    detector.load_state_dict(keep, strict=True)
+    return sorted(skipped)

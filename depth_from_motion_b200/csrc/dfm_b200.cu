@@ -26,6 +26,7 @@
 #include "resnet_kernels.cuh"
 #include "resnet101_kernels.cuh"
 #include "box_post_kernels.cuh"
+#include "image_prep_kernels.cuh"
 
 namespace {
 
@@ -1560,3 +1561,4 @@ int dfm_depth_head_forward(const float* d_cost, const float* d_depth_samples, in
 #include "liga_resnet_api.inc"
 #include "resnet101_api.inc"
 #include "box_post_api.inc"
+#include "image_prep_api.inc"

@@ -24,6 +24,7 @@ reference checkpoints load with ``strict=True``); their ``forward`` is never
 called.  There is no PyTorch fallback: without the built library or an H100 the
 modules raise.
 """
+import copy
 import ctypes
 import os
 
@@ -32,7 +33,7 @@ import torch
 import torch.nn as nn
 
 from . import capi
-from .registry import BACKBONES, HEADS, NECKS
+from .registry import BACKBONES, DETECTORS, HEADS, NECKS
 
 _IMPL = {'auto': capi.DFM_CONV_AUTO, 'simt': capi.DFM_CONV_SIMT,
          'tc': capi.DFM_CONV_TC, 'tc_neck': capi.DFM_CONV_TC_NECK,
@@ -2082,3 +2083,225 @@ class MultiViewDfMFeatureTransformation:
         if getattr(self, 'with_neck_3d', self.neck_3d is not None):
             volume_feat = self.neck_3d(volume_feat)[0]               # :263
         return (volume_feat, )                                       # :265-268
+
+
+# ---------------------------------------------------------------------------------------------
+# Whole detectors: DfM (KITTI) and MultiViewDfM (Waymo), test path only
+# ---------------------------------------------------------------------------------------------
+def bbox3d2result(bboxes, scores, labels):
+    """mmdet3d.core.bbox3d2result (core/bbox/transforms.py:53-76): results on the CPU."""
+    return dict(boxes_3d=bboxes.to('cpu'), scores_3d=scores.cpu(), labels_3d=labels.cpu())
+
+
+@DETECTORS.register_module()
+class DfM(nn.Module):
+    """The reference detector ``DfM`` (detectors/dfm.py:17-441) at test time, built from the
+    shipped ``model`` dict (minus ``type``) with the local registries and the constructor's
+    injections (:43-109).  The training-only entries (``lidar_model``, ``neck_2d``,
+    ``bbox_head_2d``, ``depth_head_2d``, ``imitation_cfgs``) are accepted and not built;
+    ``normalizer_clamp_value`` only reaches the LIGA head, as in the reference (:107-108)."""
+
+    def __init__(self, backbone, neck, backbone_stereo, backbone_3d, bbox_head_3d, neck_2d=None,
+                 neck_3d=None, feature_transformation=None, bbox_head_2d=None,
+                 depth_head_2d=None, depth_head=None, lidar_model=None, depth_cfg=None,
+                 voxel_cfg=None, normalizer_clamp_value=10, imitation_cfgs=None, train_cfg=None,
+                 test_cfg=None, pretrained=None, init_cfg=None):
+        super().__init__()
+        from .registry import build_backbone, build_head, build_neck
+        cp = copy.deepcopy
+        self.backbone = build_backbone(cp(backbone))
+        self.neck = build_neck(cp(neck))
+        if backbone_stereo is not None:
+            backbone_stereo = cp(backbone_stereo)
+            if depth_cfg is not None:
+                backbone_stereo.update(depth_cfg=depth_cfg)
+            self.backbone_stereo = build_backbone(backbone_stereo)
+        if backbone_3d is not None:
+            self.backbone_3d = build_backbone(cp(backbone_3d))
+        if neck_3d is not None:
+            self.neck_3d = build_neck(cp(neck_3d))
+        if feature_transformation is not None:
+            feature_transformation = cp(feature_transformation)
+            feature_transformation.update(cat_img_feature=self.neck.cat_img_feature,
+                                          in_sem_channels=self.neck.sem_channels[-1])
+            self.feature_transformation = build_neck(feature_transformation)
+        if depth_head is not None:
+            self.depth_head = build_head(cp(depth_head))
+        self.imitation_cfgs = imitation_cfgs
+        if depth_cfg is not None:
+            self.downsampled_depth_offset = 0.5
+            self.depth_downsample_factor = depth_cfg['downsample_factor']
+            self.prepare_depth(depth_cfg)
+            if feature_transformation is not None:
+                self.feature_transformation.depth_cfg = depth_cfg
+            if depth_head is not None:
+                self.backbone_stereo.downsampled_depth = self.downsampled_depth
+                self.depth_head.depth_samples = self.depth
+                self.depth_head.downsample_factor = self.depth_downsample_factor
+        if voxel_cfg is not None:
+            self.prepare_coordinates_3d(voxel_cfg)
+            if feature_transformation is not None:
+                self.feature_transformation.coordinates_3d = self.coordinates_3d
+        self.normalizer_clamp_value = normalizer_clamp_value
+        self.train_cfg, self.test_cfg = train_cfg, test_cfg
+        bbox_head_3d = cp(bbox_head_3d)
+        bbox_head_3d.update(train_cfg=train_cfg, test_cfg=test_cfg)
+        if bbox_head_3d['type'] == 'LIGAAnchor3DHead':
+            bbox_head_3d.update(normalizer_clamp_value=normalizer_clamp_value)
+        self.bbox_head_3d = build_head(bbox_head_3d)
+
+    @property
+    def with_backbone_3d(self):
+        return getattr(self, 'backbone_3d', None) is not None
+
+    @property
+    def with_neck_3d(self):
+        return getattr(self, 'neck_3d', None) is not None
+
+    @property
+    def with_depth_head(self):
+        return getattr(self, 'depth_head', None) is not None
+
+    @property
+    def with_depth_head_2d(self):
+        return False   # the 2-D depth head is training-only and never built here
+
+    def prepare_depth(self, depth_cfg):
+        """dfm.py:152-168: the plane depths of the cost volume and the depth-bin centres."""
+        assert depth_cfg['depth_min'] >= 0 and depth_cfg['depth_max'] > depth_cfg['depth_min']
+        interval = (depth_cfg['depth_max'] - depth_cfg['depth_min']) / depth_cfg['num_bins']
+        f = self.depth_downsample_factor
+        self.downsampled_depth = torch.zeros(depth_cfg['num_bins'] // f, dtype=torch.float32)
+        for i in range(depth_cfg['num_bins'] // f):
+            self.downsampled_depth[i] = (i + self.downsampled_depth_offset) * f * interval + \
+                depth_cfg['depth_min']
+        self.depth = torch.zeros(depth_cfg['num_bins'], dtype=torch.float32)
+        for i in range(depth_cfg['num_bins']):
+            self.depth[i] = (i + 0.5) * interval + depth_cfg['depth_min']
+
+    def prepare_coordinates_3d(self, voxel_cfg):
+        """dfm.py:170-211 (sample_rate 1): the [Nz, Ny, Nx, 3] voxel-centre grid."""
+        pcr, vs = voxel_cfg['point_cloud_range'], voxel_cfg['voxel_size']
+        grid = (np.array(pcr[3:6], dtype=np.float32) - np.array(pcr[0:3], dtype=np.float32)) / \
+            np.array(vs)
+        nx, ny, nz = np.round(grid).astype(np.int64).tolist()
+        zs = torch.linspace(pcr[2] + vs[2] / 2., pcr[5] - vs[2] / 2., nz, dtype=torch.float32)
+        ys = torch.linspace(pcr[1] + vs[1] / 2., pcr[4] - vs[1] / 2., ny, dtype=torch.float32)
+        xs = torch.linspace(pcr[0] + vs[0] / 2., pcr[3] - vs[0] / 2., nx, dtype=torch.float32)
+        zs, ys, xs = torch.meshgrid(zs, ys, xs, indexing='ij')
+        self.coordinates_3d = torch.stack([xs, ys, zs], dim=-1).float()
+
+    def _check_test_input(self, img, img_metas, min_views):
+        if self.training:
+            raise RuntimeError(f'{type(self).__name__} runs the test path only: call .eval()')
+        if img.dim() != 5 or img.shape[2] != 3 or img.shape[1] < min_views:
+            raise ValueError(f'img must be [B, N >= {min_views}, 3, H, W], got '
+                             f'{tuple(img.shape)}')
+        if len(img_metas) != img.shape[0]:
+            raise ValueError(f'{len(img_metas)} img_metas for a batch of {img.shape[0]}')
+        _check_cuda(img, 'img')
+
+    def extract_feat(self, img, img_metas):
+        """dfm.py:264-298 for one sample (the stereo backbone takes B == 1).  The cur / prev
+        pair goes through LIGAResNet in one call (eval BatchNorm: equal to two calls); the
+        reference's device copy of ``cur2prevs`` stays a host tensor, which is what the stereo
+        backbone reads, so no host synchronisation is added."""
+        pair = img[0, :2].contiguous()
+        feats = self.backbone(pair)
+        cur_feats = [pair[0:1]] + [f[0:1] for f in feats]
+        prev_feats = [pair[1:2]] + [f[1:2] for f in feats]
+        cur_stereo_feat, cur_sem_feat = self.neck(cur_feats)
+        prev_stereo_feat, _ = self.neck(prev_feats)      # prev semantic feature unused (:283)
+        for meta in img_metas:
+            c2p = meta['cur2prevs']
+            if isinstance(c2p, torch.Tensor):   # e.g. metas already through extract_feat
+                c2p = c2p.detach().cpu()
+            meta['cur2prevs'] = torch.as_tensor(np.asarray(c2p, dtype=np.float64),
+                                                dtype=img.dtype)
+        costs, stereo_feats, mono_feats = self.backbone_stereo(cur_stereo_feat,
+                                                               prev_stereo_feat, img_metas)
+        return costs, stereo_feats, mono_feats, cur_sem_feat
+
+    def _head_outputs(self, img, img_metas):
+        """dfm.py:416-432 up to the head, sample by sample; DepthHead is fused into
+        FrustumToVoxel (``CostLogits``), so no softmax volume is built."""
+        outs = []
+        for b in range(img.shape[0]):
+            metas = img_metas[b:b + 1]
+            costs, stereo_feats, _, cur_sem_feat = self.extract_feat(img[b:b + 1], metas)
+            logits = CostLogits(costs, depth_samples=self.depth_head.depth_samples)
+            volume_feat = self.feature_transformation(stereo_feats, logits, metas, cur_sem_feat)
+            _, cv, nz, ny, nx = volume_feat.shape
+            bev_feat = volume_feat.view(-1, cv * nz, ny, nx)          # height compression
+            _, bev_feat = self.backbone_3d(bev_feat)
+            outs.append(self.bbox_head_3d([bev_feat]))
+        return tuple([torch.cat([o[k][0] for o in outs])] for k in range(3))
+
+    def simple_test(self, img, img_metas):
+        """dfm.py:416-441: ``[dict(boxes_3d, scores_3d, labels_3d, pseudo_lidar=True)]`` per
+        sample.  ``img``: [B, N >= 2, 3, H, W] CUDA (current frame first)."""
+        self._check_test_input(img, img_metas, 2)
+        outs = self._head_outputs(img, img_metas)
+        bbox_list = self.bbox_head_3d.get_bboxes(*outs, img_metas)
+        results = [bbox3d2result(*r) for r in bbox_list]
+        for r in results:
+            r['pseudo_lidar'] = True
+        return results
+
+    def forward_test(self, img, img_metas, **kwargs):
+        return self.simple_test(img, img_metas)
+
+
+@DETECTORS.register_module()
+class MultiViewDfM(MultiViewDfMFeatureTransformation, DfM):
+    """The reference detector ``MultiViewDfM`` (detectors/multiview_dfm.py:12-341) at test time:
+    ResNet + FPN over every view, the lifting of ``MultiViewDfMFeatureTransformation``, the
+    3-D neck and ``Anchor3DHead``."""
+
+    def __init__(self, backbone, neck, backbone_stereo, backbone_3d, neck_3d, bbox_head_3d,
+                 voxel_size, anchor_generator, neck_2d=None, bbox_head_2d=None,
+                 depth_head_2d=None, depth_head=None, train_cfg=None, test_cfg=None,
+                 valid_sample=True, temporal_aggregate='mean', transform_depth=True,
+                 pretrained=None, init_cfg=None):
+        super().__init__(backbone=backbone, neck=neck, backbone_stereo=backbone_stereo,
+                         backbone_3d=backbone_3d, neck_3d=neck_3d, bbox_head_3d=bbox_head_3d,
+                         neck_2d=neck_2d, bbox_head_2d=bbox_head_2d,
+                         depth_head_2d=depth_head_2d, depth_head=depth_head,
+                         train_cfg=train_cfg, test_cfg=test_cfg, pretrained=pretrained,
+                         init_cfg=init_cfg)
+        self.voxel_size = voxel_size
+        self.voxel_range = anchor_generator['ranges'][0]
+        self.n_voxels = [round((self.voxel_range[3 + a] - self.voxel_range[a]) / voxel_size[a])
+                         for a in range(3)]
+        self.anchor_generator_cfg = anchor_generator
+        self.valid_sample = valid_sample
+        self.temporal_aggregate = temporal_aggregate
+        self.transform_depth = transform_depth
+
+    def extract_feat(self, img, img_metas):
+        """multiview_dfm.py:67-117.  Every view of every sample, current and previous, goes
+        through ResNet and FPN in one call; per sample the views stay in the reference's
+        current-then-previous order."""
+        batch_size, _, c_in, h, w = img.shape
+        num_views = img_metas[0]['num_views']
+        num_ref_frames = img_metas[0]['num_ref_frames']
+        num_frames = num_ref_frames + 1 if num_ref_frames > 0 else 1
+        if img.shape[1] != num_views * num_frames:
+            raise ValueError(f'img has {img.shape[1]} views, the metas say {num_views} x '
+                             f'{num_frames}')
+        input_shape = img.shape[-2:]
+        for img_meta in img_metas:
+            img_meta.update(input_shape=input_shape)
+        feats = self.neck(self.backbone(img.reshape(-1, c_in, h, w)))[0]
+        _, c_feat, h_feat, w_feat = feats.shape
+        batch_feats = feats.view(batch_size, -1, c_feat, h_feat, w_feat)
+        return self.feature_transformation(batch_feats, img_metas, num_views, num_frames)
+
+    def simple_test(self, img, img_metas):
+        """multiview_dfm.py:321-341: ``[dict(boxes_3d, scores_3d, labels_3d)]`` per sample.
+        ``img``: [B, Nv * T, 3, H, W] CUDA, current views first."""
+        self._check_test_input(img, img_metas, 1)
+        bev_feat = self.extract_feat(img, img_metas)[0]
+        outs = self.bbox_head_3d([bev_feat])
+        bbox_list = self.bbox_head_3d.get_bboxes(*outs, img_metas)
+        return [bbox3d2result(*r) for r in bbox_list]

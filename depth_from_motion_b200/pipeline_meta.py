@@ -1,8 +1,9 @@
 """Input-side metadata the DfM hot path reads (SURVEY.md section 8(f) row 4): what the
 reference's data pipeline puts into ``img_metas`` for ``DfMBackbone.forward``
-(dfm_backbone.py:150-172).  Host-side NumPy only -- no images are touched here; the
-image transforms themselves (resize / crop / pad of pixels) stay with the reference's
-pipeline.  Restated from:
+(dfm_backbone.py:150-172) and for MultiViewDfM's lifting.  Host-side NumPy only -- no images
+are touched here; the pixel half of the test pipelines (crop / resize / normalise / pad) runs
+on the GPU in ``image_prep.py``, which builds its metadata from these functions.  Restated
+from:
 
     VideoPipeline.__call__     mmdet3d/datasets/pipelines/loading.py:416-545
         reference-frame selection (:434-444), cam2global (:451-468, :495-513),
@@ -10,6 +11,8 @@ pipeline.  Restated from:
     RandomCrop3D._crop_data    mmdet3d/datasets/pipelines/transforms_3d.py:2530-2537 (offsets),
         :2583-2594 (intrinsics after the crop, ``crop_offset``)
     DfM.extract_feat           mmdet3d/models/detectors/dfm.py:288-293 (cur2prevs -> tensor)
+    MultiViewImageResize3D._resize_img  transforms_3d.py:2409-2434 (mmcv.imrescale size,
+        ``scale_factor``)
 """
 import numpy as np
 
@@ -107,6 +110,19 @@ def crop3d_meta(cam2img, crop_x1, crop_y1):
     off = np.matmul(K, T)
     cam2img[:off.shape[0], :off.shape[1]] = off
     return cam2img, [crop_x1, crop_y1]
+
+
+def rescale_meta(img_hw, img_scale):
+    """Size and ``scale_factor`` of a keep-ratio resize (MultiViewImageResize3D, keep_ratio=True):
+    mmcv ``rescale_size`` takes ``s = min(long / max(h, w), short / min(h, w))`` for the
+    (long, short) ``img_scale`` and the new size ``int(x * s + 0.5)``; the recorded factor is the
+    one actually applied per axis, ``[w_scale, h_scale, w_scale, h_scale]`` in fp32
+    (transforms_3d.py:2418-2434).  Returns ``((new_h, new_w), scale_factor)``."""
+    h, w = img_hw
+    s = min(max(img_scale) / max(h, w), min(img_scale) / min(h, w))
+    new_w, new_h = int(w * float(s) + 0.5), int(h * float(s) + 0.5)
+    w_scale, h_scale = new_w / w, new_h / h
+    return (new_h, new_w), np.array([w_scale, h_scale, w_scale, h_scale], dtype=np.float32)
 
 
 def backbone_img_meta(ori_cam2img, cur2prevs_np, ori_shape, pad_shape, crop_offset=(0, 0),

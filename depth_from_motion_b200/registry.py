@@ -63,6 +63,7 @@ class Registry:
 BACKBONES = Registry('backbone')
 NECKS = Registry('neck')
 HEADS = Registry('head')
+DETECTORS = Registry('detector')
 
 
 def build_backbone(cfg):
@@ -78,6 +79,18 @@ def build_neck(cfg):
 def build_head(cfg):
     """mmdet3d/models/builder.py:63-68."""
     return HEADS.build(cfg)
+
+
+def build_detector(cfg, train_cfg=None, test_cfg=None):
+    """mmdet3d/models/builder.py:79-96: ``DfM`` / ``MultiViewDfM`` from a config's ``model``
+    dict; ``train_cfg`` / ``test_cfg`` given here must not also be in ``cfg``."""
+    assert cfg.get('train_cfg') is None or train_cfg is None, \
+        'train_cfg specified in both outer field and model field '
+    assert cfg.get('test_cfg') is None or test_cfg is None, \
+        'test_cfg specified in both outer field and model field '
+    default_args = {k: v for k, v in (('train_cfg', train_cfg), ('test_cfg', test_cfg))
+                    if v is not None}
+    return DETECTORS.build(cfg, default_args=default_args)
 
 
 class ConfigDict(dict):
@@ -136,7 +149,8 @@ def register_into_mmdet():
                                  module=modules.DfMBackbone)
     MM_HEADS.register_module(name='DepthHead', force=True,
                              module=modules.DepthHead)
-    # (LIGAAnchor3DHead and Anchor3DHead are NOT forced into mmdet's registry: the mirrors
+    # (the detectors DfM / MultiViewDfM are registered locally only: mmdet3d's own stay in
+    # place.  LIGAAnchor3DHead and Anchor3DHead are NOT forced into mmdet's registry: the mirrors
     # implement forward only, the detector needs the reference class's loss / get_bboxes;
     # BEVHourglass's forward is the whole module)
     MM_BACKBONES.register_module(name='BEVHourglassB200', force=True,

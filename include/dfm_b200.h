@@ -668,6 +668,36 @@ int dfm_box_post_debug_tensor(dfm_box_post_t* h, const char* name, int* d_out, l
  * candidate; d_iou: device [n].  DFM_ERR_INVALID on n <= 0 or a null pointer. */
 int dfm_op_rotated_iou(const float* d_a, const float* d_b, int n, float* d_iou, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * Image preparation of the shipped test pipelines, one launch per batch of views.
+ * d_src: num_views decoded 8-bit BGR images, [num_views][src_h][src_w][3], all one size.
+ * d_out: [num_views][3][pad_h][pad_w] fp32, pad_h / pad_w = out_h / out_w rounded up to
+ * pad_divisor; every element is written (pad cells 0).
+ *   DFM_IMAGE_PREP_CROP    (KITTI): the window img[crop_y:crop_y+out_h, crop_x:crop_x+out_w]
+ *                          (RandomCrop3D), which must lie inside the image.
+ *   DFM_IMAGE_PREP_RESCALE (Waymo): cv2.resize(INTER_LINEAR) of the float image to
+ *                          out_w x out_h (mmcv.imrescale); an exact 2x downscale, which cv2
+ *                          runs as INTER_AREA, is refused.
+ * Then mmcv.imnormalize (as cv2 computes it): channel swap if to_rgb, then
+ * float(double(x - float(mean[c])) * (1 / std[c])), and
+ * impad_to_multiple(pad_divisor, pad_val=0).  DFM_ERR_INVALID for sizes it cannot serve.
+ * ---------------------------------------------------------------------------------- */
+#define DFM_IMAGE_PREP_CROP 0
+#define DFM_IMAGE_PREP_RESCALE 1
+typedef struct dfm_image_prep_desc {
+  int mode;            /* DFM_IMAGE_PREP_CROP or DFM_IMAGE_PREP_RESCALE            */
+  int num_views;       /* views stacked in d_src and d_out                         */
+  int src_h, src_w;    /* decoded view size                                        */
+  int crop_x, crop_y;  /* crop: window origin (ignored by rescale)                 */
+  int out_h, out_w;    /* crop: window size; rescale: resized size                 */
+  int pad_divisor;     /* Pad / MultiViewImagePad size_divisor                      */
+  int to_rgb;          /* 1: BGR -> RGB before normalising                         */
+  double mean[3];      /* img_norm_cfg mean, per output channel, as stored by the     */
+  double std[3];       /* Normalize transforms: fp32 values (widened), not the config's */
+} dfm_image_prep_desc_t;
+int dfm_image_prep(const dfm_image_prep_desc_t* desc, const unsigned char* d_src, float* d_out,
+                   void* stream);
+
 /* Re-entrancy: handles may live on different devices and be driven from different host
  * threads only if each thread owns its device; per-device scratch (K-slice partial sums,
  * lifting staging, the host-copy side stream) and the profiling record are shared by all
