@@ -240,6 +240,7 @@ inline void tc_build_program(int ptype, int Cin, int ncta, uint32_t* w_cursor, T
 struct TcWeights {
   DevArray<uint8_t> dev;  // [nsplit][image bytes]
   int Cin = 0, Cout = 0, ncta = 0, nsplit = 0, mode = -1, kslice = 0;
+  int cluster = 1;  // > 1: the nsplit output-channel groups share bricks as one cluster (32 -> 64)
   uint32_t image_bytes = 0, hi_bytes = 0;
   TcProgram prog[2];
 
@@ -256,6 +257,7 @@ struct TcWeights {
     Cin = cin;
     Cout = cout;
     kslice = ks ? 1 : 0;
+    cluster = 1;
     const int cin_img = ks ? 16 : cin;  // input channels of one weight image
     ncta = ks ? cout : 1024 / cin;
     nsplit = ks ? cin / 16 : cout / ncta;
@@ -294,7 +296,10 @@ struct TcWeights {
     }
     return true;
   }
-  bool build(const float* packed, int cin, int cout, int m, std::string* err) {
+  // share_bricks = false: a 32 -> 64 stride-2 layer takes the input-channel slices instead of
+  // the cluster-shared bricks (see below)
+  bool build(const float* packed, int cin, int cout, int m, std::string* err,
+             bool share_bricks = true) {
     static const bool no_ks1 = getenv("DFM_NO_KSLICE") != nullptr;
     // stride 1, 64 -> 64: four output-channel groups each re-load the input and issue N = 48
     // MMAs; four input-channel slices would issue N = 192 MMAs on a quarter of the input each
@@ -304,11 +309,23 @@ struct TcWeights {
     if (m == TC_S1) return build_mode<TC_S1>(packed, cin, cout, err,
                                              cin == 64 && cout == 64 && !no_ks1 && ks1);
     if (m == TC_S2) {
-      // stride-2 layers are loader-bound: with output-channel groups every group re-loads and
-      // re-transforms the whole input (2x for 32->64, 4x for 64->64); input-channel slices load
-      // it exactly once (DFM_NO_KSLICE=1 keeps the output-channel split for A/B runs)
+      // stride-2 layers are loader-bound: with independent output-channel groups every group
+      // re-loads and re-transforms the whole input (2x for 32->64, 4x for 64->64).
+      // 32 -> 64: the two groups run as one thread-block cluster and share every brick
+      // (conv_tc_kernel, CL), so the input is read once and no partial sums exist.
+      // 64 -> 64: input-channel slices with partial outputs in global memory and a reduce pass.
+      // Four clustered groups of 16 outputs issue N = 16 / 32 MMAs that each re-read the whole
+      // 64-channel brick from shared memory: H100 SXM, KITTI D = 112 stereo conv3, 0.570 ms
+      // clustered vs 0.220 ms sliced.
+      // A/B switches: DFM_S2_KSLICE=1 (read whenever weights are set) slices 32 -> 64 too -- the
+      // route DFM_NO_TMA / DFM_TMA_CONV3 refine --, DFM_NO_KSLICE=1 independent output groups.
       static const bool no_ks = getenv("DFM_NO_KSLICE") != nullptr;
-      return build_mode<TC_S2>(packed, cin, cout, err, cout == 64 && !no_ks);
+      static const bool tma_ab = getenv("DFM_NO_TMA") != nullptr || getenv("DFM_TMA_CONV3") != nullptr;
+      const bool ks = cout == 64 && !no_ks &&
+                      (cin == 64 || !share_bricks || tma_ab || getenv("DFM_S2_KSLICE") != nullptr);
+      if (!build_mode<TC_S2>(packed, cin, cout, err, ks)) return false;
+      if (cin == 32 && cout == 64 && !ks && !no_ks) cluster = nsplit;  // 2
+      return true;
     }
     return build_mode<TC_T>(packed, cin, cout, err);
   }
@@ -326,32 +343,64 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-// bounded wait: a protocol bug must not hang the GPU; on timeout flag the error
+// bounded wait: a protocol bug must not hang the GPU; on timeout flag the error.
+// CL: the phase is completed by arrivals of other CTAs of the cluster (acquire at cluster scope)
+template <bool CL = false>
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* err) {
   for (int it = 0; it < (1 << 26); ++it) {
     uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred q;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 q, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, q;\n\t}\n"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
+    if constexpr (CL)
+      asm volatile(
+          "{\n\t.reg .pred q;\n\t"
+          "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 q, [%1], %2;\n\t"
+          "selp.u32 %0, 1, 0, q;\n\t}\n"
+          : "=r"(ok)
+          : "r"(bar), "r"(parity)
+          : "memory");
+    else
+      asm volatile(
+          "{\n\t.reg .pred q;\n\t"
+          "mbarrier.try_wait.parity.shared::cta.b64 q, [%1], %2;\n\t"
+          "selp.u32 %0, 1, 0, q;\n\t}\n"
+          : "=r"(ok)
+          : "r"(bar), "r"(parity)
+          : "memory");
     if (ok) return;
   }
   // err is mapped host memory (TcErrFlag)
   *reinterpret_cast<volatile int*>(err) = 1;
   __threadfence_system();
 }
+template <bool CL = false>
 __device__ __forceinline__ void mbar_wait_timed(uint32_t bar, uint32_t parity, int* err,
                                                 unsigned long long& acc, bool timed) {
   if (!timed) {
-    mbar_wait(bar, parity, err);
+    mbar_wait<CL>(bar, parity, err);
     return;
   }
   const long long t0 = clock64();
-  mbar_wait(bar, parity, err);
+  mbar_wait<CL>(bar, parity, err);
   acc += (unsigned long long)(clock64() - t0);
+}
+// distributed shared memory: the address of the same shared-memory location in CTA `rank` of
+// the cluster, a release-arrive on an mbarrier there, a 16-byte store there
+__device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+  return r;
+}
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar)
+               : "memory");
+}
+__device__ __forceinline__ void st_cluster_v4(uint32_t addr, uint4 v) {
+  asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x),
+               "r"(v.y), "r"(v.z), "r"(v.w)
+               : "memory");
+}
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;"
+               ::: "memory");
 }
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
@@ -371,7 +420,7 @@ __device__ __forceinline__ void desc_add(uint64_t& d, uint32_t inc16) {
 __device__ __forceinline__ uint64_t pack64(uint32_t lo, uint32_t hi) {
   return ((uint64_t)hi << 32) | lo;
 }
-__device__ __forceinline__ void split_store(const float v[8], uint8_t* hi_dst, uint8_t* lo_dst) {
+__device__ __forceinline__ void split8(const float v[8], uint4& hi, uint4& lo) {
   uint32_t h[4], l[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
@@ -381,8 +430,14 @@ __device__ __forceinline__ void split_store(const float v[8], uint8_t* hi_dst, u
     h[i] = *reinterpret_cast<const uint32_t*>(&hh);
     l[i] = *reinterpret_cast<const uint32_t*>(&ll);
   }
-  *reinterpret_cast<uint4*>(hi_dst) = make_uint4(h[0], h[1], h[2], h[3]);
-  *reinterpret_cast<uint4*>(lo_dst) = make_uint4(l[0], l[1], l[2], l[3]);
+  hi = make_uint4(h[0], h[1], h[2], h[3]);
+  lo = make_uint4(l[0], l[1], l[2], l[3]);
+}
+__device__ __forceinline__ void split_store(const float v[8], uint8_t* hi_dst, uint8_t* lo_dst) {
+  uint4 h, l;
+  split8(v, h, l);
+  *reinterpret_cast<uint4*>(hi_dst) = h;
+  *reinterpret_cast<uint4*>(lo_dst) = l;
 }
 
 // ----------------------------------------------------------------------------------
@@ -735,13 +790,23 @@ struct TcWin<TC_T> {  // zi feeds 2zi-1 (kz=0), 2zi (kz=1), 2zi+1 (kz=2)
 // ----------------------------------------------------------------------------------
 // the kernel
 // ----------------------------------------------------------------------------------
-template <int MODE, int CIN, int NCTA, class Loader>
+// CL > 1: cluster-shared bricks.  The CL output-channel groups of one work range run as one
+// thread-block cluster (group = cluster rank); the loaders of each CTA gather and transform brick
+// rows rank, rank + CL, ... and store them into the stage of EVERY CTA of the cluster (distributed
+// shared memory), so each input value is read from HBM and transformed once, and every CTA's
+// accumulators still hold complete sums for its own output channels.  A stage is full when the
+// loader warps of all CL CTAs have arrived on it, and free when the consumer warps of all CL CTAs
+// have released it (remote mbarrier arrivals in both directions).
+template <int MODE, int CIN, int NCTA, class Loader, int CL = 1>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ TcParams p,
                                                                  const __grid_constant__ Loader ld) {
   using M = TcMode<MODE>;
   using Win = TcWin<MODE>;
   constexpr bool TMA = Loader::kTma;
+  constexpr bool CLU = CL > 1;
   static_assert(!TMA || MODE == TC_S2, "the TMA loader serves the stride-2 brick only");
+  static_assert(!CLU || (MODE == TC_S2 && !TMA && CIN != 16),
+                "cluster-shared bricks serve the stride-2 output-channel split with register loaders");
   constexpr int CG = M::CG < CIN ? M::CG : CIN;  // channels per stage
   constexpr int NCH = CG / 8;                    // 16-byte channel chunks per stage
   constexpr int NCG = CIN / CG;                  // pipeline stages per input plane
@@ -759,12 +824,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   // NCTA = all output channels): every slice stores its partial sums; kslice_reduce_kernel adds
   // them in slice order (deterministic) and takes the GroupNorm statistics on the way
   constexpr bool KSLICE = CIN == 16;
-  constexpr int NPOS = M::PXB * M::PYB;
+  // brick rows this CTA loads (every CL-th, from its cluster rank)
+  constexpr int ROWS_CTA = (M::PYB + CL - 1) / CL;
   // two loader groups (even / odd loader warps) fill alternate stages: while one group
   // waits for its global loads the other transforms and stores -> two stages in flight
   constexpr int LGROUPS = 2;
   constexpr int LG_THREADS = TC_LOAD_THREADS / LGROUPS;
-  constexpr int NITEM = (NPOS * NCH + LG_THREADS - 1) / LG_THREADS;
+  constexpr int NITEM = (ROWS_CTA * M::PXB * NCH + LG_THREADS - 1) / LG_THREADS;
   constexpr int PCOLS = M::SLOT_BLOCKS * NCTA;        // accumulator columns per output plane
   constexpr int NACC = Win::NPL * PCOLS / 2;          // accumulator registers per thread
 
@@ -782,12 +848,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   auto empty_a = [&](int s) { return bar0 + 8u * (M::NSTAGE + s); };
   const uint32_t w_bar = bar0 + 8u * (2 * M::NSTAGE);
   constexpr int LOAD_WARP0 = TC_MMA_THREADS / 32;
+  // cluster rank (a 1-D grid launched with cluster dimension (CL, 1, 1)) = output-channel group
+  const int rank = CLU ? (int)(blockIdx.x % CL) : 0;
 
   if (tid == 0) {
     for (int s = 0; s < M::NSTAGE; ++s) {
-      // one arrival per loader warp of the group; TMA: the issuing thread's expect_tx arrival
-      mbar_init(full_a(s), TMA ? 1 : LG_THREADS / 32);
-      mbar_init(empty_a(s), TC_MMA_THREADS / 32);  // one arrival per consumer warp
+      // one arrival per loader warp of the group (of every CTA of the cluster); TMA: the issuing
+      // thread's expect_tx arrival
+      mbar_init(full_a(s), TMA ? 1 : CL * LG_THREADS / 32);
+      mbar_init(empty_a(s), CL * TC_MMA_THREADS / 32);  // one arrival per consumer warp
     }
     mbar_init(w_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -808,7 +877,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
           : "memory");
     }
   }
-  __syncthreads();
+  // (cluster: no peer may arrive on or store into this CTA's shared memory before its barriers
+  // are initialised)
+  if constexpr (CLU) cluster_sync_all();
+  else __syncthreads();
 
   if constexpr (TMA) {
     if (warp == LOAD_WARP0 && lane == 0) {
@@ -861,6 +933,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     const bool timed = p.role_cycles != nullptr && lw == 0 && lane == 0;
     unsigned long long t_wait_e = 0;
     const long long t_begin = clock64();
+    // stage base of every CTA of the cluster, in the cluster's shared window
+    uint32_t peer_a[CL];
+#pragma unroll
+    for (int q = 0; q < CL; ++q) peer_a[q] = CLU ? mapa_u32(smem_u32(a_s), q) : 0u;
+    const int nitems = (M::PYB - rank + CL - 1) / CL * M::PXB * NCH;
     TcWalk walk = tc_walk_begin(p);
     TcItem it;
     while (tc_walk_next(p, walk, it)) {
@@ -869,9 +946,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
 #pragma unroll
       for (int k = 0; k < NITEM; ++k) {
         const int i = lt + k * LG_THREADS;
-        live[k] = i < NPOS * NCH;
+        live[k] = i < nitems;
         const int pos = i / NCH;
-        const int bx = pos % M::PXB, by = pos / M::PXB;
+        const int bx = pos % M::PXB, by = pos / M::PXB * CL + rank;
         int row;
         if (MODE == TC_S1) {
           gx[k] = it.x0 - 1 + bx;
@@ -896,7 +973,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
         for (int cg = 0; cg < NCG; ++cg, ++stage_ctr) {
           if ((int)(stage_ctr & (LGROUPS - 1)) != lgrp) continue;
           const int s = stage_ctr % M::NSTAGE;
-          mbar_wait_timed(empty_a(s), ((stage_ctr / M::NSTAGE) & 1) ^ 1, p.err, t_wait_e, timed);
+          mbar_wait_timed<CLU>(empty_a(s), ((stage_ctr / M::NSTAGE) & 1) ^ 1, p.err, t_wait_e,
+                               timed);
           uint8_t* st = a_s + s * STAGE_BYTES;
           const int c0 = cg * CG + chunk * 8 + (KSLICE ? it.split * CIN : 0);
           constexpr int LB = Loader::BATCH < NITEM ? Loader::BATCH : NITEM;
@@ -918,14 +996,36 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
 #pragma unroll
                   for (int i = 0; i < 8; ++i) v[i] = 0.f;
                 }
-                if (!(p.dbg & 32)) split_store(v, st + soff[k0 + b], st + A_HL + soff[k0 + b]);
-                else if (v[0] + v[1] + v[2] + v[3] + v[4] + v[5] + v[6] + v[7] == 1.2345f) st[0] = 1;
+                if (p.dbg & 32) {
+                  if (v[0] + v[1] + v[2] + v[3] + v[4] + v[5] + v[6] + v[7] == 1.2345f) st[0] = 1;
+                } else if constexpr (CLU) {
+                  uint4 h, l;
+                  split8(v, h, l);
+                  const uint32_t off = (uint32_t)(s * STAGE_BYTES + soff[k0 + b]);
+#pragma unroll
+                  for (int q = 0; q < CL; ++q) {
+                    st_cluster_v4(peer_a[q] + off, h);
+                    st_cluster_v4(peer_a[q] + off + A_HL, l);
+                  }
+                } else {
+                  split_store(v, st + soff[k0 + b], st + A_HL + soff[k0 + b]);
+                }
               }
             }
           }
-          if (!(p.dbg & 8)) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+          if (!(p.dbg & 8)) {
+            if constexpr (CLU) asm volatile("fence.proxy.async.shared::cluster;" ::: "memory");
+            else asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+          }
           __syncwarp();
-          if (lane == 0) mbar_arrive(full_a(s));
+          if (lane == 0) {
+            if constexpr (CLU) {
+#pragma unroll
+              for (int q = 0; q < CL; ++q) mbar_arrive_cluster(mapa_u32(full_a(s), q));
+            } else {
+              mbar_arrive(full_a(s));
+            }
+          }
         }
       }
     }
@@ -1048,7 +1148,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
 #pragma unroll 1
         for (int cg = 0; cg < NCG; ++cg, ++stage_ctr) {
           const int s = stage_ctr % M::NSTAGE;
-          mbar_wait_timed(full_a(s), (stage_ctr / M::NSTAGE) & 1, p.err, t_wait_a, timed);
+          mbar_wait_timed<CLU>(full_a(s), (stage_ctr / M::NSTAGE) & 1, p.err, t_wait_a, timed);
           __syncwarp();
           const uint32_t a_lo_stage =
               ((((a_base + s * STAGE_BYTES) >> 4) & 0x3FFF) + a_wg16) | (A_LBO16 << 16);
@@ -1164,7 +1264,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
           wgmma_commit();
           wgmma_wait<0>();
           __syncwarp();
-          if (lane == 0) mbar_arrive(empty_a(s));  // stage refillable: its MMAs have retired
+          // stage refillable: its MMAs have retired (cluster: tell the loaders of every CTA)
+          if (lane == 0) {
+            if constexpr (CLU) {
+#pragma unroll
+              for (int q = 0; q < CL; ++q) mbar_arrive_cluster(mapa_u32(empty_a(s), q));
+            } else {
+              mbar_arrive(empty_a(s));
+            }
+          }
         }
         // planes whose last contribution was this input plane leave the window
         if constexpr (MODE == TC_S1) {
@@ -1198,6 +1306,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
       rc[1] = t_wait_a;
     }
   }
+  // no CTA may retire while a peer can still store into its stages or arrive on its barriers
+  if constexpr (CLU) cluster_sync_all();
 }
 
 // ----------------------------------------------------------------------------------
@@ -1299,7 +1409,7 @@ struct TcOpts {
   float zw = 1.f;
   long long slice_stride = 0;
 };
-template <int MODE, int CIN, int NCTA, class Loader>
+template <int MODE, int CIN, int NCTA, class Loader, int CL = 1>
 bool tc_launch(const Loader& ld, const TcWeights& w, float* out, double* stats,
                const ConvGeom& g, cudaStream_t st, std::string* err, TcOpts opt = TcOpts()) {
   using M = TcMode<MODE>;
@@ -1307,7 +1417,11 @@ bool tc_launch(const Loader& ld, const TcWeights& w, float* out, double* stats,
   constexpr size_t STAGE_BYTES = Loader::kTma ? (size_t)2 * 4 * TMA_S2_CLSR * 16
                                               : (size_t)2 * (CG / 8) * M::ROWS * 16;
   const size_t smem = w.image_bytes + M::NSTAGE * STAGE_BYTES + (2 * M::NSTAGE + 1) * 8;
-  auto kern = conv_tc_kernel<MODE, CIN, NCTA, Loader>;
+  auto kern = conv_tc_kernel<MODE, CIN, NCTA, Loader, CL>;
+  if (w.cluster != CL || (CL > 1 && w.nsplit != CL)) {
+    if (err) *err = "conv_tc: weight image was built for a different cluster size";
+    return false;
+  }
   struct AttrTag { size_t v = 0; };
   static AttrTag attr_dev[kMaxDevices];  // per kernel instantiation and device
   size_t& attr_smem = attr_dev[cur_device()].v;
@@ -1345,8 +1459,31 @@ bool tc_launch(const Loader& ld, const TcWeights& w, float* out, double* stats,
   const long long cols = (long long)p.tiles_x * p.tiles_y;
   const long long units = cols * (g.Do / p.z_unit);
   // persistent grid: one CTA per SM, a multiple of the output-channel splits; never more
-  // CTAs per split than there are z units
+  // CTAs per split than there are z units.  Clusters: as many as fit at once (a cluster is
+  // placed inside one GPC, so SMs that are left over in a GPC stay idle)
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute cl_attr[1];
   int per_split = std::max(1, sms / p.nsplit);
+  if constexpr (CL > 1) {
+    cfg.gridDim = dim3(CL);
+    cfg.blockDim = dim3(TC_THREADS);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cl_attr[0].id = cudaLaunchAttributeClusterDimension;
+    cl_attr[0].val.clusterDim.x = CL;
+    cl_attr[0].val.clusterDim.y = 1;
+    cl_attr[0].val.clusterDim.z = 1;
+    cfg.attrs = cl_attr;
+    cfg.numAttrs = 1;
+    static int max_clusters[kMaxDevices];  // per kernel instantiation and device
+    int& mc = max_clusters[cur_device()];
+    if (!mc && (cudaOccupancyMaxActiveClusters(&mc, kern, &cfg) != cudaSuccess || mc < 1)) {
+      mc = 0;
+      if (err) *err = "conv_tc: no cluster of " + std::to_string(CL) + " CTAs fits on this device";
+      return false;
+    }
+    per_split = mc;
+  }
   per_split = (int)std::min<long long>(per_split, units);
   const int grid = per_split * p.nsplit;
   p.err = tc_err_flag().get();
@@ -1359,7 +1496,16 @@ bool tc_launch(const Loader& ld, const TcWeights& w, float* out, double* stats,
     cudaMemsetAsync(role_buf, 0, 1024 * 8 * sizeof(unsigned long long), st);
     p.role_cycles = role_buf;
   }
-  kern<<<grid, TC_THREADS, smem, st>>>(p, ld);
+  if constexpr (CL > 1) {
+    cfg.gridDim = dim3(grid);
+    const cudaError_t le = cudaLaunchKernelEx(&cfg, kern, p, ld);
+    if (le != cudaSuccess) {
+      if (err) *err = std::string("conv_tc cluster launch: ") + cudaGetErrorString(le);
+      return false;
+    }
+  } else {
+    kern<<<grid, TC_THREADS, smem, st>>>(p, ld);
+  }
   if (role_dbg) {  // debugging aid: synchronous, prints mean cycles per role
     cudaStreamSynchronize(st);
     std::vector<unsigned long long> h((size_t)grid * 8);
@@ -1368,9 +1514,9 @@ bool tc_launch(const Loader& ld, const TcWeights& w, float* out, double* stats,
     for (int b = 0; b < grid; ++b)
       for (int k = 0; k < 8; ++k) a[k] += (double)h[(size_t)b * 8 + k] / grid;
     fprintf(stderr,
-            "[tc mode=%d cin=%d ncta=%d grid=%d cols=%lld Do=%d] mma+epilogue: total %.0f "
-            "wait_full_a %.0f | load: total %.0f wait_empty_a %.0f\n",
-            MODE, CIN, NCTA, grid, cols, g.Do, a[0], a[1], a[3], a[4]);
+            "[tc mode=%d cin=%d ncta=%d cluster=%d grid=%d cols=%lld Do=%d] mma+epilogue: total "
+            "%.0f wait_full_a %.0f | load: total %.0f wait_empty_a %.0f\n",
+            MODE, CIN, NCTA, CL, grid, cols, g.Do, a[0], a[1], a[3], a[4]);
   }
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
@@ -1426,6 +1572,12 @@ bool tc_dispatch(const Loader& ld, const TcWeights& w, float* out, double* stats
     if (err) *err = "conv_tc: the TMA loader serves the K-slice stride-2 convs only";
     return false;
   } else {
+    if (mode == TC_S2 && w.cluster > 1) {
+      if (g.Cin == 32 && w.cluster == 2)
+        return tc_launch<TC_S2, 32, 32, Loader, 2>(ld, w, out, stats, g, st, err, opt);
+      if (err) *err = "conv_tc: unsupported (Cin, cluster size)";
+      return false;
+    }
 #define TC_CASE(MD, CI, NC) \
   if (mode == MD && g.Cin == CI) \
     return tc_launch<MD, CI, NC, Loader>(ld, w, out, stats, g, st, err, opt)

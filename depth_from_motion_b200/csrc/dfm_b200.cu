@@ -209,9 +209,10 @@ int upload(DevBuf& b, const float* h, size_t n) {
   return DFM_OK;
 }
 
-// tc_mode: dfm::TC_S1 / TC_S2 / TC_T, or -1 for "no tensor-core kernel for this layer"
+// tc_mode: dfm::TC_S1 / TC_S2 / TC_T, or -1 for "no tensor-core kernel for this layer";
+// share_bricks: see dfm::TcWeights::build
 int set_conv(ConvW& cw, const float* h, long long numel, int Cin, int Cout, int transposed,
-             int tc_mode) {
+             int tc_mode, bool share_bricks = true) {
   if (numel != (long long)27 * Cin * Cout)
     return fail(DFM_ERR_INVALID, "conv weight has wrong element count");
   cw.Cin = Cin;
@@ -222,7 +223,8 @@ int set_conv(ConvW& cw, const float* h, long long numel, int Cin, int Cout, int 
   cw.tc.release();
   if (tc_mode >= 0 && dfm::tc_supported(Cin, Cout, transposed)) {
     std::string err;
-    if (!cw.tc.build(p.data(), Cin, Cout, tc_mode, &err)) return fail(DFM_ERR_CUDA, err);
+    if (!cw.tc.build(p.data(), Cin, Cout, tc_mode, &err, share_bricks))
+      return fail(DFM_ERR_CUDA, err);
   }
   cw.ntk.release();
   if (tc_mode == dfm::TC_S1 && !transposed && Cin >= 64 && Cin % 32 == 0 && Cout % 32 == 0) {
@@ -370,8 +372,10 @@ int run_conv_impl(const L& simt_loader, TCFN tc_fn, const char* loader_name, con
     std::string err;
     if (gn) DFM_TRY(gn->begin_stats(st));
     {
-      // K-sliced launches carry their own tag: they also run the slice-reduce kernel
-      ProfScope ps(conv_class(w.tc.kslice ? "conv_tc_ks" : "conv_tc", g, loader_name),
+      // K-sliced launches carry their own tag (they also run the slice-reduce kernel), and so do
+      // cluster launches that share bricks
+      ProfScope ps(conv_class(w.tc.kslice ? "conv_tc_ks" : w.tc.cluster > 1 ? "conv_tc_cl" : "conv_tc",
+                              g, loader_name),
                    conv_flops(g), st);
       if (!tc_fn(gn ? gn->sums.p : nullptr, &err)) return fail(DFM_ERR_CUDA, err);
     }
@@ -729,6 +733,11 @@ int tower_set_param(Tower& t, bool mono, int cin0, int cv, const std::string& na
   if (name == "dres1" + sfx + ".gn.weight" || name == "dres1" + sfx + ".gn.bias")
     return set_norm_param(t.g1, name, h, numel);
   struct HG { const char* key; ConvW* w; Norm* n; int ci, co, tr, mode; };
+  // conv1: the stereo tower shares bricks in a CTA cluster; the mono tower keeps the TMA-fed
+  // input-channel slices, so the shipped forward keeps running (and the per-layer test of the
+  // benchmarked shape keeps checking) the presplit producer and the TMA loader.  At KITTI D = 112
+  // that costs 0.107 ms (H100 SXM: 0.432 vs 0.325 ms), the stereo tower carries 83 % of conv1's
+  // bytes.
   const HG hgs[] = {{"conv1.0", &t.c1, &t.gc1, cv, 2 * cv, 0, dfm::TC_S2},
                     {"conv2", &t.c2, &t.gc2, 2 * cv, 2 * cv, 0, dfm::TC_S1},
                     {"conv3.0", &t.c3, &t.gc3, 2 * cv, 2 * cv, 0, dfm::TC_S2},
@@ -737,7 +746,8 @@ int tower_set_param(Tower& t, bool mono, int cin0, int cv, const std::string& na
                     {"conv6", &t.c6, &t.gc6, 2 * cv, cv, 1, dfm::TC_T}};
   for (const HG& e : hgs) {
     const std::string base = hg + "." + e.key;
-    if (name == base + ".0.weight") return set_conv(*e.w, h, numel, e.ci, e.co, e.tr, e.mode);
+    if (name == base + ".0.weight")
+      return set_conv(*e.w, h, numel, e.ci, e.co, e.tr, e.mode, !mono);
     if (name == base + ".1.weight" || name == base + ".1.bias")
       return set_norm_param(*e.n, name, h, numel);
   }
@@ -848,8 +858,10 @@ int tower_forward(dfm_backbone* bb, Tower& t, bool mono, const dfm::WarpLoader& 
   // cost0 = gn1(raw1) + relu(gn0(raw0)) is never stored: consumers re-evaluate it
   const dfm::Term T1 = term(t.raw1, &t.g1, 0);
   // hourglass (conv_modules.py:129-149)
-  // the stride-2 convs are fed by TMA from a pre-split copy of their input (DFM_NO_TMA=1: the
-  // round-1 register loaders, for A/B runs)
+  // stereo conv1 runs as a cluster of two output-channel groups that share every input brick,
+  // mono conv1 and conv3 as input-channel slices (conv_tc.cuh, TcWeights::build; tower_set_param).
+  // On the K-slice route conv1 is fed by TMA from a pre-split copy of its input (DFM_NO_TMA=1:
+  // register loaders; DFM_S2_KSLICE=1 puts the stereo conv1 there too, for A/B runs)
   static const bool no_tma = getenv("DFM_NO_TMA") != nullptr;
   auto tma_ok = [&](const ConvW& w) {
     return impl != DFM_CONV_SIMT && !no_tma && w.tc.ready() && w.tc.kslice &&
