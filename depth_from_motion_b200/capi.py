@@ -56,6 +56,9 @@ SYMBOLS = (
     'dfm_resnet101_missing_params', 'dfm_resnet101_forward', 'dfm_resnet101_debug_tensor',
     'dfm_box_post_create', 'dfm_box_post_destroy', 'dfm_box_post_forward',
     'dfm_box_post_debug_tensor', 'dfm_op_rotated_iou', 'dfm_image_prep',
+    'dfm_multiview_lift_views', 'dfm_multiview_lift_views_cl', 'dfm_view_fingerprint',
+    'dfm_views_equal', 'dfm_fpn_set_num_images', 'dfm_liga_resnet_set_num_images',
+    'dfm_resnet101_set_num_images',
 )
 
 DFM_IMAGE_PREP_CROP, DFM_IMAGE_PREP_RESCALE = 0, 1
@@ -215,6 +218,12 @@ def lib():
                                      vp, vp]
     L.dfm_multiview_lift_cl.argtypes = [POINTER(LiftDesc), vp, vp, vp, vp, vp, vp,
                                      vp, vp]
+    L.dfm_multiview_lift_views.argtypes = [POINTER(LiftDesc), POINTER(vp), vp, vp, vp, vp, vp,
+                                           vp, vp]
+    L.dfm_multiview_lift_views_cl.argtypes = [POINTER(LiftDesc), POINTER(vp), vp, vp, vp, vp,
+                                              vp, vp, vp]
+    L.dfm_view_fingerprint.argtypes = [vp, c_int, c_longlong, vp, vp]
+    L.dfm_views_equal.argtypes = [POINTER(vp), POINTER(vp), c_int, c_longlong, vp, vp]
     L.dfm_neck_create.argtypes = [POINTER(NeckDesc), POINTER(vp)]
     L.dfm_neck_forward.argtypes = [vp, vp, vp, vp]
     L.dfm_neck_forward_cl.argtypes = [vp, vp, vp, vp]
@@ -245,6 +254,8 @@ def lib():
     L.dfm_liga_resnet_forward.argtypes = [vp, vp, POINTER(vp), vp]
     L.dfm_resnet101_create.argtypes = [POINTER(ResNet101Desc), POINTER(vp)]
     L.dfm_resnet101_forward.argtypes = [vp, vp, POINTER(vp), vp]
+    for f in ('fpn', 'liga_resnet', 'resnet101'):
+        getattr(L, f'dfm_{f}_set_num_images').argtypes = [vp, c_int]
     # the parameterised handle families share destroy / set_param / missing_params
     for f in ('backbone', 'neck', 'frustum', 'bev_hourglass', 'anchor_head', 'anchor3d_head',
               'stereo_tail', 'spp_neck', 'fpn', 'liga_resnet', 'resnet101'):

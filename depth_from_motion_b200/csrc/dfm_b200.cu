@@ -27,6 +27,7 @@
 #include "resnet101_kernels.cuh"
 #include "box_post_kernels.cuh"
 #include "image_prep_kernels.cuh"
+#include "view_cache_kernels.cuh"
 
 namespace {
 
@@ -1574,3 +1575,4 @@ int dfm_depth_head_forward(const float* d_cost, const float* d_depth_samples, in
 #include "resnet101_api.inc"
 #include "box_post_api.inc"
 #include "image_prep_api.inc"
+#include "view_cache_api.inc"

@@ -37,13 +37,10 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ in, float* __restr
 // pitch keeps both the (4 rows x 8 float4) store pattern and the (4 pixels x 8 channel
 // quads) gather pattern free of bank conflicts.  blockIdx.y walks a batch of images.
 template <int C>
-__global__ void __launch_bounds__(256)
-nchw_to_nhwc_v4_kernel(const float* __restrict__ in, float* __restrict__ out, long long HW,
-                       long long in_bstride, long long out_bstride) {
+__device__ __forceinline__ void nchw_to_nhwc_v4_tile(const float* __restrict__ src,
+                                                     float* __restrict__ dst, long long HW) {
   constexpr int TP = 128, P = TP + 1;
   __shared__ float tile[C * P];
-  const float* src = in + (long long)blockIdx.y * in_bstride;
-  float* dst = out + (long long)blockIdx.y * out_bstride;
   const long long p0 = (long long)blockIdx.x * TP;
   const int tid = threadIdx.x;
 #pragma unroll
@@ -67,6 +64,26 @@ nchw_to_nhwc_v4_kernel(const float* __restrict__ in, float* __restrict__ out, lo
       *reinterpret_cast<float4*>(dst + (p0 + px) * C + c) = make_float4(t[0], t[P], t[2 * P], t[3 * P]);
     }
   }
+}
+
+template <int C>
+__global__ void __launch_bounds__(256)
+nchw_to_nhwc_v4_kernel(const float* __restrict__ in, float* __restrict__ out, long long HW,
+                       long long in_bstride, long long out_bstride) {
+  nchw_to_nhwc_v4_tile<C>(in + (long long)blockIdx.y * in_bstride,
+                          out + (long long)blockIdx.y * out_bstride, HW);
+}
+
+// The same transpose of up to 16 separately allocated images (multi-view lifting's views,
+// some of them held by a feature cache): blockIdx.y indexes the pointer table.
+struct ViewTable {
+  const float* p[16];
+};
+template <int C>
+__global__ void __launch_bounds__(256)
+nchw_to_nhwc_v4_views_kernel(ViewTable in, float* __restrict__ out, long long HW,
+                             long long out_bstride) {
+  nchw_to_nhwc_v4_tile<C>(in.p[blockIdx.y], out + (long long)blockIdx.y * out_bstride, HW);
 }
 
 // channels-last [V][C] -> NCDHW [C][V]

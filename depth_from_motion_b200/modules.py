@@ -24,8 +24,10 @@ reference checkpoints load with ``strict=True``); their ``forward`` is never
 called.  There is no PyTorch fallback: without the built library or an H100 the
 modules raise.
 """
+import collections
 import copy
 import ctypes
+import itertools
 import os
 
 import numpy as np
@@ -57,6 +59,7 @@ def _check_cuda(t, name):
 
 
 _STRICT_PARAM_CHECK = bool(int(os.environ.get('DFM_PARAM_CHECK', '0')))
+_UPLOADS = itertools.count(1)
 
 
 class _ParamSync:
@@ -76,9 +79,21 @@ class _ParamSync:
     def __init__(self):
         self._sig = None
         self._finger = None
+        # a new value at every upload: the detectors' feature cache keeps the generation its
+        # entries were computed under (``_ViewFeatureCache``)
+        self.generation = 0
+        self._watch = ()
 
     def mark_dirty(self):
         self._sig = None
+
+    def pending(self):
+        """True when the next ``sync`` will upload, found without building the ``state_dict``:
+        ``mark_dirty`` was called, or a tensor of the last upload was replaced by another
+        object, written in place (version) or moved (storage pointer)."""
+        return self._sig is None or any(
+            owner.get(k) is not t or t.data_ptr() != p or t._version != v
+            for owner, k, t, p, v in self._watch)
 
     def signature(self, module):
         return tuple((k, v.data_ptr(), v._version)
@@ -103,6 +118,11 @@ class _ParamSync:
             set_fn(k.encode(), ctypes.c_void_p(h.data_ptr()), h.numel())
         self._sig = sig
         self._finger = finger
+        self.generation = next(_UPLOADS)
+        self._watch = tuple((owner, k, v, v.data_ptr(), v._version)
+                            for m in module.modules()
+                            for owner in (m._parameters, m._buffers)
+                            for k, v in owner.items() if v is not None)
 
 
 class _CudaMirror(nn.Module):
@@ -315,30 +335,48 @@ class DfMBackbone(_CudaMirror):
         assert b == 1, 'only support batch size 1 for now'
         assert c == self.in_channels
         assert prev_stereo_feats.shape == cur_stereo_feats.shape
-        L = self._prepare(h, w)
-        cur = cur_stereo_feats.contiguous()
-        prev = prev_stereo_feats.contiguous()
-        geom = geometry_from_meta(img_metas[0])
-        ho = round(h / self.cost_sample_factor)
-        wo = round(w / self.cost_sample_factor)
-        d = self.num_planes
-        dev = cur.device
-        cost = torch.empty((1, 1, d, ho, wo), device=dev, dtype=torch.float32)
-        stereo = torch.empty((1, self.cv_channels, d, ho, wo), device=dev,
-                             dtype=torch.float32)
-        mono = torch.empty_like(stereo)
         # stereo features that came out of our SPPUNetNeckTail carry a channels-last twin:
         # the plane-sweep loader reads it directly, no NCHW -> NHWC transposes
         cl_c = getattr(cur_stereo_feats, '_dfm_cl', None)
         cl_p = getattr(prev_stereo_feats, '_dfm_cl', None)
         if cl_c is not None and cl_p is not None and cl_c.shape == (h, w, c) == cl_p.shape:
-            capi.check(L.dfm_backbone_forward_cl(
-                self._handle, _ptr(cl_c), _ptr(cl_p), ctypes.byref(geom), _ptr(cost),
-                _ptr(stereo), _ptr(mono), _stream()), 'dfm_backbone_forward_cl')
-        else:
-            capi.check(L.dfm_backbone_forward(
-                self._handle, _ptr(cur), _ptr(prev), ctypes.byref(geom), _ptr(cost),
-                _ptr(stereo), _ptr(mono), _stream()), 'dfm_backbone_forward')
+            return self._forward_cl(cl_c, cl_p, img_metas)
+        L = self._prepare(h, w)
+        cur = cur_stereo_feats.contiguous()
+        prev = prev_stereo_feats.contiguous()
+        geom = geometry_from_meta(img_metas[0])
+        cost, stereo, mono = self._outputs(h, w, cur.device)
+        capi.check(L.dfm_backbone_forward(
+            self._handle, _ptr(cur), _ptr(prev), ctypes.byref(geom), _ptr(cost),
+            _ptr(stereo), _ptr(mono), _stream()), 'dfm_backbone_forward')
+        return self._finish(cost, stereo, mono)
+
+    def _outputs(self, h, w, dev):
+        ho = round(h / self.cost_sample_factor)
+        wo = round(w / self.cost_sample_factor)
+        d = self.num_planes
+        cost = torch.empty((1, 1, d, ho, wo), device=dev, dtype=torch.float32)
+        stereo = torch.empty((1, self.cv_channels, d, ho, wo), device=dev,
+                             dtype=torch.float32)
+        return cost, stereo, torch.empty_like(stereo)
+
+    def _forward_cl(self, cl_c, cl_p, img_metas):
+        """``forward`` on the channels-last twins ``[H, W, C]`` of the current and previous
+        stereo features alone (the detectors' feature cache holds only the twin)."""
+        _check_cuda(cl_c, 'cur_stereo_feats (channels-last)')
+        _check_cuda(cl_p, 'prev_stereo_feats (channels-last)')
+        h, w, c = cl_c.shape
+        assert c == self.in_channels and tuple(cl_p.shape) == (h, w, c)
+        assert cl_c.is_contiguous() and cl_p.is_contiguous()
+        L = self._prepare(h, w)
+        geom = geometry_from_meta(img_metas[0])
+        cost, stereo, mono = self._outputs(h, w, cl_c.device)
+        capi.check(L.dfm_backbone_forward_cl(
+            self._handle, _ptr(cl_c), _ptr(cl_p), ctypes.byref(geom), _ptr(cost),
+            _ptr(stereo), _ptr(mono), _stream()), 'dfm_backbone_forward_cl')
+        return self._finish(cost, stereo, mono)
+
+    def _finish(self, cost, stereo, mono):
         # the handle keeps a channels-last copy of stereo_feat until the next forward;
         # FrustumToVoxel reads it instead of transposing `stereo` again
         self._generation = getattr(self, '_generation', 0) + 1
@@ -1576,7 +1614,11 @@ class FPN(_HandleMirror):
         if b == 0:
             return outs
         L = capi.lib()
-        key = (b, tuple(sizes), self.conv_impl)
+        key = (tuple(sizes), self.conv_impl)
+        if self._handle is not None and key == self._key and b != self._batch:
+            # another batch size keeps the handle and its uploaded parameters
+            capi.check(L.dfm_fpn_set_num_images(self._handle, b), 'dfm_fpn_set_num_images')
+            self._batch = b
         if self._handle is None or key != self._key:
             self.release()
             desc = capi.FpnDesc()
@@ -1587,7 +1629,7 @@ class FPN(_HandleMirror):
             desc.num_images, desc.conv_impl = b, _IMPL[self.conv_impl]
             hd = ctypes.c_void_p()
             capi.check(L.dfm_fpn_create(ctypes.byref(desc), ctypes.byref(hd)), 'dfm_fpn_create')
-            self._handle, self._key = hd, key
+            self._handle, self._key, self._batch = hd, key, b
             self._sync = _ParamSync()
         self._sync.sync(self, lambda k, p, m: capi.check(
             L.dfm_fpn_set_param(self._handle, k, p, m), f'dfm_fpn_set_param({k.decode()})'))
@@ -1719,14 +1761,19 @@ class LIGAResNet(_HandleMirror):
         if b == 0:
             return outs
         L = capi.lib()
-        key = (b, h, w, self.conv_impl)
+        key = (h, w, self.conv_impl)
+        if self._handle is not None and key == self._key and b != self._batch:
+            # another batch size keeps the handle and its uploaded parameters
+            capi.check(L.dfm_liga_resnet_set_num_images(self._handle, b),
+                       'dfm_liga_resnet_set_num_images')
+            self._batch = b
         if self._handle is None or key != self._key:
             self.release()
             desc = capi.LigaResNetDesc(h, w, b, _IMPL[self.conv_impl])
             hd = ctypes.c_void_p()
             capi.check(L.dfm_liga_resnet_create(ctypes.byref(desc), ctypes.byref(hd)),
                        'dfm_liga_resnet_create')
-            self._handle, self._key = hd, key
+            self._handle, self._key, self._batch = hd, key, b
             self._sync = _ParamSync()
         self._sync.sync(self, lambda k, p, m: capi.check(
             L.dfm_liga_resnet_set_param(self._handle, k, p, m),
@@ -1880,14 +1927,19 @@ class ResNet(_HandleMirror):
         if b == 0:
             return outs
         L = capi.lib()
-        key = (b, h, w, self.conv_impl)
+        key = (h, w, self.conv_impl)
+        if self._handle is not None and key == self._key and b != self._batch:
+            # another batch size keeps the handle and its uploaded parameters
+            capi.check(L.dfm_resnet101_set_num_images(self._handle, b),
+                       'dfm_resnet101_set_num_images')
+            self._batch = b
         if self._handle is None or key != self._key:
             self.release()
             desc = capi.ResNet101Desc(h, w, b, _IMPL[self.conv_impl])
             hd = ctypes.c_void_p()
             capi.check(L.dfm_resnet101_create(ctypes.byref(desc), ctypes.byref(hd)),
                        'dfm_resnet101_create')
-            self._handle, self._key = hd, key
+            self._handle, self._key, self._batch = hd, key, b
             self._sync = _ParamSync()
         self._sync.sync(self, lambda k, p, m: capi.check(
             L.dfm_resnet101_set_param(self._handle, k, p, m),
@@ -1944,14 +1996,23 @@ def multiview_lift(feats, img_meta, n_voxels, voxel_range, num_views,
                    num_frames, temporal_aggregate='mean', out=None, channels_last=True):
     """The lifting loop of MultiViewDfM.feature_transformation
     (multiview_dfm.py:139-209, valid_sample=True) for one sample.
-    feats: [T*Nv, C, Hf, Wf] CUDA -> [C(*T), Nx, Ny, Nz].  The returned tensor has the
+    feats: [T*Nv, C, Hf, Wf] CUDA, or a sequence of T*Nv [C, Hf, Wf] CUDA views anywhere in
+    memory (the kernel reads them through a pointer table, so cached and freshly computed views
+    are lifted without a concatenation) -> [C(*T), Nx, Ny, Nz].  The returned tensor has the
     reference's shape but channels-last strides (memory [Nx, Ny, Nz, C]): that is what the
     necks' conv loaders read, so neither the lifting kernel's stores nor the neck pay for a
     layout change.  ``out``: optional contiguous [Nx, Ny, Nz, C(*T)] CUDA buffer to fill.
     ``channels_last=False`` runs the reference-layout kernel (contiguous [C, Nx, Ny, Nz])."""
-    _check_cuda(feats, 'feats')
-    s, c, hf, wf = feats.shape
+    views = list(feats)
+    for i, v in enumerate(views):
+        _check_cuda(v, f'feats[{i}]')
+    s = len(views)
+    c, hf, wf = views[0].shape
     assert s == num_views * num_frames
+    assert all(tuple(v.shape) == (c, hf, wf) for v in views)
+    views = [v.contiguous() for v in views]
+    table = (ctypes.c_void_p * s)(*[v.data_ptr() for v in views])
+    dev = views[0].device
     _require_identity_3d_aug(img_meta)
     sf = img_meta.get('scale_factor', 1.0)
     sf = np.atleast_1d(np.asarray(sf, dtype=np.float32))
@@ -1978,26 +2039,26 @@ def multiview_lift(feats, img_meta, n_voxels, voxel_range, num_views,
     if not channels_last:
         assert out is None
         vol = torch.empty((cout, n_voxels[0], n_voxels[1], n_voxels[2]),
-                          device=feats.device, dtype=torch.float32)
-        capi.check(capi.lib().dfm_multiview_lift(
-            ctypes.byref(desc), _ptr(feats.contiguous()),
+                          device=dev, dtype=torch.float32)
+        capi.check(capi.lib().dfm_multiview_lift_views(
+            ctypes.byref(desc), table,
             proj.ctypes.data_as(ctypes.c_void_p),
             img_w.ctypes.data_as(ctypes.c_void_p),
             ctypes.c_void_p(xs.data_ptr()), ctypes.c_void_p(ys.data_ptr()),
             ctypes.c_void_p(zs.data_ptr()), _ptr(vol), _stream()),
-            'dfm_multiview_lift')
+            'dfm_multiview_lift_views')
         return vol
     shape_cl = (n_voxels[0], n_voxels[1], n_voxels[2], cout)
     if out is None:
-        out = torch.empty(shape_cl, device=feats.device, dtype=torch.float32)
+        out = torch.empty(shape_cl, device=dev, dtype=torch.float32)
     assert tuple(out.shape) == shape_cl and out.is_contiguous() and out.is_cuda
-    capi.check(capi.lib().dfm_multiview_lift_cl(
-        ctypes.byref(desc), _ptr(feats.contiguous()),
+    capi.check(capi.lib().dfm_multiview_lift_views_cl(
+        ctypes.byref(desc), table,
         proj.ctypes.data_as(ctypes.c_void_p),
         img_w.ctypes.data_as(ctypes.c_void_p),
         ctypes.c_void_p(xs.data_ptr()), ctypes.c_void_p(ys.data_ptr()),
         ctypes.c_void_p(zs.data_ptr()), _ptr(out), _stream()),
-        'dfm_multiview_lift_cl')
+        'dfm_multiview_lift_views_cl')
     return out.permute(3, 0, 1, 2)
 
 
@@ -2069,10 +2130,12 @@ class MultiViewDfMFeatureTransformation:
         if not getattr(self, 'valid_sample', True):
             raise NotImplementedError('valid_sample=False is not implemented')
         nvx = list(self.n_voxels)
-        cout = batch_feats[0].shape[1] * (num_frames if self.temporal_aggregate == 'concat' else 1)
+        # batch_feats: [B, T*Nv, C, Hf, Wf], or per sample a list of T*Nv [C, Hf, Wf] views
+        view0 = batch_feats[0][0]
+        cout = view0.shape[0] * (num_frames if self.temporal_aggregate == 'concat' else 1)
         # one channels-last buffer for the batch; the reference-shaped view is returned
         buf = torch.empty((len(batch_feats), nvx[0], nvx[1], nvx[2], cout),
-                          device=batch_feats[0].device, dtype=torch.float32)
+                          device=view0.device, dtype=torch.float32)
         for b, (feature, img_meta) in enumerate(zip(batch_feats, img_metas)):   # :128
             meta = dict(img_meta)
             if 'scale_factor' not in meta:                           # :129-138
@@ -2083,6 +2146,127 @@ class MultiViewDfMFeatureTransformation:
         if getattr(self, 'with_neck_3d', self.neck_3d is not None):
             volume_feat = self.neck_3d(volume_feat)[0]               # :263
         return (volume_feat, )                                       # :265-268
+
+
+# ---------------------------------------------------------------------------------------------
+# Per-view image-feature cache of the detectors
+# ---------------------------------------------------------------------------------------------
+_U64 = (1 << 64) - 1
+
+
+def _view_fingerprints(batch):
+    """[N, ...] contiguous fp32 CUDA views -> N hashable 128-bit fingerprints (one launch of
+    ``dfm_view_fingerprint``, one device-to-host copy)."""
+    n = batch.shape[0]
+    out = torch.empty((n, 2), dtype=torch.int64, device=batch.device)
+    capi.check(capi.lib().dfm_view_fingerprint(_ptr(batch), n, batch[0].numel(), _ptr(out),
+                                               _stream()), 'dfm_view_fingerprint')
+    return [(a & _U64, b & _U64) for a, b in out.cpu().tolist()]
+
+
+def _views_equal(pairs):
+    """[(a, b)] of equally shaped fp32 CUDA views -> [bool]: bitwise equality of each pair (one
+    launch of ``dfm_views_equal``, one device-to-host copy)."""
+    n = len(pairs)
+    a = (ctypes.c_void_p * n)(*[x.data_ptr() for x, _ in pairs])
+    b = (ctypes.c_void_p * n)(*[y.data_ptr() for _, y in pairs])
+    mismatch = torch.empty(n, dtype=torch.int32, device=pairs[0][0].device)
+    capi.check(capi.lib().dfm_views_equal(a, b, n, pairs[0][0].numel(), _ptr(mismatch),
+                                          _stream()), 'dfm_views_equal')
+    return [m == 0 for m in mismatch.cpu().tolist()]
+
+
+def _as_batch(views):
+    """Equally shaped contiguous views -> one [N, ...] tensor: a view of their storage when
+    they lie back to back in it (a run of one ``img``), else a stacked copy."""
+    v0 = views[0]
+    step = v0.numel() * v0.element_size()
+    if all(v.is_contiguous() and v.untyped_storage().data_ptr() == v0.untyped_storage().data_ptr()
+           and v.data_ptr() == v0.data_ptr() + i * step for i, v in enumerate(views)):
+        return torch.as_strided(v0, (len(views),) + tuple(v0.shape),
+                                (v0.numel(),) + tuple(v0.stride()))
+    return torch.stack(views)
+
+
+class _ViewFeatureCache:
+    """Image features of single input views, keyed by the view's exact content.
+
+    An entry holds a copy of the view (callers may overwrite their input buffer), what the
+    detector keeps of its features, and the state of the image modules it was computed under.
+    The fingerprint only finds a candidate: a view is served from an entry only when it is
+    bitwise equal to the entry's copy.  Least recently used entries go first; a hit refreshes
+    its entry.  ``max_views`` counts entries."""
+
+    def __init__(self, max_views):
+        self.max_views = max_views
+        self.entries = collections.OrderedDict()   # (shape, fingerprint) -> [view, feat, state]
+        self.hits = self.misses = self.rejected = 0
+
+    def clear(self):
+        self.entries.clear()
+
+    def stats(self):
+        nbytes = sum(t.numel() * t.element_size() for e in self.entries.values() for t in e[:2])
+        return dict(hits=self.hits, misses=self.misses, rejected=self.rejected,
+                    views=len(self.entries), bytes=nbytes)
+
+    def run(self, batch, compute, state, forced=()):
+        """batch: [N, ...] contiguous views.  ``compute(views)`` returns, for a list of views,
+        a list of ``(kept, extra)``: ``kept`` is stored, ``extra`` only handed back.  Views in
+        ``forced`` are always computed (the caller needs their ``extra``).  Returns per view
+        ``(kept, extra)``, ``extra`` None unless the view was computed in this call.  The
+        missing views go to one ``compute`` call; a view equal to another view of the same call
+        is computed once.  ``state(check)`` is the state of the modules that compute features
+        (``check``: first empty the cache if a parameter upload is already due): entries
+        recorded under another state are dropped, and new entries record the state after
+        ``compute``."""
+        views = list(batch)
+        shape = tuple(batch.shape[1:])
+        keys = [(shape,) + tuple(k) for k in _view_fingerprints(batch)]
+        now = state(True)
+        first = {}                    # key -> the view of this call that stands for it
+        checks = []                   # (view index, the view it may equal, from the cache?)
+        for i in sorted(range(len(views)), key=lambda i: i not in forced):
+            k = keys[i]
+            if k in first:
+                checks.append((i, views[first[k]], False))
+                continue
+            first[k] = i
+            e = self.entries.get(k)
+            if e is not None and e[2] != now:
+                del self.entries[k]
+            elif e is not None and i not in forced:
+                checks.append((i, e[0], True))
+        equal = _views_equal([(views[i], other) for i, other, _ in checks]) if checks else []
+        result = [None] * len(views)
+        same_as = {}
+        for (i, _, cached), ok in zip(checks, equal):
+            if not ok:
+                self.rejected += 1
+            elif cached:
+                self.entries.move_to_end(keys[i])
+                result[i] = (self.entries[keys[i]][1], None)
+            else:
+                same_as[i] = first[keys[i]]
+        todo = [i for i in range(len(views)) if result[i] is None and i not in same_as]
+        if todo:
+            for i, r in zip(todo, compute([views[i] for i in todo])):
+                result[i] = r
+            after = state(False)
+            for i in todo:
+                if first[keys[i]] == i:       # a colliding twin of this call is not kept
+                    kept = result[i][0]
+                    if kept.untyped_storage().nbytes() != kept.numel() * kept.element_size():
+                        kept = kept.clone()   # a view into a batch would keep the whole batch
+                    self.entries.pop(keys[i], None)
+                    self.entries[keys[i]] = [views[i].clone(), kept, after]
+            while len(self.entries) > self.max_views:
+                self.entries.popitem(last=False)
+        for i, j in same_as.items():
+            result[i] = (result[j][0], None)
+        self.hits += len(views) - len(todo)
+        self.misses += len(todo)
+        return result
 
 
 # ---------------------------------------------------------------------------------------------
@@ -2149,6 +2333,48 @@ class DfM(nn.Module):
         if bbox_head_3d['type'] == 'LIGAAnchor3DHead':
             bbox_head_3d.update(normalizer_clamp_value=normalizer_clamp_value)
         self.bbox_head_3d = build_head(bbox_head_3d)
+        self._feature_cache = None
+
+    # ---- per-view image-feature cache ----------------------------------------------------
+    def set_feature_cache(self, max_views):
+        """Reuse image features across ``simple_test`` calls, for video.  A view of ``img``
+        whose content is bitwise equal to a view an earlier call computed (within the last
+        ``max_views`` distinct views) takes that call's features instead of going through the
+        image backbone and neck again; the results are bitwise those of a run without the
+        cache.  DfM keeps the stereo feature's channels-last twin of each frame (current
+        frames are always computed, previous frames are looked up); MultiViewDfM keeps FPN
+        level 0 of every view of a multi-frame config (the single-frame camsync config never
+        uses the cache).  ``0`` (the default) turns it off.  Every call empties the cache."""
+        max_views = int(max_views)
+        if max_views < 0:
+            raise ValueError(f'max_views must be >= 0, got {max_views}')
+        self._feature_cache = _ViewFeatureCache(max_views) if max_views else None
+
+    def feature_cache_stats(self):
+        """``dict(hits, misses, rejected, views, bytes)`` since ``set_feature_cache``: views
+        served without computing / views computed / fingerprint matches that failed the
+        bitwise check; entries held and their device bytes (view copies and features)."""
+        c = self._feature_cache
+        if c is None:
+            return dict(hits=0, misses=0, rejected=0, views=0, bytes=0)
+        return c.stats()
+
+    def _feature_cache_state(self, device, check=True):
+        """What cached features depend on besides the view: the image modules' parameter
+        uploads and conv_impl, and the device.  With ``check``, an upload that is already due
+        (``train()``, ``load_state_dict``, ``sync_params()``, a parameter written in place,
+        replaced or moved) empties the cache at once."""
+        mods = (self.backbone, self.neck)
+        syncs = [getattr(m, '_sync', None) for m in mods]
+        if check and any(sy is not None and sy.pending() for sy in syncs):
+            self._feature_cache.clear()
+        return (str(device),) + tuple((m.conv_impl, sy.generation if sy is not None else 0)
+                                      for m, sy in zip(mods, syncs))
+
+    def train(self, mode=True):
+        if getattr(self, '_feature_cache', None) is not None:
+            self._feature_cache.clear()
+        return super().train(mode)
 
     @property
     def with_backbone_3d(self):
@@ -2205,22 +2431,43 @@ class DfM(nn.Module):
         """dfm.py:264-298 for one sample (the stereo backbone takes B == 1).  The cur / prev
         pair goes through LIGAResNet in one call (eval BatchNorm: equal to two calls); the
         reference's device copy of ``cur2prevs`` stays a host tensor, which is what the stereo
-        backbone reads, so no host synchronisation is added."""
+        backbone reads, so no host synchronisation is added.  With the feature cache on, the
+        previous frame's stereo feature may come from an earlier call."""
         pair = img[0, :2].contiguous()
-        feats = self.backbone(pair)
-        cur_feats = [pair[0:1]] + [f[0:1] for f in feats]
-        prev_feats = [pair[1:2]] + [f[1:2] for f in feats]
-        cur_stereo_feat, cur_sem_feat = self.neck(cur_feats)
-        prev_stereo_feat, _ = self.neck(prev_feats)      # prev semantic feature unused (:283)
+        if self._feature_cache is None:
+            feats = self.backbone(pair)
+            cur_feats = [pair[0:1]] + [f[0:1] for f in feats]
+            prev_feats = [pair[1:2]] + [f[1:2] for f in feats]
+            cur_stereo_feat, cur_sem_feat = self.neck(cur_feats)
+            prev_stereo_feat, _ = self.neck(prev_feats)      # prev semantic feature unused (:283)
+        else:
+            (cur_cl, cur_sem_feat), (prev_cl, _) = self._feature_cache.run(
+                pair, self._stereo_twins, lambda check: self._feature_cache_state(img.device, check),
+                forced=(0,))
         for meta in img_metas:
             c2p = meta['cur2prevs']
             if isinstance(c2p, torch.Tensor):   # e.g. metas already through extract_feat
                 c2p = c2p.detach().cpu()
             meta['cur2prevs'] = torch.as_tensor(np.asarray(c2p, dtype=np.float64),
                                                 dtype=img.dtype)
-        costs, stereo_feats, mono_feats = self.backbone_stereo(cur_stereo_feat,
-                                                               prev_stereo_feat, img_metas)
+        if self._feature_cache is not None:
+            costs, stereo_feats, mono_feats = self.backbone_stereo._forward_cl(
+                cur_cl, prev_cl, img_metas)
+        else:
+            costs, stereo_feats, mono_feats = self.backbone_stereo(cur_stereo_feat,
+                                                                   prev_stereo_feat, img_metas)
         return costs, stereo_feats, mono_feats, cur_sem_feat
+
+    def _stereo_twins(self, views):
+        """The feature function of DfM's cache: [3, H, W] views through LIGAResNet in one call
+        and SPPUNetNeck one by one -> ``(stereo twin [H, W, 32], semantic feature)`` each."""
+        x = _as_batch(views)
+        feats = self.backbone(x)
+        out = []
+        for i in range(len(views)):
+            stereo, sem = self.neck([x[i:i + 1]] + [f[i:i + 1] for f in feats])
+            out.append((stereo._dfm_cl, sem))
+        return out
 
     def _head_outputs(self, img, img_metas):
         """dfm.py:416-432 up to the head, sample by sample; DepthHead is fused into
@@ -2292,10 +2539,23 @@ class MultiViewDfM(MultiViewDfMFeatureTransformation, DfM):
         input_shape = img.shape[-2:]
         for img_meta in img_metas:
             img_meta.update(input_shape=input_shape)
+        if self._feature_cache is not None and num_frames > 1:
+            got = self._feature_cache.run(
+                img.reshape(-1, c_in, h, w).contiguous(), self._fpn_level0,
+                lambda check: self._feature_cache_state(img.device, check))
+            s = img.shape[1]
+            batch_feats = [[got[b * s + j][0] for j in range(s)] for b in range(batch_size)]
+            return self.feature_transformation(batch_feats, img_metas, num_views, num_frames)
         feats = self.neck(self.backbone(img.reshape(-1, c_in, h, w)))[0]
         _, c_feat, h_feat, w_feat = feats.shape
         batch_feats = feats.view(batch_size, -1, c_feat, h_feat, w_feat)
         return self.feature_transformation(batch_feats, img_metas, num_views, num_frames)
+
+    def _fpn_level0(self, views):
+        """The feature function of MultiViewDfM's cache: views through ResNet and FPN in one
+        call -> FPN level 0 ``[64, H/4, W/4]`` of each."""
+        f0 = self.neck(self.backbone(_as_batch(views)))[0]
+        return [(f0[i], None) for i in range(len(views))]
 
     def simple_test(self, img, img_metas):
         """multiview_dfm.py:321-341: ``[dict(boxes_3d, scores_3d, labels_3d)]`` per sample.

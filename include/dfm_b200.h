@@ -210,6 +210,17 @@ int dfm_multiview_lift_cl(const dfm_lift_desc_t* desc, const float* d_feats,
                           const double* h_lidar2img, const int* h_img_w, const float* h_xs,
                           const float* h_ys, const float* h_zs, float* d_volume_cl,
                           void* stream);
+/* The same two liftings with the T*Nv views at separate addresses: h_view_feats is a host
+ * array of T*Nv device pointers, each to one NCHW [C][Hf][Wf] view (current frame's views
+ * first).  Values are bit-identical to the contiguous forms above, which build this table. */
+int dfm_multiview_lift_views(const dfm_lift_desc_t* desc, const float* const* h_view_feats,
+                             const double* h_lidar2img, const int* h_img_w, const float* h_xs,
+                             const float* h_ys, const float* h_zs, float* d_volume,
+                             void* stream);
+int dfm_multiview_lift_views_cl(const dfm_lift_desc_t* desc, const float* const* h_view_feats,
+                                const double* h_lidar2img, const int* h_img_w, const float* h_xs,
+                                const float* h_ys, const float* h_zs, float* d_volume_cl,
+                                void* stream);
 
 /* ------------------------------------------------------------------------------------
  * DfMNeck / OutdoorImVoxelNeck, eval mode (mmdet3d/models/necks/dfm_neck.py:10-122,
@@ -522,6 +533,10 @@ typedef struct dfm_fpn_desc {
 } dfm_fpn_desc_t;
 int dfm_fpn_create(const dfm_fpn_desc_t* desc, dfm_fpn_t** out);
 int dfm_fpn_destroy(dfm_fpn_t* f);
+/* Sets the number of images the next forwards take, keeping the handle and its parameters
+ * (buffers grow at the next forward when needed).  DFM_ERR_INVALID when num_images < 1 or the
+ * batch exceeds the limits create checks. */
+int dfm_fpn_set_num_images(dfm_fpn_t* f, int num_images);
 /* Keys: "lateral_convs.{0..3}.conv.{weight,bias}" (weights (out, in_l, 1, 1)) and
  * "fpn_convs.{0..3}.conv.{weight,bias}" (weights (out, out, 3, 3)); a wrong numel fails with
  * DFM_ERR_INVALID. */
@@ -558,6 +573,10 @@ typedef struct dfm_liga_resnet_desc {
 } dfm_liga_resnet_desc_t;
 int dfm_liga_resnet_create(const dfm_liga_resnet_desc_t* desc, dfm_liga_resnet_t** out);
 int dfm_liga_resnet_destroy(dfm_liga_resnet_t* r);
+/* Sets the number of images the next forwards take, keeping the handle and its parameters
+ * (buffers grow at the next forward when needed).  DFM_ERR_INVALID when num_images < 1 or the
+ * batch exceeds the limits create checks. */
+int dfm_liga_resnet_set_num_images(dfm_liga_resnet_t* r, int num_images);
 /* Keys are the reference state_dict's: "conv1.weight", "bn1.{weight,bias,running_mean,
  * running_var}", "layer{1..4}.{j}.conv{1,2}.weight", "layer{1..4}.{j}.bn{1,2}.*",
  * "layer2.0.downsample.0.weight", "layer2.0.downsample.1.*" ("num_batches_tracked" is not
@@ -596,6 +615,10 @@ typedef struct dfm_resnet101_desc {
 } dfm_resnet101_desc_t;
 int dfm_resnet101_create(const dfm_resnet101_desc_t* desc, dfm_resnet101_t** out);
 int dfm_resnet101_destroy(dfm_resnet101_t* r);
+/* Sets the number of images the next forwards take, keeping the handle and its parameters
+ * (buffers grow at the next forward when needed).  DFM_ERR_INVALID when num_images < 1 or the
+ * batch exceeds the limits create checks. */
+int dfm_resnet101_set_num_images(dfm_resnet101_t* r, int num_images);
 /* Keys are mmdet's state_dict's: "conv1.weight", "bn1.{weight,bias,running_mean,running_var}",
  * "layer{1..4}.{j}.conv{1,2,3}.weight", "layer{1..4}.{j}.bn{1,2,3}.*",
  * "layer{3,4}.{j}.conv2.conv_offset.{weight,bias}", "layer{1..4}.0.downsample.0.weight",
@@ -703,6 +726,23 @@ int dfm_image_prep(const dfm_image_prep_desc_t* desc, const unsigned char* d_src
  * lifting staging, the host-copy side stream) and the profiling record are shared by all
  * handles of a device and are NOT locked -- the same one-thread-per-process model as the
  * reference (tools/slurm_train.sh:15-24, SURVEY.md section 8b "Threading"). */
+
+/* ------------------------------------------------------------------------------------
+ * The per-view image-feature cache of the detectors (modules.DfM.set_feature_cache).
+ *
+ * dfm_view_fingerprint: a 128-bit fingerprint of each of num_views consecutive views of
+ * view_elems fp32 elements (d_views 4-byte aligned), in one launch.  d_out[v][0..1] are two
+ * 64-bit lanes: lane j is the sum modulo 2^64 over elements i of y ^ (y >> 32), y =
+ * (((bits(x_i) << 32) ^ i ^ K_j) * M_j) mod 2^64 (view_cache_kernels.cuh).  The raw bits are hashed, so
+ * -0.0 != +0.0 and NaN payloads count; the result does not depend on thread order.
+ * ---------------------------------------------------------------------------------- */
+int dfm_view_fingerprint(const float* d_views, int num_views, long long view_elems,
+                         unsigned long long* d_out /* [num_views][2] */, void* stream);
+/* Compares num_pairs view pairs of view_elems fp32 elements bit for bit (h_a / h_b: host
+ * arrays of device pointers).  d_mismatch[i] = 1 when pair i differs in any bit, else 0.  One
+ * launch per 64 pairs. */
+int dfm_views_equal(const float* const* h_a, const float* const* h_b, int num_pairs,
+                    long long view_elems, int* d_mismatch, void* stream);
 
 #ifdef __cplusplus
 }
