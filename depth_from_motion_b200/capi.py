@@ -58,7 +58,8 @@ SYMBOLS = (
     'dfm_box_post_debug_tensor', 'dfm_op_rotated_iou', 'dfm_image_prep',
     'dfm_multiview_lift_views', 'dfm_multiview_lift_views_cl', 'dfm_view_fingerprint',
     'dfm_views_equal', 'dfm_fpn_set_num_images', 'dfm_liga_resnet_set_num_images',
-    'dfm_resnet101_set_num_images',
+    'dfm_resnet101_set_num_images', 'dfm_kitti_eval_create', 'dfm_kitti_eval_destroy',
+    'dfm_kitti_eval_forward', 'dfm_kitti_eval_debug_tensor', 'dfm_op_eval_rotated_iou',
 )
 
 DFM_IMAGE_PREP_CROP, DFM_IMAGE_PREP_RESCALE = 0, 1
@@ -155,6 +156,13 @@ class ImagePrepDesc(ctypes.Structure):
     _fields_ = [(n, c_int) for n in ('mode', 'num_views', 'src_h', 'src_w', 'crop_x', 'crop_y',
                                      'out_h', 'out_w', 'pad_divisor', 'to_rgb')] + \
                [('mean', c_double * 3), ('std', c_double * 3)]
+
+
+class KittiEvalDesc(ctypes.Structure):
+    """``dfm_kitti_eval_desc_t``."""
+    _fields_ = [('num_classes', c_int), ('classes', c_int * 3), ('num_metrics', c_int),
+                ('metrics', c_int * 3), ('compute_aos', c_int), ('f32_flags', c_int),
+                ('min_overlap', c_double * 18)]
 
 
 class VoxelSampleDesc(ctypes.Structure):
@@ -270,6 +278,11 @@ def lib():
     L.dfm_box_post_forward.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.dfm_op_rotated_iou.argtypes = [vp, vp, c_int, vp, vp]
     L.dfm_voxel_sample.argtypes = [POINTER(VoxelSampleDesc), vp, vp, POINTER(c_double), vp, vp]
+    L.dfm_kitti_eval_create.argtypes = [POINTER(KittiEvalDesc), POINTER(vp)]
+    L.dfm_kitti_eval_destroy.argtypes = [vp]
+    L.dfm_kitti_eval_forward.argtypes = [vp, c_int, c_int, c_int, c_longlong] + [vp] * 10 + [vp]
+    L.dfm_kitti_eval_debug_tensor.argtypes = [vp, c_char_p, vp, c_longlong, vp]
+    L.dfm_op_eval_rotated_iou.argtypes = [vp, vp, c_int, c_int, c_int, vp, vp]
     L.dfm_image_prep.argtypes = [POINTER(ImagePrepDesc), vp, vp, vp]
     _lib = L
     return L

@@ -28,6 +28,7 @@
 #include "box_post_kernels.cuh"
 #include "image_prep_kernels.cuh"
 #include "view_cache_kernels.cuh"
+#include "kitti_eval_kernels.cuh"
 
 namespace {
 
@@ -1576,3 +1577,4 @@ int dfm_depth_head_forward(const float* d_cost, const float* d_depth_samples, in
 #include "box_post_api.inc"
 #include "image_prep_api.inc"
 #include "view_cache_api.inc"
+#include "kitti_eval_api.inc"

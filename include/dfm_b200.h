@@ -692,6 +692,55 @@ int dfm_box_post_debug_tensor(dfm_box_post_t* h, const char* name, int* d_out, l
 int dfm_op_rotated_iou(const float* d_a, const float* d_b, int n, float* d_iou, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * KITTI evaluation (mmdet3d kitti_utils/eval.py: eval_class of every requested metric) of N
+ * frames of ground truth and detections in CSR form.  Per box, fp64:
+ *   gt [num_gt][14]: bbox[4] alpha location[3] dimensions[3] rotation_y occluded truncated
+ *   dt [num_dt][13]: bbox[4] alpha location[3] dimensions[3] rotation_y score
+ * gt_code: class id (0 Car, 1 Pedestrian, 2 Cyclist, 3 Van, 4 Person_sitting, 7 other), plus 8
+ * when the name is exactly "DontCare"; dt_code: class id.  gt_off / dt_off [N + 1] int32,
+ * pair_off [N + 1] int64 (sum of dt * gt counts of earlier frames), num_pairs = pair_off[N].
+ * A config is (metric slot, class slot, difficulty, overlap set), index
+ * ((m * num_classes + c) * 3 + difficulty) * 2 + k; there are num_metrics * num_classes * 6.
+ * ---------------------------------------------------------------------------------- */
+typedef struct dfm_kitti_eval dfm_kitti_eval_t;
+typedef struct dfm_kitti_eval_desc {
+  int num_classes;               /* 1..3                                                  */
+  int classes[3];                /* 0 Car, 1 Pedestrian, 2 Cyclist                         */
+  int num_metrics;               /* 1..3                                                  */
+  int metrics[3];                /* ascending: 0 bbox, 1 bev, 2 3d                         */
+  int compute_aos;               /* AOS similarity on the bbox metric                      */
+  int f32_flags;                 /* input arrays the caller held as float32: 1 gt bbox, 2 dt
+                                    bbox, 4 gt 3-D box, 8 dt 3-D box, 16 gt (bbox, alpha),
+                                    32 dt (bbox, alpha, score)                              */
+  double min_overlap[3][3][2];   /* [metric slot][class slot][overlap set]                 */
+} dfm_kitti_eval_desc_t;
+int dfm_kitti_eval_create(const dfm_kitti_eval_desc_t* desc, dfm_kitti_eval_t** out);
+int dfm_kitti_eval_destroy(dfm_kitti_eval_t* h);
+/* d_pr: device [configs][41][4] fp64 (tp, fp, fn, similarity per threshold; zero past the
+ * count); d_thr_count: device [configs] int32, 42 when a config has more thresholds than the
+ * reference's 41-point arrays hold; d_status: device int32, 0 on success, bit 0 set when a
+ * frame holds more than 1024 detections (the limit per frame; such a frame is not evaluated
+ * and the counts are not valid).  The caller reads d_status after the stream completes.
+ * The workspace grows on demand. */
+int dfm_kitti_eval_forward(dfm_kitti_eval_t* h, int num_frames, int num_gt, int num_dt,
+                           long long num_pairs, const double* d_gt, const int* d_gt_code,
+                           const int* d_gt_off, const double* d_dt, const int* d_dt_code,
+                           const int* d_dt_off, const long long* d_pair_off, double* d_pr,
+                           int* d_thr_count, int* d_status, void* stream);
+/* Test hook, from the last forward: "overlap<metric>" fp64 [num_pairs] ([dt][gt] per frame),
+ * "tp_scores" fp64 [configs][S] (each config's TP scores sorted descending, S = the power of
+ * two >= num_gt), "tp_count" int32 [configs], "thresholds" fp64 [configs][41],
+ * "num_valid_gt" int32 [num_classes * 3].  DFM_ERR_STATE before a forward, DFM_ERR_INVALID on
+ * an unknown name or a wrong element count. */
+int dfm_kitti_eval_debug_tensor(dfm_kitti_eval_t* h, const char* name, void* d_out,
+                                long long numel, void* stream);
+/* rotate_iou_gpu_eval: d_iou [n][k] = IoU of (d_qboxes[k], d_boxes[n]) by criterion (-1 IoU,
+ * 0 / 1 over the first / second box's area, 2 intersection area); boxes [.][5] fp32
+ * (x, z, l, w, ry) in camera BEV. */
+int dfm_op_eval_rotated_iou(const float* d_boxes, const float* d_qboxes, int n, int k,
+                            int criterion, float* d_iou, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Image preparation of the shipped test pipelines, one launch per batch of views.
  * d_src: num_views decoded 8-bit BGR images, [num_views][src_h][src_w][3], all one size.
  * d_out: [num_views][3][pad_h][pad_w] fp32, pad_h / pad_w = out_h / out_w rounded up to
