@@ -14,7 +14,8 @@ DEPS = [os.path.join(HERE, 'csrc', f) for f in
          'liga_resnet_api.inc', 'resnet101_kernels.cuh', 'resnet101_api.inc',
          'box_post_kernels.cuh', 'box_post_api.inc', 'image_prep_kernels.cuh',
          'image_prep_api.inc', 'view_cache_kernels.cuh', 'view_cache_api.inc',
-         'kitti_eval_kernels.cuh', 'kitti_eval_api.inc')] + [os.path.join(HERE, '..', 'include', 'dfm_b200.h')]
+         'kitti_eval_kernels.cuh', 'kitti_eval_api.inc', 'waymo_eval_kernels.cuh',
+         'waymo_eval_api.inc')] + [os.path.join(HERE, '..', 'include', 'dfm_b200.h')]
 
 
 def nvcc_path():

@@ -60,6 +60,7 @@ SYMBOLS = (
     'dfm_views_equal', 'dfm_fpn_set_num_images', 'dfm_liga_resnet_set_num_images',
     'dfm_resnet101_set_num_images', 'dfm_kitti_eval_create', 'dfm_kitti_eval_destroy',
     'dfm_kitti_eval_forward', 'dfm_kitti_eval_debug_tensor', 'dfm_op_eval_rotated_iou',
+    'dfm_op_let_iou',
 )
 
 DFM_IMAGE_PREP_CROP, DFM_IMAGE_PREP_RESCALE = 0, 1
@@ -283,6 +284,7 @@ def lib():
     L.dfm_kitti_eval_forward.argtypes = [vp, c_int, c_int, c_int, c_longlong] + [vp] * 10 + [vp]
     L.dfm_kitti_eval_debug_tensor.argtypes = [vp, c_char_p, vp, c_longlong, vp]
     L.dfm_op_eval_rotated_iou.argtypes = [vp, vp, c_int, c_int, c_int, vp, vp]
+    L.dfm_op_let_iou.argtypes = [vp, vp, c_int, c_int, vp, vp]
     L.dfm_image_prep.argtypes = [POINTER(ImagePrepDesc), vp, vp, vp]
     _lib = L
     return L

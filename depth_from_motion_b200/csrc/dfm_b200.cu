@@ -29,6 +29,7 @@
 #include "image_prep_kernels.cuh"
 #include "view_cache_kernels.cuh"
 #include "kitti_eval_kernels.cuh"
+#include "waymo_eval_kernels.cuh"
 
 namespace {
 
@@ -1578,3 +1579,4 @@ int dfm_depth_head_forward(const float* d_cost, const float* d_depth_samples, in
 #include "image_prep_api.inc"
 #include "view_cache_api.inc"
 #include "kitti_eval_api.inc"
+#include "waymo_eval_api.inc"

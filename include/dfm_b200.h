@@ -741,6 +741,18 @@ int dfm_op_eval_rotated_iou(const float* d_boxes, const float* d_qboxes, int n, 
                             int criterion, float* d_iou, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * Pair stage of Waymo's camera-only LET-3D-AP (compute_detection_let_metrics_main).
+ * d_pred [n][7], d_gt [k][7]: fp64 boxes (center x, y, z, length, width, height, heading)
+ * in the vehicle frame.  d_out [n][k][3] fp64: for prediction i and GT j, the 3-D rotated
+ * IoU of the prediction aligned along the sensor -> prediction ray to the point closest to
+ * the GT centre (LET-IoU), the longitudinal affinity 1 - min(|e_lon| / tol, 1) with
+ * tol = max(0.1 |c_gt - s|, 0.5 m) and s = (1.43, 0, 2.18), and the heading accuracy
+ * 1 - |wrapped heading error| / pi.
+ * ---------------------------------------------------------------------------------- */
+int dfm_op_let_iou(const double* d_pred, const double* d_gt, int n, int k, double* d_out,
+                   void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Image preparation of the shipped test pipelines, one launch per batch of views.
  * d_src: num_views decoded 8-bit BGR images, [num_views][src_h][src_w][3], all one size.
  * d_out: [num_views][3][pad_h][pad_w] fp32, pad_h / pad_w = out_h / out_w rounded up to
