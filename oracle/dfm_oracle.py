@@ -149,10 +149,11 @@ def build_dfm_cost(cur_feats, prev_feats, depths, feat_sample_factor,
     cur_grid[..., 1] = cur_grid[..., 1] / (h_in - 1) * 2 - 1
     prev_grid[..., 0] = prev_grid[..., 0] / (w_in - 1) * 2 - 1
     prev_grid[..., 1] = prev_grid[..., 1] / (h_in - 1) * 2 - 1
-    cur_cost = F.grid_sample(cur_feats, cur_grid, mode='bilinear',
+    # the grid keeps the reference's fp32 geometry; fp64 features sample it exactly widened
+    cur_cost = F.grid_sample(cur_feats, cur_grid.to(cur_feats.dtype), mode='bilinear',
                              padding_mode='zeros', align_corners=True)
     cur_cost = cur_cost.view(batch_size, -1, num_depths, h_out, w_out)
-    prev_cost = F.grid_sample(prev_feats, prev_grid, mode='bilinear',
+    prev_cost = F.grid_sample(prev_feats, prev_grid.to(prev_feats.dtype), mode='bilinear',
                               padding_mode='zeros', align_corners=True)
     prev_cost = prev_cost.view(batch_size, -1, num_depths, h_out, w_out)
     return torch.cat([cur_cost, prev_cost], dim=1)                # :313
@@ -326,8 +327,19 @@ def point_sample(img_features, points, proj_mat, img_scale_factor,
     norm_x = coor_x / w * 2 - 1
     grid = torch.cat([norm_x, norm_y], dim=1).unsqueeze(0).unsqueeze(0)
     mode = 'bilinear' if aligned else 'nearest'
-    feats = F.grid_sample(img_features, grid, mode=mode, padding_mode='zeros',
-                          align_corners=True)
+    if aligned or img_features.dtype == grid.dtype:
+        feats = F.grid_sample(img_features, grid.to(img_features.dtype), mode=mode,
+                              padding_mode='zeros', align_corners=True)
+    else:
+        # wider features (fp64 reference runs): the tap is the one grid_sample picks in the
+        # geometry's precision, found by sampling a map of 1-based pixel indices, and its value
+        # is gathered exactly
+        hf, wf = img_features.shape[-2:]
+        tags = torch.arange(1, hf * wf + 1, dtype=grid.dtype, device=grid.device)
+        tap = F.grid_sample(tags.view(1, 1, hf, wf), grid, mode='nearest',
+                            padding_mode='zeros', align_corners=True).view(-1).long()
+        flat = img_features.reshape(img_features.shape[1], hf * wf)
+        feats = (flat[:, (tap - 1).clamp(min=0)] * (tap > 0))[None, :, None]
     if valid_flag:
         valid = (coor_x.squeeze() < w) & (coor_x.squeeze() > 0) & \
             (coor_y.squeeze() < h) & (coor_y.squeeze() > 0) & (depths > 0)
@@ -532,9 +544,10 @@ def frustum_to_voxel_forward(p, stereo_feat, stereo_feat_softmax, img_metas,
         norms.append(n)
         v2ds.append(v2)
         vs.append(v)
-    norm = torch.stack(norms)
-    valid2d = torch.stack(v2ds)
-    valid = torch.stack(vs)
+    # the fp32 geometry is built on the CPU; widened exactly for fp64 features
+    norm = torch.stack(norms).to(stereo_feat)
+    valid2d = torch.stack(v2ds).to(stereo_feat.device)
+    valid = torch.stack(vs).to(stereo_feat.device)
     voxel = F.grid_sample(stereo_feat, norm, align_corners=True)
     voxel = voxel * valid[:, None]
     pred_disp = None
