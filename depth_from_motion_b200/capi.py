@@ -60,7 +60,8 @@ SYMBOLS = (
     'dfm_views_equal', 'dfm_fpn_set_num_images', 'dfm_liga_resnet_set_num_images',
     'dfm_resnet101_set_num_images', 'dfm_kitti_eval_create', 'dfm_kitti_eval_destroy',
     'dfm_kitti_eval_forward', 'dfm_kitti_eval_debug_tensor', 'dfm_op_eval_rotated_iou',
-    'dfm_op_let_iou',
+    'dfm_op_let_iou', 'dfm_kitti_eval_set_overlap_limit', 'dfm_kitti_eval_workspace',
+    'dfm_waymo_kitti_convert',
 )
 
 DFM_IMAGE_PREP_CROP, DFM_IMAGE_PREP_RESCALE = 0, 1
@@ -285,6 +286,11 @@ def lib():
     L.dfm_kitti_eval_debug_tensor.argtypes = [vp, c_char_p, vp, c_longlong, vp]
     L.dfm_op_eval_rotated_iou.argtypes = [vp, vp, c_int, c_int, c_int, vp, vp]
     L.dfm_op_let_iou.argtypes = [vp, vp, c_int, c_int, vp, vp]
+    L.dfm_kitti_eval_set_overlap_limit.argtypes = [vp, c_longlong]
+    L.dfm_kitti_eval_workspace.argtypes = [vp, POINTER(c_longlong), POINTER(c_longlong),
+                                           POINTER(c_int)]
+    L.dfm_waymo_kitti_convert.argtypes = [c_int, c_int] + [vp] * 5 + [POINTER(c_float)] + \
+        [vp] * 4
     L.dfm_image_prep.argtypes = [POINTER(ImagePrepDesc), vp, vp, vp]
     _lib = L
     return L

@@ -2,11 +2,18 @@
 // eval_class) for one set of N frames, ground truth and detections in CSR form:
 //
 //   ignore codes per (class, difficulty, frame)                      (clean_data, eval.py:30-82)
-//   overlaps per (metric, frame, dt, gt), only within a frame          (calculate_iou_partly)
-//   pass 1: TP scores per (config, frame)          (compute_statistics_jit, compute_fp=False)
+//   per part of frames: overlaps per (metric, frame, dt, gt), only within a frame
+//                       (calculate_iou_partly), then pass 1: TP scores per (config, frame)
+//                       (compute_statistics_jit, compute_fp=False)
 //   thresholds per config: bitonic sort of its TP scores + the 41-point pick (get_thresholds)
-//   pass 2: tp / fp / fn / similarity per (config, threshold, frame)   (compute_fp=True)
+//   per part of frames: overlaps again, then pass 2: tp / fp / fn / similarity per (config,
+//                       threshold, frame)   (compute_fp=True)
 //   reduce per (config, threshold): integer counts, similarity summed in frame order
+//
+// A part is a run of whole frames whose overlaps fit the handle's limit.  Every per-frame
+// result (TP scores, counts, similarity term) depends on that frame's overlaps alone, the
+// counts are integers and the similarity is summed in frame order afterwards, so the results
+// are bitwise the same for any division into parts.
 //
 // A config is (metric slot, class slot, difficulty, overlap set), indexed in the order
 // eval_class walks them.  The rotated IoU restates rotate_iou.py op for op, typed as numba
@@ -44,12 +51,16 @@ struct Params {
   const int* gt_off;       // [N + 1]
   const int* dt_off;       // [N + 1]
   const long long* pair_off;  // [N + 1] sum of dt * gt counts of the frames before
-  long long P;
+  long long P;             // pairs of the whole set
+  // the current part: frames [f0, f0 + nf), pairs [q0, q0 + nq) of the set
+  int f0, nf;
+  long long q0, nq;
+  long long OP;            // pairs the overlap buffer holds per metric (the largest part)
   // workspace
   signed char* ign_gt;     // [C * 3][G]
   signed char* ign_dt;     // [C * 3][D]
   int* num_valid;          // [C * 3]
-  double* ov;              // [M][P]  [dt][gt] within each frame
+  double* ov;              // [M][OP] [dt][gt] within each frame of the current part
   double* tp_scores;       // [NC][G] at each frame's gt offset
   int* tp_count;           // [NC][N]
   double* sorted;          // [NC][S] S = pow2 >= G
@@ -317,14 +328,15 @@ __device__ __forceinline__ int frame_of_pair(const long long* off, int N, long l
   return lo;
 }
 
-// calculate_iou_partly(dt_annos, gt_annos, metric): ov[ms][pair] for each (dt, gt) of a frame
+// calculate_iou_partly(dt_annos, gt_annos, metric): ov[ms][pair - q0] for each (dt, gt) of a
+// frame of the current part
 __global__ void ke_overlap_kernel(Params p) {
   const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const int ms = blockIdx.y;
-  if (q >= p.P) return;
-  const int f = frame_of_pair(p.pair_off, p.N, q);
+  if (q >= p.nq) return;
+  const int f = p.f0 + frame_of_pair(p.pair_off + p.f0, p.nf, p.q0 + q);
   const int ng = p.gt_off[f + 1] - p.gt_off[f];
-  const long long local = q - p.pair_off[f];
+  const long long local = p.q0 + q - p.pair_off[f];
   const int j = p.dt_off[f] + (int)(local / ng), i = p.gt_off[f] + (int)(local % ng);
   const double* g = p.gt + (size_t)i * GT_W;
   const double* d = p.dt + (size_t)j * DT_W;
@@ -350,7 +362,7 @@ __global__ void ke_overlap_kernel(Params p) {
                    : d3_overlap<double, double>(d + 5, g + 5, rinc));
     }
   }
-  p.ov[(size_t)ms * p.P + q] = v;
+  p.ov[(size_t)ms * p.OP + q] = v;
 }
 
 __device__ __forceinline__ void config_parts(const Params& p, int cfg, int& ms, int& cd, int& k) {
@@ -382,7 +394,7 @@ __device__ Stats frame_statistics(const Params& p, int cfg, int f, bool compute_
   }
   const signed char* ig = p.ign_gt + (size_t)cd * p.G + g0;
   const signed char* id = p.ign_dt + (size_t)cd * p.D + d0;
-  const double* ov = p.ov + (size_t)ms * p.P + p.pair_off[f];
+  const double* ov = p.ov + (size_t)ms * p.OP + (p.pair_off[f] - p.q0);
   unsigned assigned[MAX_DT_FRAME / 32];
   unsigned below[MAX_DT_FRAME / 32];
   for (int w = 0; w < (nd + 31) / 32; ++w) {
@@ -472,10 +484,11 @@ __device__ Stats frame_statistics(const Params& p, int cfg, int f, bool compute_
   return s;
 }
 
-// pass 1: grid (frames, configs)
+// pass 1: grid (frames of the part, configs)
 __global__ void ke_pass1_kernel(Params p) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x, cfg = blockIdx.y;
-  if (f >= p.N) return;
+  const int fl = blockIdx.x * blockDim.x + threadIdx.x, cfg = blockIdx.y;
+  if (fl >= p.nf) return;
+  const int f = p.f0 + fl;
   const Stats s = frame_statistics(p, cfg, f, false, 0.0,
                                    p.tp_scores + (size_t)cfg * p.G + p.gt_off[f]);
   p.tp_count[(size_t)cfg * p.N + f] = s.tp;
@@ -543,10 +556,11 @@ __global__ void __launch_bounds__(1024) ke_thresholds_kernel(Params p) {
   p.thr_count[cfg] = min(count, MAX_T + 1);
 }
 
-// pass 2: grid (frames, thresholds, configs)
+// pass 2: grid (frames of the part, thresholds, configs)
 __global__ void ke_pass2_kernel(Params p) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x, t = blockIdx.y, cfg = blockIdx.z;
-  if (f >= p.N || t >= min(p.thr_count[cfg], MAX_T)) return;
+  const int fl = blockIdx.x * blockDim.x + threadIdx.x, t = blockIdx.y, cfg = blockIdx.z;
+  if (fl >= p.nf || t >= min(p.thr_count[cfg], MAX_T)) return;
+  const int f = p.f0 + fl;
   const Stats s = frame_statistics(p, cfg, f, true, p.thresholds[(size_t)cfg * MAX_T + t],
                                    nullptr);
   unsigned long long* c = p.cnt + ((size_t)cfg * MAX_T + t) * 3;

@@ -143,5 +143,108 @@ __global__ void let_iou_kernel(const double* __restrict__ pd, const double* __re
   for (int c = 0; c < 3; ++c) out[q * 3 + c] = r[c];
 }
 
+
+// ---- WaymoDataset.convert_valid_bboxes + bbox2result_kitti, load_mode 'lidar_frame' ----
+// One thread per LiDAR box of the set (CSR: box_off[F + 1]).  float32 throughout, each
+// product and sum rounded on its own in the order of the reference's torch / numpy calls:
+// limit_yaw(0.5, 2 pi); Box3DMode LIDAR -> CAM with rt = R0_rect @ Tr_velo_to_cam (the
+// caller's float32 product); the camera box's corners projected with P0; the min / max of
+// the projection clipped to image_shape; alpha = -arctan2(-y, x) + ry_cam.  A box is kept iff
+// its centre lies strictly inside the limit range.  The matrix products of the reference run
+// through BLAS, whose summation order is not fixed, so the values agree with it to float32
+// rounding; the keep mask depends on the input centre alone and is exact.
+// out columns: the anno's bbox[4] (clipped) alpha location[3] dimensions[3] rotation_y, then
+// convert_valid_bboxes' LiDAR yaw and its unclipped 2-D box[4]
+constexpr int KC_W = 17;
+
+__device__ __forceinline__ float fmulr(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ float faddr(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ float fsubr(float a, float b) { return __fsub_rn(a, b); }
+
+// limit_period(val, 0.5, 2 pi) of a float32 tensor: the period is rounded to float32
+__device__ __forceinline__ float limit_2pi(float v) {
+  const float period = (float)(2.0 * PI);
+  return fsubr(v, fmulr(floorf(faddr(__fdiv_rn(v, period), 0.5f)), period));
+}
+
+// one row of a [K, 4] @ [4, 4]^T product: sum_j a[j] * m[row][j], j ascending
+__device__ __forceinline__ float row_dot4(const float* m, float a0, float a1, float a2, float a3) {
+  return faddr(faddr(faddr(fmulr(a0, m[0]), fmulr(a1, m[1])), fmulr(a2, m[2])), fmulr(a3, m[3]));
+}
+
+__global__ void kitti_convert_kernel(int F, int K, const float* __restrict__ boxes,
+                                     const int* __restrict__ box_off,
+                                     const float* __restrict__ calib,
+                                     const int* __restrict__ image_shape,
+                                     const long long* __restrict__ image_idx, float lx0, float ly0,
+                                     float lz0, float lx1, float ly1, float lz1,
+                                     unsigned char* __restrict__ keep, float* __restrict__ out,
+                                     long long* __restrict__ sample_idx) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= K) return;
+  int lo = 0, hi = F - 1;   // the last frame with box_off[f] <= k
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (box_off[mid] <= k) lo = mid;
+    else hi = mid - 1;
+  }
+  const int f = lo;
+  const float* b = boxes + (size_t)k * 7;
+  const float* rt = calib + (size_t)f * 32;   // R0_rect @ Tr_velo_to_cam, [4][4]
+  const float* P0 = rt + 16;                  // [4][4]
+  const float x = b[0], y = b[1], z = b[2], dx = b[3], dy = b[4], dz = b[5];
+  const float yaw = limit_2pi(b[6]);
+  keep[k] = (x > lx0 && y > ly0 && z > lz0 && x < lx1 && y < ly1 && z < lz1) ? 1 : 0;
+  sample_idx[k] = image_idx[f];
+  // Box3DMode.convert: xyz @ rt^T, sizes (dx, dz, dy), yaw -> limit_period(-yaw - pi / 2)
+  const float cx = row_dot4(rt, x, y, z, 1.f), cy = row_dot4(rt + 4, x, y, z, 1.f),
+              cz = row_dot4(rt + 8, x, y, z, 1.f);
+  const float ry = limit_2pi(fsubr(-yaw, (float)(PI / 2)));
+  const float dims[3] = {dx, dz, dy};
+  // CameraInstance3DBoxes.corners: dims * (unit corner - (0.5, 1, 0.5)), rotated about y
+  const float rc = cosf(ry), rs = sinf(ry);
+  float u0 = INFINITY, v0 = INFINITY, u1 = -INFINITY, v1 = -INFINITY;
+  bool nan = false;
+#pragma unroll
+  for (int c = 0; c < 8; ++c) {
+    const float n0 = (float)((c >> 2) & 1) - 0.5f, n1 = (float)((c >> 1) & 1) - 1.f,
+                n2 = (float)(c & 1) - 0.5f;
+    const float c0 = fmulr(dims[0], n0), c1 = fmulr(dims[1], n1), c2 = fmulr(dims[2], n2);
+    const float px = faddr(faddr(fmulr(c0, rc), fmulr(c2, rs)), cx);
+    const float py = faddr(c1, cy);
+    const float pz = faddr(faddr(fmulr(c0, -rs), fmulr(c2, rc)), cz);
+    // points_cam2img: (p, 1) @ P0^T, then the first two over the third
+    const float w = row_dot4(P0 + 8, px, py, pz, 1.f);
+    const float u = __fdiv_rn(row_dot4(P0, px, py, pz, 1.f), w);
+    const float v = __fdiv_rn(row_dot4(P0 + 4, px, py, pz, 1.f), w);
+    nan |= u != u || v != v;   // torch.min / max propagate NaN
+    u0 = fminf(u0, u);
+    v0 = fminf(v0, v);
+    u1 = fmaxf(u1, u);
+    v1 = fmaxf(v1, v);
+  }
+  if (nan) u0 = v0 = u1 = v1 = NAN;
+  // bbox2result_kitti: bbox[2:] = min(bbox[2:], (W, H)), bbox[:2] = max(bbox[:2], 0)
+  const float H = (float)image_shape[2 * f], W = (float)image_shape[2 * f + 1];
+  float* o = out + (size_t)k * KC_W;
+  o[0] = u0 < 0.f ? 0.f : u0;
+  o[1] = v0 < 0.f ? 0.f : v0;
+  o[2] = u1 > W ? W : u1;
+  o[3] = v1 > H ? H : v1;
+  o[4] = faddr(-atan2f(-y, x), ry);
+  o[5] = cx;
+  o[6] = cy;
+  o[7] = cz;
+  o[8] = dims[0];
+  o[9] = dims[1];
+  o[10] = dims[2];
+  o[11] = ry;
+  o[12] = yaw;
+  o[13] = u0;
+  o[14] = v0;
+  o[15] = u1;
+  o[16] = v1;
+}
+
 }  // namespace we
 }  // namespace dfm

@@ -88,6 +88,133 @@ def compute_aos_flag(gt_annos, dt_annos):
     return pred_alpha and valid_alpha_gt
 
 
+def compute_aos_flag_columns(gt, dt):
+    """``compute_aos_flag`` of sets in column form (see ``pack_columns``)."""
+    pred_alpha = bool(np.any(np.asarray(dt['alpha']) != -10))
+    off = np.asarray(gt['off'], np.int64)
+    ng = np.diff(off)
+    alpha = np.asarray(gt['alpha'])
+    first = np.full(len(ng), -10.0)
+    first[ng > 0] = alpha[off[:-1][ng > 0]]
+    stop = (ng == 0) | (first != -10)   # the reference's loop ends at the first of these
+    if not stop.any():
+        return False
+    if ng[int(np.argmax(stop))] == 0:
+        raise ValueError('a GT frame without boxes comes before the first frame with boxes: '
+                         'the reference reads its alpha[0] and fails')
+    return pred_alpha
+
+
+def name_codes(names, gt):
+    """Device class codes of an array of names: clean_data's lower-cased comparisons, one
+    vectorised comparison per class name."""
+    names = np.asarray(names)
+    codes = np.full(len(names), CODE_OTHER, np.int32)
+    if len(names) == 0:
+        return codes
+    names = names.astype(str)
+    done = np.zeros(len(names), bool)
+    for n, c in CODE_OF_NAME.items():   # the spellings KITTI and Waymo annos use
+        m = names == CLASS_TO_NAME[c]
+        codes[m] = c
+        done |= m
+    rest = np.flatnonzero(~done)        # any other spelling: lower-cased, once per name
+    if len(rest):
+        uniq, inv = np.unique(names[rest], return_inverse=True)
+        codes[rest] = np.array([CODE_OF_NAME.get(n.lower(), CODE_OTHER) for n in uniq],
+                               np.int32)[inv.reshape(-1)]
+    if gt:
+        codes[names == 'DontCare'] |= CODE_DONTCARE
+    return codes
+
+
+GT_COLS = ('bbox', 'alpha', 'location', 'dimensions', 'rotation_y', 'occluded', 'truncated')
+DT_COLS = ('bbox', 'alpha', 'location', 'dimensions', 'rotation_y', 'score')
+_WIDTH = {'bbox': 4, 'location': 3, 'dimensions': 3}
+
+
+def _columns(c, cols, what, values=True):
+    off = np.asarray(c['off'], np.int64)
+    if off.ndim != 1 or len(off) < 2 or off[0] != 0 or np.any(np.diff(off) < 0):
+        raise ValueError(f'{what}: off must be ascending from 0 with one entry per frame + 1')
+    n = int(off[-1])
+    if n >= 1 << 31:
+        raise ValueError(f'{what}: {n} boxes, more than the int32 offsets index')
+    if not values:   # the caller has the rows: check the class column only
+        cols = ()
+    # one fp64 row per box, each column written into place once
+    flat = np.empty((n, sum(_WIDTH.get(k, 1) for k in cols)), np.float64)
+    j = 0
+    for k in (('code',) if 'code' in c else ('name',)) + cols:
+        if k not in c:
+            raise ValueError(f'{what} lacks {k!r}')
+        v = np.asarray(c[k])
+        w = _WIDTH.get(k)
+        if (v.shape != (n, w)) if w else (v.shape != (n,)):
+            raise ValueError(f'{what}[{k!r}] has shape {v.shape} for {n} boxes')
+        if k not in ('name', 'code'):
+            flat[:, j:j + (w or 1)] = v.reshape(n, w or 1)
+            j += w or 1
+    return off, flat
+
+
+def column_f32_flags(gt, dt):
+    """``pack``'s dtype flags of sets in column form: a group is float32 when all its
+    columns are."""
+    f32 = lambda c, keys: all(np.asarray(c[k]).dtype == np.float32 for k in keys)
+    return (f32(gt, ('bbox',)) * 1 | f32(dt, ('bbox',)) * 2 |
+            f32(gt, ('location', 'dimensions', 'rotation_y')) * 4 |
+            f32(dt, ('location', 'dimensions', 'rotation_y')) * 8 |
+            f32(gt, ('bbox', 'alpha')) * 16 | f32(dt, ('bbox', 'alpha', 'score')) * 32)
+
+
+def pack_columns(gt, dt, f32_flags=None, dt_rows=None):
+    """Flat fp64 inputs of the device evaluator from sets in column form: ``gt`` / ``dt`` are
+    dicts of the anno keys concatenated over frames (``name``, ``bbox`` [n, 4], ...) plus
+    ``off`` [frames + 1], each frame's first box.  An int32 ``code`` column (``name_codes``
+    of the names) may stand in for ``name``.  ``f32_flags`` (see ``pack``) defaults to the
+    columns' own dtypes: a column group is float32 when all its columns are.  ``dt_rows``, an
+    fp64 [detections, 13] array or CUDA tensor in the device layout (bbox, alpha, location,
+    dimensions, rotation_y, score), stands in for dt's value columns (``dt`` then needs only
+    ``off``, ``name`` or ``code``, and the flags)."""
+    g_off, g = _columns(gt, GT_COLS, 'gt')
+    d_off, d = _columns(dt, DT_COLS, 'dt', values=dt_rows is None)
+    if dt_rows is not None:
+        if f32_flags is None:
+            raise ValueError('dt_rows needs f32_flags')
+        if tuple(dt_rows.shape) != (int(d_off[-1]), 13):
+            raise ValueError(f'dt_rows has shape {tuple(dt_rows.shape)} for {int(d_off[-1])} '
+                             'detections')
+        d = dt_rows
+    if len(g_off) != len(d_off):
+        raise ValueError(f'{len(g_off) - 1} GT frames but {len(d_off) - 1} detection frames')
+    nd = np.diff(d_off)
+    if nd.size and nd.max() > MAX_DT_PER_FRAME:
+        f = int(np.argmax(nd))
+        raise ValueError(f'dt frame {f} holds {int(nd[f])} detections, more than '
+                         f'{MAX_DT_PER_FRAME}')
+    if f32_flags is None:
+        f32_flags = column_f32_flags(gt, dt)
+    ng = np.diff(g_off)
+    code = lambda c, is_gt: (np.asarray(c['code'], np.int32) if 'code' in c else
+                             name_codes(c['name'], is_gt))
+    return dict(gt=g, dt=d, gt_code=code(gt, True), dt_code=code(dt, False),
+                gt_off=g_off.astype(np.int32),
+                dt_off=d_off.astype(np.int32),
+                pair_off=np.concatenate([[0], np.cumsum(ng * nd)]).astype(np.int64),
+                f32_flags=int(f32_flags))
+
+
+def concat_annos(annos, keys):
+    """Per-frame anno dicts -> one dict of concatenated columns plus ``off``."""
+    out = {'off': np.concatenate([[0], np.cumsum([len(a['name']) for a in annos])])}
+    for k in keys:
+        w = _WIDTH.get(k)
+        out[k] = np.concatenate([np.asarray(a[k]).reshape(-1, w) if w else
+                                 np.asarray(a[k]).reshape(-1) for a in annos])
+    return out
+
+
 def pack(gt_annos, dt_annos):
     """Flat fp64 inputs of the device evaluator plus the dtype flags."""
     if len(gt_annos) != len(dt_annos):
@@ -100,42 +227,22 @@ def pack(gt_annos, dt_annos):
         if len(a['name']) > MAX_DT_PER_FRAME:
             raise ValueError(f'dt_annos[{f}] holds {len(a["name"])} detections, more than '
                              f'{MAX_DT_PER_FRAME}')
-
-    def flat(annos, cols):
-        width = {'bbox': 4, 'location': 3, 'dimensions': 3}
-        rows = [np.concatenate([np.asarray(a[k], np.float64).reshape(len(a['name']),
-                                                                     width.get(k, 1))
-                                for k in cols], 1) for a in annos]
-        return np.ascontiguousarray(np.concatenate(rows, 0))
-
-    gt = flat(gt_annos, ('bbox', 'alpha', 'location', 'dimensions', 'rotation_y', 'occluded',
-                         'truncated'))
-    dt = flat(dt_annos, ('bbox', 'alpha', 'location', 'dimensions', 'rotation_y', 'score'))
-    gt_code = np.array([CODE_OF_NAME.get(str(n).lower(), CODE_OTHER) |
-                        (CODE_DONTCARE if str(n) == 'DontCare' else 0)
-                        for a in gt_annos for n in a['name']], np.int32)
-    dt_code = np.array([CODE_OF_NAME.get(str(n).lower(), CODE_OTHER)
-                        for a in dt_annos for n in a['name']], np.int32)
-    ng = np.array([len(a['name']) for a in gt_annos], np.int64)
-    nd = np.array([len(a['name']) for a in dt_annos], np.int64)
     flags = (_is_f32(gt_annos, ('bbox',)) * 1 | _is_f32(dt_annos, ('bbox',)) * 2 |
              _is_f32(gt_annos, ('location', 'dimensions', 'rotation_y')) * 4 |
              _is_f32(dt_annos, ('location', 'dimensions', 'rotation_y')) * 8 |
              _is_f32(gt_annos, ('bbox', 'alpha')) * 16 |
              _is_f32(dt_annos, ('bbox', 'alpha', 'score')) * 32)
-    return dict(gt=gt, dt=dt, gt_code=gt_code, dt_code=dt_code,
-                gt_off=np.concatenate([[0], np.cumsum(ng)]).astype(np.int32),
-                dt_off=np.concatenate([[0], np.cumsum(nd)]).astype(np.int32),
-                pair_off=np.concatenate([[0], np.cumsum(ng * nd)]).astype(np.int64),
-                f32_flags=int(flags))
+    return pack_columns(concat_annos(gt_annos, ('name',) + GT_COLS),
+                        concat_annos(dt_annos, ('name',) + DT_COLS), flags)
 
 
 class KittiEvaluator:
     """Owns one ``dfm_kitti_eval`` handle for a (classes, metrics, aos) setting."""
 
-    def __init__(self, classes, metrics, compute_aos):
+    def __init__(self, classes, metrics, compute_aos, overlap_limit=None):
         self.classes, self.metrics = list(classes), list(metrics)
         self.compute_aos = bool(compute_aos)
+        self.overlap_limit = overlap_limit   # bytes of one part's overlaps; None: the default
         self.f32_flags = None
         self._h = None
 
@@ -160,7 +267,18 @@ class KittiEvaluator:
         capi.check(capi.lib().dfm_kitti_eval_create(ctypes.byref(d), ctypes.byref(h)),
                    'dfm_kitti_eval_create')
         self._h, self.f32_flags = h, f32_flags
+        if self.overlap_limit is not None:
+            capi.check(capi.lib().dfm_kitti_eval_set_overlap_limit(h, int(self.overlap_limit)),
+                       'dfm_kitti_eval_set_overlap_limit')
         return h
+
+    def workspace(self):
+        """The last forward's (workspace bytes, overlap buffer bytes, number of parts)."""
+        w, o, n = ctypes.c_longlong(), ctypes.c_longlong(), ctypes.c_int()
+        capi.check(capi.lib().dfm_kitti_eval_workspace(self._h, ctypes.byref(w), ctypes.byref(o),
+                                                       ctypes.byref(n)),
+                   'dfm_kitti_eval_workspace')
+        return w.value, o.value, n.value
 
     @property
     def num_configs(self):
@@ -171,8 +289,8 @@ class KittiEvaluator:
         import torch
         h = self._handle(packed['f32_flags'])
         dev = torch.device('cuda')
-        t = {k: torch.from_numpy(v).to(dev) for k, v in packed.items()
-             if isinstance(v, np.ndarray)}
+        t = {k: (v if isinstance(v, torch.Tensor) else torch.from_numpy(v)).to(dev)
+             for k, v in packed.items() if isinstance(v, (np.ndarray, torch.Tensor))}
         nc = self.num_configs
         pr = torch.empty(nc, N_SAMPLE_PTS, 4, dtype=torch.float64, device=dev)
         cnt = torch.empty(nc, dtype=torch.int32, device=dev)
@@ -330,10 +448,33 @@ def kitti_eval(gt_annos, dt_annos, current_classes, eval_types=('bbox', 'bev', '
     classes = class_ids(current_classes)
     packed = pack(gt_annos, dt_annos)
     compute_aos = compute_aos_flag(gt_annos, dt_annos)
+    return _evaluate_packed(packed, classes, eval_types, compute_aos, return_intermediates)
+
+
+def kitti_eval_columns(gt, dt, current_classes, eval_types=('bbox', 'bev', '3d'),
+                       return_intermediates=False, f32_flags=None, overlap_limit=None,
+                       dt_rows=None):
+    """``kitti_eval`` of sets in column form (see ``pack_columns``): the same results as
+    ``kitti_eval`` of the per-frame annos, without a Python loop over frames or boxes.
+    ``overlap_limit`` bounds the bytes of one part's overlaps (see ``KittiEvaluator``);
+    ``dt_rows`` see ``pack_columns``."""
+    eval_types = check_eval_types(eval_types)
+    classes = class_ids(current_classes)
+    packed = pack_columns(gt, dt, f32_flags, dt_rows)
+    compute_aos = compute_aos_flag_columns(gt, dt)
+    if compute_aos and 'bbox' not in eval_types:
+        raise ValueError('the alphas are valid, so kitti_eval computes AOS, which needs the bbox '
+                         'metric: the reference fails on these eval_types')
+    return _evaluate_packed(packed, classes, eval_types, compute_aos, return_intermediates,
+                            overlap_limit)
+
+
+def _evaluate_packed(packed, classes, eval_types, compute_aos, return_intermediates,
+                     overlap_limit=None):
     if compute_aos and 'aos' not in eval_types:
         eval_types.append('aos')
     metrics = [m for m, n in enumerate(METRICS) if n in eval_types]
-    ev = KittiEvaluator(classes, metrics, 'aos' in eval_types)
+    ev = KittiEvaluator(classes, metrics, 'aos' in eval_types, overlap_limit)
     try:
         pr, cnt = ev.forward(packed)
     finally:

@@ -716,6 +716,16 @@ typedef struct dfm_kitti_eval_desc {
 } dfm_kitti_eval_desc_t;
 int dfm_kitti_eval_create(const dfm_kitti_eval_desc_t* desc, dfm_kitti_eval_t** out);
 int dfm_kitti_eval_destroy(dfm_kitti_eval_t* h);
+/* The forward evaluates the frames in parts: runs of whole frames whose overlaps (num_metrics
+ * fp64 per (detection, GT) pair) fit `bytes` (default 4 GiB).  The rest of the workspace is
+ * O(frames + GT + detections).  The results are bitwise the same for every limit; a frame
+ * whose own overlaps exceed the limit is refused with DFM_ERR_INVALID.  With more than one
+ * part the forward reads pair_off back to the host and synchronises the stream. */
+int dfm_kitti_eval_set_overlap_limit(dfm_kitti_eval_t* h, long long bytes);
+/* The last forward's workspace in bytes, its overlap buffer in bytes, and its part count;
+ * DFM_ERR_STATE before a forward. */
+int dfm_kitti_eval_workspace(const dfm_kitti_eval_t* h, long long* workspace_bytes,
+                             long long* overlap_bytes, int* num_parts);
 /* d_pr: device [configs][41][4] fp64 (tp, fp, fn, similarity per threshold; zero past the
  * count); d_thr_count: device [configs] int32, 42 when a config has more thresholds than the
  * reference's 41-point arrays hold; d_status: device int32, 0 on success, bit 0 set when a
@@ -727,7 +737,8 @@ int dfm_kitti_eval_forward(dfm_kitti_eval_t* h, int num_frames, int num_gt, int 
                            const int* d_gt_off, const double* d_dt, const int* d_dt_code,
                            const int* d_dt_off, const long long* d_pair_off, double* d_pr,
                            int* d_thr_count, int* d_status, void* stream);
-/* Test hook, from the last forward: "overlap<metric>" fp64 [num_pairs] ([dt][gt] per frame),
+/* Test hook, from the last forward: "overlap<metric>" fp64 [pairs of the last part] ([dt][gt]
+ * per frame; all num_pairs when the set fit in one part),
  * "tp_scores" fp64 [configs][S] (each config's TP scores sorted descending, S = the power of
  * two >= num_gt), "tp_count" int32 [configs], "thresholds" fp64 [configs][41],
  * "num_valid_gt" int32 [num_classes * 3].  DFM_ERR_STATE before a forward, DFM_ERR_INVALID on
@@ -751,6 +762,23 @@ int dfm_op_eval_rotated_iou(const float* d_boxes, const float* d_qboxes, int n, 
  * ---------------------------------------------------------------------------------- */
 int dfm_op_let_iou(const double* d_pred, const double* d_gt, int n, int k, double* d_out,
                    void* stream);
+
+/* ------------------------------------------------------------------------------------
+ * WaymoDataset.convert_valid_bboxes + bbox2result_kitti (mmdet3d datasets/waymo_dataset.py)
+ * for load_mode 'lidar_frame', for a whole set in one launch.  d_boxes [num_boxes][7] fp32
+ * LiDAR boxes (x, y, z, dx, dy, dz, yaw; bottom centre), d_box_off [num_frames + 1] int32;
+ * per frame d_calib [num_frames][32] fp32 (R0_rect @ Tr_velo_to_cam as float32 [4][4], then
+ * P0 [4][4]), d_image_shape [num_frames][2] int32 (H, W), d_image_idx [num_frames] int64;
+ * limit_range: host float[6] (x0, y0, z0, x1, y1, z1).  Writes per box d_keep (1 iff the
+ * centre lies strictly inside limit_range), d_sample_idx (its frame's image_idx) and d_out
+ * [num_boxes][17] fp32: the 2-D box from the P0 projection of the camera box's corners,
+ * clipped to the image (x0, y0, x1, y1), alpha, camera location[3], dimensions[3] (l, h, w),
+ * rotation_y, the LiDAR yaw after limit_yaw(0.5, 2 pi), and the 2-D box before clipping. */
+int dfm_waymo_kitti_convert(int num_frames, int num_boxes, const float* d_boxes,
+                            const int* d_box_off, const float* d_calib, const int* d_image_shape,
+                            const long long* d_image_idx, const float* limit_range,
+                            unsigned char* d_keep, float* d_out, long long* d_sample_idx,
+                            void* stream);
 
 /* ------------------------------------------------------------------------------------
  * Image preparation of the shipped test pipelines, one launch per batch of views.
