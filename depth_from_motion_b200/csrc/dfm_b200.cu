@@ -8,6 +8,7 @@
 #include <atomic>
 #include <cmath>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <memory>
 #include <set>
@@ -137,12 +138,39 @@ int require_sm90() {
   return DFM_OK;
 }
 
+// The state_dict of a parameterised handle: its create registers every key once, with the
+// key's element count and what to do with the host data, and its set_param is set().
+struct ParamTable {
+  // key -> (element count, what to do with the host data)
+  std::map<std::string, std::pair<long long, std::function<int(const float*)>>> entries;
+  std::set<std::string> missing;  // sorted: forward_prologue names the first
+  void add(std::string key, long long numel, std::function<int(const float*)> set) {
+    missing.insert(key);
+    entries[std::move(key)] = {numel, std::move(set)};
+  }
+  // a setter's error is returned as it is and leaves the key missing
+  int set(const char* family, const char* key, const float* h, long long numel) {
+    if (!key || !h) return fail(DFM_ERR_INVALID, "null argument");
+    const auto it = entries.find(key);
+    if (it == entries.end())
+      return fail(DFM_ERR_INVALID, std::string("unknown ") + family + " parameter: " + key);
+    if (numel != it->second.first)
+      return fail(DFM_ERR_INVALID, it->first + ": wrong element count (expected " +
+                                       std::to_string(it->second.first) + ", got " +
+                                       std::to_string(numel) + ")");
+    DFM_TRY(it->second.second(h));
+    missing.erase(it->first);
+    return DFM_OK;
+  }
+};
+
 // every handle's forward: refuse to run after a tensor-core kernel timed out, or with
 // parameters missing (the message names the first missing key in sorted order)
-int forward_prologue(const std::set<std::string>& missing) {
+int forward_prologue(const ParamTable& params) {
   if (dfm::tc_consume_error())
     return fail(DFM_ERR_CUDA, "an earlier tensor-core conv kernel timed out on an mbarrier "
                               "hand-over: its outputs were invalid");
+  const std::set<std::string>& missing = params.missing;
   if (!missing.empty())
     return fail(DFM_ERR_STATE, "missing parameter: " + *missing.begin() + " (+" +
                                    std::to_string(missing.size() - 1) + " more)");
@@ -184,6 +212,45 @@ struct Norm {  // GroupNorm (statistics computed per frame) or folded BatchNorm 
     return DFM_OK;
   }
 };
+
+// eval-mode BatchNorm (weight, bias, running_mean, running_var) folded on the host into the
+// static scale / shift of `n`, once all four fields have arrived
+struct FoldedBn {
+  Norm n;
+  std::vector<float> v[4];
+  bool have[4] = {false, false, false, false};
+  int set(int field, const float* h) {
+    v[field].assign(h, h + n.C);
+    have[field] = true;
+    if (!(have[0] && have[1] && have[2] && have[3])) return DFM_OK;
+    const int C = n.C;
+    std::vector<float> sc(C), sh(C);
+    for (int c = 0; c < C; ++c) {
+      const double s = (double)v[0][c] / std::sqrt((double)v[3][c] + 1e-5);
+      sc[c] = (float)s;
+      sh[c] = (float)((double)v[1][c] - (double)v[2][c] * s);
+    }
+    CU_TRY(cudaMemcpy(n.scale.p, sc.data(), C * 4, cudaMemcpyHostToDevice));
+    CU_TRY(cudaMemcpy(n.shift.p, sh.data(), C * 4, cudaMemcpyHostToDevice));
+    return DFM_OK;
+  }
+};
+
+// registration of <prefix>.weight / .bias of a GroupNorm and of the four fields of a BatchNorm;
+// both need the norm's channel count (Norm::init) first
+void add_norm(ParamTable& t, const std::string& prefix, Norm& n) {
+  for (DevBuf* dst : {&n.gamma, &n.beta})
+    t.add(prefix + (dst == &n.gamma ? ".weight" : ".bias"), n.C, [dst, &n](const float* h) {
+      CU_TRY(cudaMemcpy(dst->p, h, n.C * sizeof(float), cudaMemcpyHostToDevice));
+      return DFM_OK;
+    });
+}
+
+void add_bn(ParamTable& t, const std::string& prefix, FoldedBn& bn) {
+  const char* const field[4] = {".weight", ".bias", ".running_mean", ".running_var"};
+  for (int f = 0; f < 4; ++f)
+    t.add(prefix + field[f], bn.n.C, [&bn, f](const float* h) { return bn.set(f, h); });
+}
 
 struct ConvW {
   int Cin = 0, Cout = 0, transposed = 0;
@@ -621,7 +688,7 @@ struct dfm_backbone {
   DevBuf out_st, out_mo, pipe_sem, pipe_vox, pipe_preds, pipe_samples;
   std::vector<float> pipe_samples_host;  // what pipe_samples holds (re-uploaded on change only)
   bool depths_set = false;
-  std::set<std::string> missing;
+  ParamTable params;
   struct DebugTensor {
     const DevBuf* buf;
     const bool* written;  // null: every forward writes it
@@ -674,50 +741,20 @@ int tower_alloc(Tower& t, int D, int Ho, int Wo, int cv) {
   return DFM_OK;
 }
 
-std::vector<std::string> tower_param_names(bool mono) {
-  const std::string sfx = mono ? "_mono" : "";
-  const std::string hg = mono ? "hg_mono.0" : "hg_stereo.0";
-  const std::string pr = mono ? "pred_mono.0" : "pred_stereo.0";
-  std::vector<std::string> v;
-  for (const char* m : {"dres0", "dres1"}) {
-    v.push_back(std::string(m) + sfx + ".conv.weight");
-    v.push_back(std::string(m) + sfx + ".gn.weight");
-    v.push_back(std::string(m) + sfx + ".gn.bias");
-  }
-  for (const char* c : {"conv1.0", "conv2", "conv3.0", "conv4.0", "conv5", "conv6"}) {
-    v.push_back(hg + "." + c + ".0.weight");
-    v.push_back(hg + "." + c + ".1.weight");
-    v.push_back(hg + "." + c + ".1.bias");
-  }
-  v.push_back(pr + ".0.conv.weight");
-  v.push_back(pr + ".0.gn.weight");
-  v.push_back(pr + ".0.gn.bias");
-  v.push_back(pr + ".1.weight");
-  return v;
-}
-
 bool ends_with(const std::string& s, const std::string& e) {
   return s.size() >= e.size() && s.compare(s.size() - e.size(), e.size(), e) == 0;
 }
 
-int set_norm_param(Norm& n, const std::string& name, const float* h, long long numel) {
-  if (numel != n.C) return fail(DFM_ERR_INVALID, name + ": wrong element count");
-  DevBuf& dst = ends_with(name, ".weight") ? n.gamma : n.beta;
-  CU_TRY(cudaMemcpy(dst.p, h, numel * sizeof(float), cudaMemcpyHostToDevice));
-  return DFM_OK;
-}
-
-int tower_set_param(Tower& t, bool mono, int cin0, int cv, const std::string& name,
-                    const float* h, long long numel, bool* handled) {
+// one tower's keys: dres0 / dres1, the hourglass and the pred convs (cin0: dres0's input
+// channels).  The norms are initialised (tower_alloc).
+void tower_add_params(ParamTable& p, Tower& t, bool mono, int cin0, int cv) {
   const std::string sfx = mono ? "_mono" : "";
   const std::string hg = mono ? "hg_mono.0" : "hg_stereo.0";
   const std::string pr = mono ? "pred_mono.0" : "pred_stereo.0";
-  *handled = true;
-  if (name == "dres0" + sfx + ".conv.weight") {
+  const long long n0 = 27LL * cin0 * cv, n1 = 27LL * cv * cv;
+  p.add("dres0" + sfx + ".conv.weight", n0, [&t, mono, cin0, cv, n0](const float* h) {
     if (!mono) {  // (cv, 2C, 27): channel halves as two C -> cv convs
       const int C = cin0 / 2;
-      if (numel != (long long)27 * cin0 * cv)
-        return fail(DFM_ERR_INVALID, name + ": wrong element count");
       std::vector<float> hc((size_t)cv * C * 27), hp((size_t)cv * C * 27);
       for (int co = 0; co < cv; ++co)
         for (int ci = 0; ci < C; ++ci)
@@ -728,14 +765,12 @@ int tower_set_param(Tower& t, bool mono, int cin0, int cv, const std::string& na
       DFM_TRY(set_conv(t.d0cur, hc.data(), (long long)hc.size(), C, cv, 0, dfm::TC_S1));
       DFM_TRY(set_conv(t.d0prev, hp.data(), (long long)hp.size(), C, cv, 0, dfm::TC_S1));
     }
-    return set_conv(t.dres0, h, numel, cin0, cv, 0, dfm::TC_S1);
-  }
-  if (name == "dres1" + sfx + ".conv.weight")
-    return set_conv(t.dres1, h, numel, cv, cv, 0, dfm::TC_S1);
-  if (name == "dres0" + sfx + ".gn.weight" || name == "dres0" + sfx + ".gn.bias")
-    return set_norm_param(t.g0, name, h, numel);
-  if (name == "dres1" + sfx + ".gn.weight" || name == "dres1" + sfx + ".gn.bias")
-    return set_norm_param(t.g1, name, h, numel);
+    return set_conv(t.dres0, h, n0, cin0, cv, 0, dfm::TC_S1);
+  });
+  p.add("dres1" + sfx + ".conv.weight", n1,
+        [&t, cv, n1](const float* h) { return set_conv(t.dres1, h, n1, cv, cv, 0, dfm::TC_S1); });
+  add_norm(p, "dres0" + sfx + ".gn", t.g0);
+  add_norm(p, "dres1" + sfx + ".gn", t.g1);
   struct HG { const char* key; ConvW* w; Norm* n; int ci, co, tr, mode; };
   // conv1: the stereo tower shares bricks in a CTA cluster; the mono tower keeps the TMA-fed
   // input-channel slices, so the shipped forward keeps running (and the per-layer test of the
@@ -750,16 +785,16 @@ int tower_set_param(Tower& t, bool mono, int cin0, int cv, const std::string& na
                     {"conv6", &t.c6, &t.gc6, 2 * cv, cv, 1, dfm::TC_T}};
   for (const HG& e : hgs) {
     const std::string base = hg + "." + e.key;
-    if (name == base + ".0.weight")
-      return set_conv(*e.w, h, numel, e.ci, e.co, e.tr, e.mode, !mono);
-    if (name == base + ".1.weight" || name == base + ".1.bias")
-      return set_norm_param(*e.n, name, h, numel);
+    const long long n = 27LL * e.ci * e.co;
+    p.add(base + ".0.weight", n, [e, n, mono](const float* h) {
+      return set_conv(*e.w, h, n, e.ci, e.co, e.tr, e.mode, !mono);
+    });
+    add_norm(p, base + ".1", *e.n);
   }
-  if (name == pr + ".0.conv.weight") return set_conv(t.p0, h, numel, cv, cv, 0, dfm::TC_S1);
-  if (name == pr + ".0.gn.weight" || name == pr + ".0.gn.bias")
-    return set_norm_param(t.gp0, name, h, numel);
-  if (name == pr + ".1.weight") {
-    if (numel != 27LL * cv) return fail(DFM_ERR_INVALID, name + ": wrong element count");
+  p.add(pr + ".0.conv.weight", n1,
+        [&t, cv, n1](const float* h) { return set_conv(t.p0, h, n1, cv, cv, 0, dfm::TC_S1); });
+  add_norm(p, pr + ".0.gn", t.gp0);
+  p.add(pr + ".1.weight", 27LL * cv, [&t, cv](const float* h) {
     std::vector<float> p((size_t)27 * cv);  // (1,cv,3,3,3) -> [tap][c]
     for (int c = 0; c < cv; ++c)
       for (int k = 0; k < 27; ++k) p[(size_t)k * cv + c] = h[(size_t)c * 27 + k];
@@ -770,9 +805,7 @@ int tower_set_param(Tower& t, bool mono, int cin0, int cv, const std::string& na
     t.p1w_host = p;
     if (cv == 32 && !t.p1q.build(p.data())) return fail(DFM_ERR_CUDA, "logits weight upload failed");
     return upload(t.p1w, p.data(), p.size());
-  }
-  *handled = false;
-  return DFM_OK;
+  });
 }
 
 // one tower of DfMBackbone.forward: dfm_backbone.py:175-183 / 189-197 + pred convs
@@ -863,7 +896,7 @@ int tower_forward(dfm_backbone* bb, Tower& t, bool mono, const dfm::WarpLoader& 
   const dfm::Term T1 = term(t.raw1, &t.g1, 0);
   // hourglass (conv_modules.py:129-149)
   // stereo conv1 runs as a cluster of two output-channel groups that share every input brick,
-  // mono conv1 and conv3 as input-channel slices (conv_tc.cuh, TcWeights::build; tower_set_param).
+  // mono conv1 and conv3 as input-channel slices (conv_tc.cuh, TcWeights::build; tower_add_params).
   // On the K-slice route conv1 is fed by TMA from a pre-split copy of its input (DFM_NO_TMA=1:
   // register loaders; DFM_S2_KSLICE=1 puts the stereo conv1 there too, for A/B runs)
   static const bool no_tma = getenv("DFM_NO_TMA") != nullptr;
@@ -1063,9 +1096,18 @@ int dfm_backbone_create(const dfm_backbone_desc_t* desc, dfm_backbone_t** out) {
   DFM_TRY(bb->cost.alloc((size_t)D * Ho * Wo));
   DFM_TRY(tower_alloc(bb->st, D, Ho, Wo, desc->cv_channels));
   DFM_TRY(tower_alloc(bb->mo, D, Ho, Wo, desc->cv_channels));
-  for (bool mono : {false, true})
-    for (const std::string& n : tower_param_names(mono)) bb->missing.insert(n);
-  bb->missing.insert("aggregate_cost.weight");
+  tower_add_params(bb->params, bb->st, false, 2 * desc->in_channels, desc->cv_channels);
+  tower_add_params(bb->params, bb->mo, true, desc->in_channels, desc->cv_channels);
+  dfm_backbone* b = bb.get();
+  bb->params.add("aggregate_cost.weight", (long long)D * 2 * D, [b, D](const float* h) {
+    CU_TRY(cudaMemcpy(b->wagg.p, h, (size_t)D * 2 * D * sizeof(float), cudaMemcpyHostToDevice));
+    // transposed, padded copy [2D][gate_row_pitch(D)] for the persistent gate kernel
+    const int pitch = dfm::gate_row_pitch(D);
+    std::vector<float> wt((size_t)2 * D * pitch, 0.f);
+    for (int d = 0; d < D; ++d)
+      for (int j = 0; j < 2 * D; ++j) wt[(size_t)j * pitch + d] = h[(size_t)d * 2 * D + j];
+    return upload(b->waggT, wt.data(), wt.size());
+  });
   for (int m = 0; m < 2; ++m) {
     Tower& t = m ? bb->mo : bb->st;
     const std::string s = m ? "_mono" : "";
@@ -1096,29 +1138,8 @@ int dfm_backbone_destroy(dfm_backbone_t* bb) {
 
 int dfm_backbone_set_param(dfm_backbone_t* bb, const char* name, const float* h_data,
                            long long numel) {
-  if (!bb || !name || !h_data) return fail(DFM_ERR_INVALID, "null argument");
-  const std::string n(name);
-  const int cv = bb->d.cv_channels, ci = bb->d.in_channels;
-  if (n == "aggregate_cost.weight") {
-    if (numel != (long long)bb->D * 2 * bb->D)
-      return fail(DFM_ERR_INVALID, "aggregate_cost.weight: expected (D, 2D, 1, 1)");
-    CU_TRY(cudaMemcpy(bb->wagg.p, h_data, numel * sizeof(float), cudaMemcpyHostToDevice));
-    {  // transposed, padded copy [2D][gate_row_pitch(D)] for the persistent gate kernel
-      const int D = bb->D, pitch = dfm::gate_row_pitch(D);
-      std::vector<float> wt((size_t)2 * D * pitch, 0.f);
-      for (int d = 0; d < D; ++d)
-        for (int j = 0; j < 2 * D; ++j) wt[(size_t)j * pitch + d] = h_data[(size_t)d * 2 * D + j];
-      DFM_TRY(upload(bb->waggT, wt.data(), wt.size()));
-    }
-    bb->missing.erase(n);
-    return DFM_OK;
-  }
-  bool handled = false;
-  DFM_TRY(tower_set_param(bb->st, false, 2 * ci, cv, n, h_data, numel, &handled));
-  if (!handled) DFM_TRY(tower_set_param(bb->mo, true, ci, cv, n, h_data, numel, &handled));
-  if (!handled) return fail(DFM_ERR_INVALID, "unknown DfMBackbone parameter: " + n);
-  bb->missing.erase(n);
-  return DFM_OK;
+  return bb ? bb->params.set("DfMBackbone", name, h_data, numel)
+            : fail(DFM_ERR_INVALID, "null argument");
 }
 
 int dfm_backbone_set_depths(dfm_backbone_t* bb, const float* h_depths, int n) {
@@ -1130,7 +1151,7 @@ int dfm_backbone_set_depths(dfm_backbone_t* bb, const float* h_depths, int n) {
 }
 
 int dfm_backbone_missing_params(const dfm_backbone_t* bb) {
-  return bb ? (int)bb->missing.size() : -1;
+  return bb ? (int)bb->params.missing.size() : -1;
 }
 
 long long dfm_backbone_workspace_bytes(const dfm_backbone_t* bb) {
@@ -1155,7 +1176,7 @@ int backbone_forward_impl(dfm_backbone_t* bb, const float* d_cur, const float* d
                           float* d_mono, void* stream, cudaEvent_t prev_ready,
                           bool channels_last = false) {
   if (!bb || !d_cur || !d_prev || !geom) return fail(DFM_ERR_INVALID, "null argument");
-  DFM_TRY(forward_prologue(bb->missing));
+  DFM_TRY(forward_prologue(bb->params));
   if (!bb->depths_set) return fail(DFM_ERR_STATE, "downsampled_depth not set");
   cudaStream_t st = (cudaStream_t)stream;
   ProfScope ps_all("backbone_forward_total", 0.0, st);

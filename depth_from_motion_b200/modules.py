@@ -160,6 +160,66 @@ class _CudaMirror(nn.Module):
                 'is not implemented')
 
 
+class _HandleMirror(_CudaMirror):
+    """A mirror that owns one handle of include/dfm_b200.h, of the family ``_family``
+    (``dfm_<family>_create`` / ``_destroy`` / ``_set_param`` / ``_debug_tensor``).  Subclasses
+    give the key the handle is built for, the create arguments and the forward."""
+    _family = None
+    _handle = None
+    _key = None
+    _batch = None
+
+    def _ensure(self, key, create_args, batch=None):
+        """``capi.lib()``, with a handle for ``key`` that holds the current parameters.  Another
+        key destroys the handle and creates a new one, ``dfm_<family>_create(*create_args(),
+        &handle)``, with a fresh ``_ParamSync``.  ``batch``, for the families with
+        ``set_num_images``: another batch size alone keeps the handle and its uploads."""
+        L = capi.lib()
+        fn = f'dfm_{self._family}'
+        if self._handle is not None and key == self._key:
+            if batch is not None and batch != self._batch:
+                capi.check(getattr(L, fn + '_set_num_images')(self._handle, batch),
+                           fn + '_set_num_images')
+                self._batch = batch
+        else:
+            self.release()
+            hd = ctypes.c_void_p()
+            capi.check(getattr(L, fn + '_create')(*create_args(), ctypes.byref(hd)),
+                       fn + '_create')
+            self._handle, self._key, self._batch = hd, key, batch
+            self._sync = _ParamSync()
+        set_param = getattr(L, fn + '_set_param')
+        self._sync.sync(self, lambda k, p, n: capi.check(set_param(self._handle, k, p, n),
+                                                         f'{fn}_set_param({k.decode()})'))
+        return L
+
+    def release(self):
+        if self._handle is not None:
+            getattr(capi.lib(), f'dfm_{self._family}_destroy')(self._handle)
+            self._handle = None
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
+
+    def init_weights(self):
+        pass
+
+    def debug_tensor(self, name, shape):
+        """Channels-last copy of the intermediate ``name`` the handle's last forward wrote, through
+        the test hook ``dfm_<family>_debug_tensor`` (shape must hold exactly that tensor; tests
+        only).  The class docstring lists the names."""
+        fn = f'dfm_{self._family}_debug_tensor'
+        if self._handle is None:
+            raise RuntimeError(f'{fn}: no forward has run')
+        out = torch.empty(shape, device='cuda', dtype=torch.float32)
+        capi.check(getattr(capi.lib(), fn)(self._handle, name.encode(), _ptr(out), out.numel(),
+                                           _stream()), f'{fn}({name})')
+        return out
+
+
 class _ConvGN(nn.Module):
     """Parameter layout of mmcv ConvModule(Conv3d, norm=GN): .conv / .gn."""
 
@@ -215,8 +275,11 @@ def geometry_from_meta(img_meta):
 
 
 @BACKBONES.register_module()
-class DfMBackbone(_CudaMirror):
-    """Drop-in for the reference ``DfMBackbone`` (dfm_backbone.py:14-214)."""
+class DfMBackbone(_HandleMirror):
+    """Drop-in for the reference ``DfMBackbone`` (dfm_backbone.py:14-214).  Debug tensors
+    (channels-last), each tower's 'raw0', 'cls3', 'raw1', 'c1' .. 'c6', 'cur', 'p0' and 'logit'
+    ('<name>_mono' for the mono tower)."""
+    _family = 'backbone'
 
     def __init__(self, in_channels, num_hg=1, cost_sample_factor=4,
                  feat_sample_factor=1, cv_channels=32,
@@ -258,13 +321,8 @@ class DfMBackbone(_CudaMirror):
                                 depth_cfg['downsample_factor'])
         self.aggregate_cost = nn.Conv2d(2 * self.num_planes, self.num_planes, 1,
                                         bias=False)
-        self._handle = None
-        self._handle_key = None
         self._sync = _ParamSync()
         self._depth_sig = None
-
-    def init_weights(self):
-        pass
 
     # ------------------------------------------------------------------
     def _default_depths(self):
@@ -278,41 +336,14 @@ class DfMBackbone(_CudaMirror):
             d[i] = (i + 0.5) * ds * interval + cfg['depth_min']
         return d
 
-    def _ensure_handle(self, h, w):
-        L = capi.lib()
-        key = (h, w, self.conv_impl)
-        if self._handle is not None and self._handle_key == key:
-            return L
-        self.release()
-        desc = capi.BackboneDesc(self.in_channels, self.cv_channels, h, w,
-                                 self.num_planes, self.cost_sample_factor,
-                                 int(self.feat_sample_factor),
-                                 _IMPL[self.conv_impl])
-        hd = ctypes.c_void_p()
-        capi.check(L.dfm_backbone_create(ctypes.byref(desc), ctypes.byref(hd)),
-                   'dfm_backbone_create')
-        self._handle, self._handle_key = hd, key
-        self._sync = _ParamSync()
-        self._depth_sig = None
-        return L
-
-    def release(self):
-        if self._handle is not None:
-            capi.lib().dfm_backbone_destroy(self._handle)
-            self._handle = None
-
-    def __del__(self):
-        try:
-            self.release()
-        except Exception:
-            pass
-
     def _prepare(self, h, w):
-        L = self._ensure_handle(h, w)
-        self._sync.sync(
-            self, lambda k, p, n: capi.check(
-                L.dfm_backbone_set_param(self._handle, k, p, n),
-                f'dfm_backbone_set_param({k.decode()})'))
+        def create_args():
+            self._depth_sig = None   # a new handle has no depths
+            return (ctypes.byref(capi.BackboneDesc(
+                self.in_channels, self.cv_channels, h, w, self.num_planes,
+                self.cost_sample_factor, int(self.feat_sample_factor), _IMPL[self.conv_impl])),)
+
+        L = self._ensure((h, w, self.conv_impl), create_args)
         depths = getattr(self, 'downsampled_depth', None)
         if depths is None:
             depths = self._default_depths()
@@ -382,21 +413,6 @@ class DfMBackbone(_CudaMirror):
         self._generation = getattr(self, '_generation', 0) + 1
         stereo._dfm_channels_last = (self, self._generation)
         return cost, stereo, mono
-
-    def debug_tensor(self, name, shape):
-        """Channels-last copy of an intermediate (tests only)."""
-        return _debug_tensor(self._handle, 'dfm_backbone_debug_tensor', name, shape)
-
-
-def _debug_tensor(handle, fn, name, shape):
-    """Channels-last copy of the intermediate `name` the handle's last forward wrote, through
-    the test hook `fn` of include/dfm_b200.h (shape must hold exactly that tensor)."""
-    if handle is None:
-        raise RuntimeError(f'{fn}: no forward has run')
-    out = torch.empty(shape, device='cuda', dtype=torch.float32)
-    capi.check(getattr(capi.lib(), fn)(handle, name.encode(), _ptr(out), out.numel(), _stream()),
-               f'{fn}({name})')
-    return out
 
 
 def build_dfm_cost(cur_feats, prev_feats, depths, feat_sample_factor,
@@ -512,7 +528,11 @@ class DepthHead(_CudaMirror):
         return vol, sm, preds
 
 
-class _NeckBase(_CudaMirror):
+class _NeckBase(_HandleMirror):
+    """Debug tensors: the raw output [Nx, Ny, Zo, C] of conv layer i of a tower, 'mono.<i>' /
+    'stereo.<i>' (OutdoorImVoxelNeck's one tower is 'mono')."""
+    _family = 'neck'
+
     def _make_tower(self, c0, c1, c2, cout):
         def cm(ci, co, **kw):
             m = nn.Module()
@@ -535,20 +555,8 @@ class _NeckBase(_CudaMirror):
         assert not self.training, \
             'the CUDA necks fold BatchNorm3d running statistics: call .eval()'
         n, c, nx, ny, nz = x.shape
-        L = capi.lib()
-        key = (nx, ny, nz, conv_impl)
-        if getattr(self, '_handle', None) is None or self._handle_key != key:
-            self.release()
-            desc = capi.NeckDesc(self._c0, self._cout, num_frames, nx, ny, nz,
-                                 _IMPL[conv_impl])
-            hd = ctypes.c_void_p()
-            capi.check(L.dfm_neck_create(ctypes.byref(desc), ctypes.byref(hd)),
-                       'dfm_neck_create')
-            self._handle, self._handle_key = hd, key
-            self._sync = _ParamSync()
-        self._sync.sync(self, lambda k, p, m: capi.check(
-            L.dfm_neck_set_param(self._handle, k, p, m),
-            f'dfm_neck_set_param({k.decode()})'))
+        L = self._ensure((nx, ny, nz, conv_impl), lambda: (ctypes.byref(capi.NeckDesc(
+            self._c0, self._cout, num_frames, nx, ny, nz, _IMPL[conv_impl])),))
         outs = []
         for i in range(n):
             bev = torch.empty((self._cout, ny, nx), device=x.device)
@@ -562,25 +570,6 @@ class _NeckBase(_CudaMirror):
                            'dfm_neck_forward')
             outs.append(bev)
         return [torch.stack(outs)]
-
-    def debug_tensor(self, name, shape):
-        """Raw output of conv layer i of a tower, [Nx, Ny, Zo, C] ('mono.<i>' / 'stereo.<i>';
-        OutdoorImVoxelNeck's one tower is 'mono'), from the last forward (tests only)."""
-        return _debug_tensor(getattr(self, '_handle', None), 'dfm_neck_debug_tensor', name, shape)
-
-    def release(self):
-        if getattr(self, '_handle', None) is not None:
-            capi.lib().dfm_neck_destroy(self._handle)
-            self._handle = None
-
-    def __del__(self):
-        try:
-            self.release()
-        except Exception:
-            pass
-
-    def init_weights(self):
-        pass
 
 
 @NECKS.register_module()
@@ -600,7 +589,6 @@ class OutdoorImVoxelNeck(_NeckBase):
         assert in_channels[2] == 4 * in_channels[0]
         self.conv_impl = conv_impl
         self.model = self._make_tower(*in_channels, out_channels)
-        self._handle = None
 
     def forward(self, x):
         return self._run(x, 0, self.conv_impl)
@@ -625,7 +613,6 @@ class DfMNeck(_NeckBase):
                                               in_channels[1], in_channels[2],
                                               out_channels)
         self.aggregate_layer = nn.Conv2d(2 * out_channels, 1, 1, bias=False)
-        self._handle = None
 
     def forward(self, x):
         assert x.shape[1] == self.in_channels[0] * self.num_frames
@@ -649,13 +636,15 @@ class CostLogits:
 
 
 @NECKS.register_module()
-class FrustumToVoxel(_CudaMirror):
+class FrustumToVoxel(_HandleMirror):
     """Drop-in for the reference ``FrustumToVoxel``
     (necks/feature_transformation.py:12-173): same constructor arguments and
     ``state_dict`` keys (``voxel_convs.<i>.0.conv.weight`` /
     ``voxel_convs.<i>.0.gn.{weight,bias}``); ``depth_cfg`` and ``coordinates_3d``
     are injected by the detector exactly like the reference
-    (detectors/dfm.py:85-100)."""
+    (detectors/dfm.py:85-100).  Debug tensors: 'vox' ([nz, ny, nx, cv], the gathered conv
+    input) and 'conv<i>' (raw output of voxel_convs[i], [nz, ny, nx, 32])."""
+    _family = 'frustum'
 
     def __init__(self, num_3dconvs=1, cv_channels=32, out_channels=32,
                  in_sem_channels=32, sem_atten_feat=True,
@@ -678,27 +667,6 @@ class FrustumToVoxel(_CudaMirror):
             nn.Sequential(_ConvGN(cin if i == 0 else out_channels,
                                   out_channels, 32))
             for i in range(num_3dconvs)])
-        self._handle = None
-        self._key = None
-
-    def init_weights(self):
-        pass
-
-    def debug_tensor(self, name, shape):
-        """'vox' ([nz, ny, nx, cv], the gathered conv input) or 'conv<i>' (raw output of
-        voxel_convs[i], [nz, ny, nx, 32]) of the last forward (tests only)."""
-        return _debug_tensor(self._handle, 'dfm_frustum_debug_tensor', name, shape)
-
-    def release(self):
-        if getattr(self, '_handle', None) is not None:
-            capi.lib().dfm_frustum_destroy(self._handle)
-            self._handle = None
-
-    def __del__(self):
-        try:
-            self.release()
-        except Exception:
-            pass
 
     @staticmethod
     def _separable_centres(c3d):
@@ -715,28 +683,27 @@ class FrustumToVoxel(_CudaMirror):
             raise RuntimeError('coordinates_3d is not a separable (meshgrid) voxel grid')
         return xs, ys, zs
 
-    def _ensure_handle(self, d, h, w, sh, sw, f):
+    def _prepare(self, d, h, w, sh, sw, f):
+        """The handle for these shapes, with the current parameters (``forward`` and
+        ``HotPathPipeline``)."""
         c3d = self.coordinates_3d
         key = (d, h, w, sh, sw, f, tuple(c3d.shape), c3d.data_ptr(),
                c3d._version, float(self.depth_cfg['depth_min']),
                float(self.depth_cfg['depth_max']))
-        if self._handle is not None and key == self._key:
-            return
-        self.release()
-        xs, ys, zs = self._separable_centres(c3d)
-        nz, ny, nx = c3d.shape[:3]
-        desc = capi.FrustumDesc(
-            self.num_3dconvs, self.cv_channels, self.out_channels,
-            self.in_sem_channels, int(self.sem_atten_feat),
-            int(self.stereo_atten_feat), int(self.cat_img_feature), d, h, w, sh,
-            sw, f, nx, ny, nz, float(self.depth_cfg['depth_min']),
-            float(self.depth_cfg['depth_max']), _IMPL[self.conv_impl])
-        hd = ctypes.c_void_p()
-        capi.check(capi.lib().dfm_frustum_create(
-            ctypes.byref(desc), _ptr(xs), _ptr(ys), _ptr(zs), ctypes.byref(hd)),
-            'dfm_frustum_create')
-        self._handle, self._key = hd, key
-        self._sync = _ParamSync()
+
+        def create_args():
+            nz, ny, nx = c3d.shape[:3]
+            desc = capi.FrustumDesc(
+                self.num_3dconvs, self.cv_channels, self.out_channels,
+                self.in_sem_channels, int(self.sem_atten_feat),
+                int(self.stereo_atten_feat), int(self.cat_img_feature), d, h, w, sh,
+                sw, f, nx, ny, nz, float(self.depth_cfg['depth_min']),
+                float(self.depth_cfg['depth_max']), _IMPL[self.conv_impl])
+            # ctypes arrays own their copies of the axes for the duration of the call
+            return (ctypes.byref(desc),) + tuple((ctypes.c_float * len(a))(*a.tolist())
+                                                 for a in self._separable_centres(c3d))
+
+        return self._ensure(key, create_args)
 
     def forward(self, stereo_feat, stereo_feat_softmax, img_metas,
                 cur_sem_feats=None):
@@ -772,11 +739,7 @@ class FrustumToVoxel(_CudaMirror):
             _check_cuda(cur_sem_feats, 'cur_sem_feats')
             sem = cur_sem_feats.contiguous()
             sh, sw = sem.shape[-2:]
-        self._ensure_handle(d, h, w, sh, sw, f)
-        L = capi.lib()
-        self._sync.sync(self, lambda k, p, m: capi.check(
-            L.dfm_frustum_set_param(self._handle, k, p, m),
-            f'dfm_frustum_set_param({k.decode()})'))
+        L = self._prepare(d, h, w, sh, sw, f)
         nz, ny, nx = self.coordinates_3d.shape[:3]
         pad = img_metas[0]['pad_shape']
         x = stereo_feat.contiguous()
@@ -824,10 +787,7 @@ class HotPathPipeline:
         ho = round(feat_h / bb.cost_sample_factor)
         wo = round(feat_w / bb.cost_sample_factor)
         f = int(self.depth_head.downsample_factor)
-        fr._ensure_handle(bb.num_planes, ho, wo, sem_hw[0], sem_hw[1], f)
-        fr._sync.sync(fr, lambda k, p, m: capi.check(
-            L.dfm_frustum_set_param(fr._handle, k, p, m),
-            f'dfm_frustum_set_param({k.decode()})'))
+        fr._prepare(bb.num_planes, ho, wo, sem_hw[0], sem_hw[1], f)
         nz, ny, nx = fr.coordinates_3d.shape[:3]
         if self._outs is None or self._outs[0][0].shape[-3:] != (nz // 4, ny, nx) or \
                 self._outs[0][1].shape[-2:] != (f * ho, f * wo):
@@ -929,25 +889,6 @@ class _Hourglass2d(nn.Module):
                                bias=False), nn.GroupNorm(32, c))
 
 
-class _HandleMirror(_CudaMirror):
-    """create / destroy / parameter-sync plumbing shared by the 2-D BEV mirrors."""
-    _destroy = None
-
-    def release(self):
-        if getattr(self, '_handle', None) is not None:
-            getattr(capi.lib(), self._destroy)(self._handle)
-            self._handle = None
-
-    def __del__(self):
-        try:
-            self.release()
-        except Exception:
-            pass
-
-    def init_weights(self):
-        pass
-
-
 @NECKS.register_module()
 class SPPUNetNeckTail(_HandleMirror):
     """The last two layers of the reference ``SPPUNetNeck`` (necks/spp_unet_neck.py:60-75
@@ -958,7 +899,7 @@ class SPPUNetNeckTail(_HandleMirror):
     returned ``[B, 32, H, W]`` tensor carries a channels-last twin that our ``DfMBackbone``
     consumes directly.  Patch: ``neck.lastconv = SPPUNetNeckTail(...)`` (it is called with the
     same single tensor argument as the ``nn.Sequential`` it replaces)."""
-    _destroy = 'dfm_stereo_tail_destroy'
+    _family = 'stereo_tail'
 
     def __init__(self, stereo_channels=(32, 32), in_channels=32,
                  norm_cfg=dict(type='GN', num_groups=32, requires_grad=True), conv_impl='auto'):
@@ -967,26 +908,13 @@ class SPPUNetNeckTail(_HandleMirror):
         assert norm_cfg.get('type') == 'GN' and norm_cfg.get('num_groups', 32) == 32
         self.conv_impl = conv_impl
         self.lastconv = nn.Sequential(_ConvGN2d(32, 32), nn.Conv2d(32, 32, 1, bias=False))
-        self._handle = None
-        self._key = None
 
     def forward(self, x):
         _check_cuda(x, 'x')
         self._forward_only(x)
         b, c, h, w = x.shape
         assert c == 32
-        L = capi.lib()
-        key = (h, w, self.conv_impl)
-        if self._handle is None or key != self._key:
-            self.release()
-            hd = ctypes.c_void_p()
-            capi.check(L.dfm_stereo_tail_create(h, w, _IMPL[self.conv_impl], ctypes.byref(hd)),
-                       'dfm_stereo_tail_create')
-            self._handle, self._key = hd, key
-            self._sync = _ParamSync()
-        self._sync.sync(self, lambda k, p, m: capi.check(
-            L.dfm_stereo_tail_set_param(self._handle, k, p, m),
-            f'dfm_stereo_tail_set_param({k.decode()})'))
+        L = self._ensure((h, w, self.conv_impl), lambda: (h, w, _IMPL[self.conv_impl]))
         x = x.contiguous()
         out = torch.empty_like(x)
         twins = []
@@ -1035,8 +963,10 @@ class SPPUNetNeck(_HandleMirror):
     [3 @ H, 64 @ H/2, 128 @ H/4 x 3]).  The ``state_dict`` is the reference's (46 entries, BN
     running statistics included); BatchNorm runs in eval form.  For B == 1 the stereo feature
     carries a channels-last twin that our ``DfMBackbone`` consumes without transposes.
-    Patch: ``model.neck = SPPUNetNeck(**cfg.model.neck)``."""
-    _destroy = 'dfm_spp_neck_destroy'
+    Patch: ``model.neck = SPPUNetNeck(**cfg.model.neck)``.  Debug tensors (channels-last): raw
+    conv outputs 'conv0', 'redir0', 'conv1', 'rpn0', 'rpn1', 'lastconv'; 'pool64' .. 'pool8',
+    'spp64' .. 'spp8', 'concat', 'x0', 'x1'."""
+    _family = 'spp_neck'
 
     def __init__(self, in_channels, start_level, sem_channels=[128, 32], stereo_channels=[32, 32],
                  spp_channel=32, with_upconv=True, cat_img_feature=True, norm_cfg=None,
@@ -1059,8 +989,6 @@ class SPPUNetNeck(_HandleMirror):
         self.upconv_module = _UpconvModule()
         self.lastconv = nn.Sequential(_ConvGN2d(32, 32), nn.Conv2d(32, 32, 1, bias=False))
         self.rpnconv = nn.Sequential(_ConvGN2d(512, 128), _ConvGN2d(128, 32))
-        self._handle = None
-        self._key = None
 
     @staticmethod
     def check_shapes(feats):
@@ -1086,18 +1014,7 @@ class SPPUNetNeck(_HandleMirror):
             _check_cuda(f, f'feats[{i}]')
         self._forward_only(*feats)
         b, _, h, w = feats[0].shape
-        L = capi.lib()
-        key = (h, w, self.conv_impl)
-        if self._handle is None or key != self._key:
-            self.release()
-            hd = ctypes.c_void_p()
-            capi.check(L.dfm_spp_neck_create(h, w, _IMPL[self.conv_impl], ctypes.byref(hd)),
-                       'dfm_spp_neck_create')
-            self._handle, self._key = hd, key
-            self._sync = _ParamSync()
-        self._sync.sync(self, lambda k, p, m: capi.check(
-            L.dfm_spp_neck_set_param(self._handle, k, p, m),
-            f'dfm_spp_neck_set_param({k.decode()})'))
+        L = self._ensure((h, w, self.conv_impl), lambda: (h, w, _IMPL[self.conv_impl]))
         feats = [f.contiguous() for f in feats]
         dev = feats[0].device
         stereo = torch.empty((b, 32, h, w), device=dev)
@@ -1111,20 +1028,15 @@ class SPPUNetNeck(_HandleMirror):
             stereo._dfm_cl = cl
         return stereo, sem
 
-    def debug_tensor(self, name, shape):
-        """Channels-last intermediate of the last forward: raw conv outputs 'conv0', 'redir0',
-        'conv1', 'rpn0', 'rpn1', 'lastconv'; 'pool64' .. 'pool8', 'spp64' .. 'spp8', 'concat',
-        'x0', 'x1' (tests only)."""
-        return _debug_tensor(self._handle, 'dfm_spp_neck_debug_tensor', name, shape)
-
 
 @BACKBONES.register_module()
 class BEVHourglass(_HandleMirror):
     """Drop-in for the reference ``BEVHourglass`` forward with GroupNorm
     (backbones/bev_hourglass.py:11-137; ``backbone_3d`` of
     configs/dfm/dfm_r34_1x8_kitti-3d-3class.py:146-150).  The SyncBN variant is the frozen
-    LiDAR teacher's (config :30-36, training only) and is not mirrored."""
-    _destroy = 'dfm_bev_hourglass_destroy'
+    LiDAR teacher's (config :30-36, training only) and is not mirrored.  Debug tensors: the raw
+    output [H, W, C] of 'compress' and 'conv1' .. 'conv6'."""
+    _family = 'bev_hourglass'
 
     def __init__(self, in_channels, out_channels, norm_cfg=None, output_prehg_feat=True,
                  conv_impl='auto'):
@@ -1139,28 +1051,14 @@ class BEVHourglass(_HandleMirror):
         self.compress_conv = _ConvGN2d(in_channels, out_channels)
         self.bev_hourglass = _Hourglass2d(out_channels)
         self.num_bev_features = out_channels
-        self._handle = None
-        self._key = None
 
     def forward(self, spatial_features):
         _check_cuda(spatial_features, 'spatial_features')
         self._forward_only(spatial_features)
         b, c, ny, nx = spatial_features.shape
         assert c == self.in_channels
-        L = capi.lib()
-        key = (ny, nx, self.conv_impl)
-        if self._handle is None or key != self._key:
-            self.release()
-            desc = capi.BevDesc(self.in_channels, self.out_channels, ny, nx,
-                                _IMPL[self.conv_impl])
-            hd = ctypes.c_void_p()
-            capi.check(L.dfm_bev_hourglass_create(ctypes.byref(desc), ctypes.byref(hd)),
-                       'dfm_bev_hourglass_create')
-            self._handle, self._key = hd, key
-            self._sync = _ParamSync()
-        self._sync.sync(self, lambda k, p, m: capi.check(
-            L.dfm_bev_hourglass_set_param(self._handle, k, p, m),
-            f'dfm_bev_hourglass_set_param({k.decode()})'))
+        L = self._ensure((ny, nx, self.conv_impl), lambda: (ctypes.byref(capi.BevDesc(
+            self.in_channels, self.out_channels, ny, nx, _IMPL[self.conv_impl])),))
         x = spatial_features.contiguous()
         out = torch.empty((b, self.out_channels, ny, nx), device=x.device)
         pre = torch.empty_like(out) if self.output_prehg_feat else None
@@ -1169,10 +1067,6 @@ class BEVHourglass(_HandleMirror):
                 self._handle, _ptr(x[i]), _ptr(pre[i]) if pre is not None else None,
                 _ptr(out[i]), _stream()), 'dfm_bev_hourglass_forward')
         return (pre, out) if self.output_prehg_feat else out   # bev_hourglass.py:46-50
-
-    def debug_tensor(self, name, shape):
-        """Raw output [H, W, C] of 'compress' or 'conv1' .. 'conv6' (tests only)."""
-        return _debug_tensor(self._handle, 'dfm_bev_hourglass_debug_tensor', name, shape)
 
 
 def grid_anchors(anchor_generator, ny, nx, device):
@@ -1324,8 +1218,10 @@ class LIGAAnchor3DHead(_HandleMirror):
     12-128): ``forward(feats) -> ([cls_score], [bbox_pred], [dir_cls_preds])``, and the
     inherited ``get_bboxes`` (anchors, decode, rotated BEV NMS) on CUDA.  Target assignment
     and losses stay with the reference's PyTorch code; the constructor keeps their arguments
-    so the config block builds unchanged."""
-    _destroy = 'dfm_anchor_head_destroy'
+    so the config block builds unchanged.  Debug tensors: the raw output [ny, nx, C] of
+    'cls<i>' / 'reg<i>' and of the output convs 'cls_out' (cls + dir channels) / 'reg_out', at
+    their widths padded to 32."""
+    _family = 'anchor_head'
 
     def __init__(self, num_classes, in_channels, feat_channels=256, num_convs=2,
                  norm_cfg=None, use_direction_classifier=True,
@@ -1360,8 +1256,6 @@ class LIGAAnchor3DHead(_HandleMirror):
         self.conv_reg = nn.Conv2d(feat_channels, self.num_anchors * self.box_code_size, 3, 1, 1)
         if use_direction_classifier:
             self.conv_dir_cls = nn.Conv2d(feat_channels, self.num_anchors * 2, 1)
-        self._handle = None
-        self._key = None
 
     def forward(self, feats):
         if not isinstance(feats, list):                      # :104-105
@@ -1374,22 +1268,10 @@ class LIGAAnchor3DHead(_HandleMirror):
         self._forward_only(x)
         b, c, ny, nx = x.shape
         assert c == self.in_channels
-        L = capi.lib()
         nd = self.num_anchors * 2 if self.use_direction_classifier else 0
-        key = (ny, nx, self.conv_impl)
-        if self._handle is None or key != self._key:
-            self.release()
-            desc = capi.AnchorHeadDesc(
-                self.in_channels, self.feat_channels, self.num_convs, self.cls_out_channels,
-                self.num_anchors * self.box_code_size, nd, ny, nx, _IMPL[self.conv_impl])
-            hd = ctypes.c_void_p()
-            capi.check(L.dfm_anchor_head_create(ctypes.byref(desc), ctypes.byref(hd)),
-                       'dfm_anchor_head_create')
-            self._handle, self._key = hd, key
-            self._sync = _ParamSync()
-        self._sync.sync(self, lambda k, p, m: capi.check(
-            L.dfm_anchor_head_set_param(self._handle, k, p, m),
-            f'dfm_anchor_head_set_param({k.decode()})'))
+        L = self._ensure((ny, nx, self.conv_impl), lambda: (ctypes.byref(capi.AnchorHeadDesc(
+            self.in_channels, self.feat_channels, self.num_convs, self.cls_out_channels,
+            self.num_anchors * self.box_code_size, nd, ny, nx, _IMPL[self.conv_impl])),))
         x = x.contiguous()
         cls = torch.empty((b, self.cls_out_channels, ny, nx), device=x.device)
         box = torch.empty((b, self.num_anchors * self.box_code_size, ny, nx), device=x.device)
@@ -1400,11 +1282,6 @@ class LIGAAnchor3DHead(_HandleMirror):
                 _ptr(dirc[i]) if dirc is not None else None, _stream()),
                 'dfm_anchor_head_forward')
         return cls, box, dirc
-
-    def debug_tensor(self, name, shape):
-        """Raw output [ny, nx, C] of 'cls<i>' / 'reg<i>' or of the output convs 'cls_out'
-        (cls + dir channels) / 'reg_out', at their widths padded to 32 (tests only)."""
-        return _debug_tensor(self._handle, 'dfm_anchor_head_debug_tensor', name, shape)
 
     def get_bboxes(self, cls_scores, bbox_preds, dir_cls_preds, input_metas, cfg=None,
                    rescale=False):
@@ -1433,7 +1310,7 @@ class Anchor3DHead(_HandleMirror):
     PyTorch code; the constructor keeps their arguments so the config block builds unchanged,
     and the
     ``state_dict`` (``conv_cls`` / ``conv_reg`` / ``conv_dir_cls``) is the reference's."""
-    _destroy = 'dfm_anchor3d_head_destroy'
+    _family = 'anchor3d_head'
 
     def __init__(self, num_classes, in_channels, train_cfg=None, test_cfg=None,
                  feat_channels=256, use_direction_classifier=True,
@@ -1475,8 +1352,6 @@ class Anchor3DHead(_HandleMirror):
         self.conv_reg = nn.Conv2d(feat_channels, self.num_anchors * self.box_code_size, 1)
         if use_direction_classifier:
             self.conv_dir_cls = nn.Conv2d(feat_channels, self.num_anchors * 2, 1)
-        self._handle = None
-        self._key = None
 
     def forward(self, feats):
         outs = [self.forward_single(x) for x in feats]       # multi_apply (:166-185)
@@ -1489,22 +1364,10 @@ class Anchor3DHead(_HandleMirror):
         if c != self.feat_channels:
             raise RuntimeError(f'Anchor3DHead: input has {c} channels, the convs take '
                                f'feat_channels = {self.feat_channels}')
-        L = capi.lib()
         nd = self.num_anchors * 2 if self.use_direction_classifier else 0
         nr = self.num_anchors * self.box_code_size
-        key = (ny, nx, self.conv_impl)
-        if self._handle is None or key != self._key:
-            self.release()
-            desc = capi.Anchor3DHeadDesc(self.feat_channels, self.cls_out_channels, nr, nd,
-                                         ny, nx, _IMPL[self.conv_impl])
-            hd = ctypes.c_void_p()
-            capi.check(L.dfm_anchor3d_head_create(ctypes.byref(desc), ctypes.byref(hd)),
-                       'dfm_anchor3d_head_create')
-            self._handle, self._key = hd, key
-            self._sync = _ParamSync()
-        self._sync.sync(self, lambda k, p, m: capi.check(
-            L.dfm_anchor3d_head_set_param(self._handle, k, p, m),
-            f'dfm_anchor3d_head_set_param({k.decode()})'))
+        L = self._ensure((ny, nx, self.conv_impl), lambda: (ctypes.byref(capi.Anchor3DHeadDesc(
+            self.feat_channels, self.cls_out_channels, nr, nd, ny, nx, _IMPL[self.conv_impl])),))
         x = x.contiguous()
         cls = torch.empty((b, self.cls_out_channels, ny, nx), device=x.device)
         box = torch.empty((b, nr, ny, nx), device=x.device)
@@ -1549,8 +1412,10 @@ class FPN(_HandleMirror):
     ``num_outs`` other than the number of levels raise ``NotImplementedError``.  It is
     registered in the local ``NECKS`` only: KITTI's ``neck_2d`` is also an mmdet ``FPN`` (with
     extra convs) and must keep resolving to mmdet's class.
-    Patch: ``model.neck = FPN(**cfg.model.neck)``."""
-    _destroy = 'dfm_fpn_destroy'
+    Patch: ``model.neck = FPN(**cfg.model.neck)``.  Debug tensors (channels-last [B, H, W, C]):
+    the merged laterals 'merged0' .. 'merged3' and the raw fpn_conv outputs before the bias
+    'fpn0' .. 'fpn3'."""
+    _family = 'fpn'
 
     def __init__(self, in_channels, out_channels, num_outs, start_level=0, end_level=-1,
                  add_extra_convs=False, relu_before_extra_convs=False, no_norm_on_lateral=False,
@@ -1590,8 +1455,6 @@ class FPN(_HandleMirror):
                                            for c in in_channels)
         self.fpn_convs = nn.ModuleList(_ConvModuleConv(out_channels, out_channels, 3)
                                        for _ in in_channels)
-        self._handle = None
-        self._key = None
 
     def check_shapes(self, inputs):
         """Raises ValueError on inputs that disagree with the constructor."""
@@ -1613,38 +1476,23 @@ class FPN(_HandleMirror):
         outs = tuple(torch.empty((b, self.out_channels) + s, device=dev) for s in sizes)
         if b == 0:
             return outs
-        L = capi.lib()
-        key = (tuple(sizes), self.conv_impl)
-        if self._handle is not None and key == self._key and b != self._batch:
-            # another batch size keeps the handle and its uploaded parameters
-            capi.check(L.dfm_fpn_set_num_images(self._handle, b), 'dfm_fpn_set_num_images')
-            self._batch = b
-        if self._handle is None or key != self._key:
-            self.release()
+
+        def create_args():
             desc = capi.FpnDesc()
             desc.in_channels[:] = self.in_channels
             desc.out_channels = self.out_channels
             desc.level_h[:] = [s[0] for s in sizes]
             desc.level_w[:] = [s[1] for s in sizes]
             desc.num_images, desc.conv_impl = b, _IMPL[self.conv_impl]
-            hd = ctypes.c_void_p()
-            capi.check(L.dfm_fpn_create(ctypes.byref(desc), ctypes.byref(hd)), 'dfm_fpn_create')
-            self._handle, self._key, self._batch = hd, key, b
-            self._sync = _ParamSync()
-        self._sync.sync(self, lambda k, p, m: capi.check(
-            L.dfm_fpn_set_param(self._handle, k, p, m), f'dfm_fpn_set_param({k.decode()})'))
+            return (ctypes.byref(desc),)
+
+        L = self._ensure((tuple(sizes), self.conv_impl), create_args, batch=b)
         xs = [x.contiguous() for x in inputs]
         arr = ctypes.c_void_p * 4
         capi.check(L.dfm_fpn_forward(self._handle, arr(*[x.data_ptr() for x in xs]),
                                      arr(*[o.data_ptr() for o in outs]), _stream()),
                    'dfm_fpn_forward')
         return outs
-
-    def debug_tensor(self, name, shape):
-        """Channels-last [B, H, W, C] intermediate of the last forward: the merged laterals
-        'merged0' .. 'merged3' and the raw fpn_conv outputs before the bias 'fpn0' .. 'fpn3'
-        (tests only)."""
-        return _debug_tensor(self._handle, 'dfm_fpn_debug_tensor', name, shape)
 
 
 class _LigaBasicBlock(nn.Module):
@@ -1675,8 +1523,10 @@ class LIGAResNet(_HandleMirror):
     dilations or channel factors, ``with_max_pool``, ``block_with_final_relu``, ``deep_stem``,
     ``avg_down``, ``dcn``, ``plugins`` and non-BN norms raise ``NotImplementedError``.  It is
     registered in the local ``BACKBONES`` only (forward-only: training keeps mmdet3d's class).
-    Patch: ``model.backbone = LIGAResNet(**cfg.model.backbone)``."""
-    _destroy = 'dfm_liga_resnet_destroy'
+    Patch: ``model.backbone = LIGAResNet(**cfg.model.backbone)``.  Debug tensors (channels-last
+    [B, h, w, C]): 'stem' (raw conv1), 'layerI.J.conv1' / 'layerI.J.conv2' /
+    'layer2.0.downsample' (raw conv outputs) and the block outputs 'layerI.J'."""
+    _family = 'liga_resnet'
     STAGE_BLOCKS = (3, 4, 6, 3)
 
     def __init__(self, depth, in_channels=3, stem_channels=None, base_channels=64, num_stages=4,
@@ -1732,8 +1582,6 @@ class LIGAResNet(_HandleMirror):
                 inplanes = planes
             self.add_module(f'layer{i + 1}', nn.Sequential(*blocks))
             self.res_layers.append(f'layer{i + 1}')
-        self._handle = None
-        self._key = None
 
     @staticmethod
     def output_sizes(h, w):
@@ -1760,36 +1608,14 @@ class LIGAResNet(_HandleMirror):
             tuple(torch.empty((b, 128, h4, w4), device=dev) for _ in range(3))
         if b == 0:
             return outs
-        L = capi.lib()
-        key = (h, w, self.conv_impl)
-        if self._handle is not None and key == self._key and b != self._batch:
-            # another batch size keeps the handle and its uploaded parameters
-            capi.check(L.dfm_liga_resnet_set_num_images(self._handle, b),
-                       'dfm_liga_resnet_set_num_images')
-            self._batch = b
-        if self._handle is None or key != self._key:
-            self.release()
-            desc = capi.LigaResNetDesc(h, w, b, _IMPL[self.conv_impl])
-            hd = ctypes.c_void_p()
-            capi.check(L.dfm_liga_resnet_create(ctypes.byref(desc), ctypes.byref(hd)),
-                       'dfm_liga_resnet_create')
-            self._handle, self._key, self._batch = hd, key, b
-            self._sync = _ParamSync()
-        self._sync.sync(self, lambda k, p, m: capi.check(
-            L.dfm_liga_resnet_set_param(self._handle, k, p, m),
-            f'dfm_liga_resnet_set_param({k.decode()})'))
+        L = self._ensure((h, w, self.conv_impl), lambda: (ctypes.byref(capi.LigaResNetDesc(
+            h, w, b, _IMPL[self.conv_impl])),), batch=b)
         x = img.contiguous()
         arr = ctypes.c_void_p * 4
         capi.check(L.dfm_liga_resnet_forward(self._handle, _ptr(x),
                                              arr(*[o.data_ptr() for o in outs]), _stream()),
                    'dfm_liga_resnet_forward')
         return outs
-
-    def debug_tensor(self, name, shape):
-        """Channels-last [B, h, w, C] intermediate of the last forward: 'stem' (raw conv1),
-        'layerI.J.conv1' / 'layerI.J.conv2' / 'layer2.0.downsample' (raw conv outputs) and the
-        block outputs 'layerI.J' (tests only)."""
-        return _debug_tensor(self._handle, 'dfm_liga_resnet_debug_tensor', name, shape)
 
 
 class _ModulatedDeformConv2dPack(nn.Module):
@@ -1838,8 +1664,12 @@ class ResNet(_HandleMirror):
     other DCN placement, caffe style, deep stem, plugins, non-BN norms, ...) raises
     ``NotImplementedError``.  It is registered in the local ``BACKBONES`` only, never over
     mmdet's global ``ResNet`` (forward-only: training keeps mmdet's class).
-    Patch: ``model.backbone = ResNet(**cfg.model.backbone)``."""
-    _destroy = 'dfm_resnet101_destroy'
+    Patch: ``model.backbone = ResNet(**cfg.model.backbone)``.  Debug tensors (channels-last
+    [B, h, w, C]): 'stem' (raw conv1), 'pool', 'layerI.J.conv1' / '.conv2' / '.conv3' /
+    'layerI.0.downsample' (raw conv outputs), 'layerI.J.conv2.conv_offset' (conv_offset + bias,
+    32 channels of which 27 are real), 'layerI.J.conv2.offset_mask' (the same with the sigmoid
+    on channels 18..26) and the block outputs 'layerI.J'."""
+    _family = 'resnet101'
     STAGE_BLOCKS = (3, 4, 23, 3)
     DCN = dict(type='DCNv2', deform_groups=1, fallback_on_stride=False)
 
@@ -1895,8 +1725,6 @@ class ResNet(_HandleMirror):
                 inplanes = planes * 4
             self.add_module(f'layer{i + 1}', nn.Sequential(*blocks))
             self.res_layers.append(f'layer{i + 1}')
-        self._handle = None
-        self._key = None
 
     @staticmethod
     def output_sizes(h, w):
@@ -1926,38 +1754,14 @@ class ResNet(_HandleMirror):
         outs = tuple(torch.empty((b, 256 << l) + sizes[l], device=dev) for l in range(4))
         if b == 0:
             return outs
-        L = capi.lib()
-        key = (h, w, self.conv_impl)
-        if self._handle is not None and key == self._key and b != self._batch:
-            # another batch size keeps the handle and its uploaded parameters
-            capi.check(L.dfm_resnet101_set_num_images(self._handle, b),
-                       'dfm_resnet101_set_num_images')
-            self._batch = b
-        if self._handle is None or key != self._key:
-            self.release()
-            desc = capi.ResNet101Desc(h, w, b, _IMPL[self.conv_impl])
-            hd = ctypes.c_void_p()
-            capi.check(L.dfm_resnet101_create(ctypes.byref(desc), ctypes.byref(hd)),
-                       'dfm_resnet101_create')
-            self._handle, self._key, self._batch = hd, key, b
-            self._sync = _ParamSync()
-        self._sync.sync(self, lambda k, p, m: capi.check(
-            L.dfm_resnet101_set_param(self._handle, k, p, m),
-            f'dfm_resnet101_set_param({k.decode()})'))
+        L = self._ensure((h, w, self.conv_impl), lambda: (ctypes.byref(capi.ResNet101Desc(
+            h, w, b, _IMPL[self.conv_impl])),), batch=b)
         x = img.contiguous()
         arr = ctypes.c_void_p * 4
         capi.check(L.dfm_resnet101_forward(self._handle, _ptr(x),
                                            arr(*[o.data_ptr() for o in outs]), _stream()),
                    'dfm_resnet101_forward')
         return outs
-
-    def debug_tensor(self, name, shape):
-        """Channels-last [B, h, w, C] intermediate of the last forward: 'stem' (raw conv1),
-        'pool', 'layerI.J.conv1' / '.conv2' / '.conv3' / 'layerI.0.downsample' (raw conv
-        outputs), 'layerI.J.conv2.conv_offset' (conv_offset + bias, 32 channels of which 27 are
-        real), 'layerI.J.conv2.offset_mask' (the same with the sigmoid on channels 18..26) and
-        the block outputs 'layerI.J' (tests only)."""
-        return _debug_tensor(self._handle, 'dfm_resnet101_debug_tensor', name, shape)
 
 
 def aligned_voxel_centers(n_voxels, voxel_range):
