@@ -12,7 +12,8 @@ DEPS = [os.path.join(HERE, 'csrc', f) for f in
          'neck_api.inc', 'frustum_api.inc', 'frustum_kernels.cuh', 'pipeline_api.inc', 'bev_api.inc', 'tail_kernels.cuh', 'voxel_sample_api.inc', 'stereo_tail_api.inc', 'logits_tc.cuh', 'wgmma.cuh', 'head1x1_tc.cuh', 'anchor3d_head_api.inc', 'spp_neck_kernels.cuh',
          'spp_neck_api.inc', 'fpn_kernels.cuh', 'fpn_api.inc', 'resnet_kernels.cuh',
          'liga_resnet_api.inc', 'resnet101_kernels.cuh', 'resnet101_api.inc',
-         'box_post_kernels.cuh', 'box_post_api.inc', 'image_prep_kernels.cuh',
+         'box_post_kernels.cuh', 'box_post_api.inc', 'anchor_loss_kernels.cuh',
+         'anchor_loss_api.inc', 'image_prep_kernels.cuh',
          'image_prep_api.inc', 'view_cache_kernels.cuh', 'view_cache_api.inc',
          'kitti_eval_kernels.cuh', 'kitti_eval_api.inc', 'waymo_eval_kernels.cuh',
          'waymo_eval_api.inc')] + [os.path.join(HERE, '..', 'include', 'dfm_b200.h')]

@@ -61,7 +61,8 @@ SYMBOLS = (
     'dfm_resnet101_set_num_images', 'dfm_kitti_eval_create', 'dfm_kitti_eval_destroy',
     'dfm_kitti_eval_forward', 'dfm_kitti_eval_debug_tensor', 'dfm_op_eval_rotated_iou',
     'dfm_op_let_iou', 'dfm_kitti_eval_set_overlap_limit', 'dfm_kitti_eval_workspace',
-    'dfm_waymo_kitti_convert',
+    'dfm_waymo_kitti_convert', 'dfm_anchor_loss_create', 'dfm_anchor_loss_destroy',
+    'dfm_anchor_loss_forward', 'dfm_anchor_loss_finish', 'dfm_anchor_loss_debug_tensor',
 )
 
 DFM_IMAGE_PREP_CROP, DFM_IMAGE_PREP_RESCALE = 0, 1
@@ -151,6 +152,18 @@ class BoxPostDesc(ctypes.Structure):
     _fields_ = [(n, c_int) for n in ('num_classes', 'num_anchors', 'ny', 'nx', 'batch',
                                      'use_sigmoid', 'nms_pre', 'max_num')] + \
                [(n, c_float) for n in ('score_thr', 'nms_thr', 'dir_offset', 'dir_limit_offset')]
+
+
+class AnchorLossDesc(ctypes.Structure):
+    """``dfm_anchor_loss_desc_t``."""
+    _fields_ = [(n, c_int) for n in ('num_classes', 'num_sizes', 'num_rotations', 'ny', 'nx',
+                                     'batch', 'assign_per_class', 'diff_rad_by_sin',
+                                     'use_direction_classifier', 'with_iou', 'liga')] + \
+               [(n, c_float * 8) for n in ('pos_iou_thr', 'neg_iou_thr', 'min_pos_iou')] + \
+               [(n, c_float) for n in ('pos_weight', 'gamma', 'alpha', 'beta')] + \
+               [('loss_weight', c_float * 4)] + \
+               [(n, c_float) for n in ('dir_offset', 'dir_limit_offset',
+                                       'normalizer_clamp_value')]
 
 
 class ImagePrepDesc(ctypes.Structure):
@@ -279,6 +292,11 @@ def lib():
     L.dfm_box_post_destroy.argtypes = [vp]
     L.dfm_box_post_forward.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.dfm_op_rotated_iou.argtypes = [vp, vp, c_int, vp, vp]
+    L.dfm_anchor_loss_create.argtypes = [POINTER(AnchorLossDesc), vp, POINTER(vp)]
+    L.dfm_anchor_loss_destroy.argtypes = [vp]
+    L.dfm_anchor_loss_forward.argtypes = [vp] * 14
+    L.dfm_anchor_loss_finish.argtypes = [vp] * 5
+    L.dfm_anchor_loss_debug_tensor.argtypes = [vp, c_char_p, vp, c_longlong, vp]
     L.dfm_voxel_sample.argtypes = [POINTER(VoxelSampleDesc), vp, vp, POINTER(c_double), vp, vp]
     L.dfm_kitti_eval_create.argtypes = [POINTER(KittiEvalDesc), POINTER(vp)]
     L.dfm_kitti_eval_destroy.argtypes = [vp]

@@ -193,6 +193,21 @@ __global__ void __launch_bounds__(1024) bp_topk_sort_kernel(BoxPostParams p) {
 
 // ---- decode (DeltaXYZWLHRBBoxCoder.decode, op for op) and per-class candidate lists ----
 
+// box = decode(an, t): both [7] (x, y, z, w, l, h, yaw), z at the bottom centre
+__device__ __forceinline__ void bp_decode_box(const float* t, const float* an, float* box) {
+  const float xa = an[0], ya = an[1], wa = an[3], la = an[4], ha = an[5], ra = an[6];
+  const float za = __fadd_rn(an[2], __fdiv_rn(ha, 2.f));
+  const float diag = __fsqrt_rn(__fadd_rn(__fmul_rn(la, la), __fmul_rn(wa, wa)));
+  box[0] = __fadd_rn(__fmul_rn(t[0], diag), xa);
+  box[1] = __fadd_rn(__fmul_rn(t[1], diag), ya);
+  const float zg = __fadd_rn(__fmul_rn(t[2], ha), za);
+  box[4] = __fmul_rn(expf(t[4]), la);
+  box[3] = __fmul_rn(expf(t[3]), wa);
+  box[5] = __fmul_rn(expf(t[5]), ha);
+  box[6] = __fadd_rn(t[6], ra);
+  box[2] = __fsub_rn(zg, __fdiv_rn(box[5], 2.f));
+}
+
 __global__ void bp_decode_kernel(BoxPostParams p) {
   const int b = blockIdx.y;
   const int slot = blockIdx.x * blockDim.x + threadIdx.x;
@@ -210,19 +225,9 @@ __global__ void bp_decode_kernel(BoxPostParams p) {
     t[k] = __ldg(rg + (size_t)k * p.HW);
     an[k] = __ldg(p.anchors + (size_t)a * 7 + k);
   }
-  const float xa = an[0], ya = an[1], wa = an[3], la = an[4], ha = an[5], ra = an[6];
-  const float za = __fadd_rn(an[2], __fdiv_rn(ha, 2.f));
-  const float diag = __fsqrt_rn(__fadd_rn(__fmul_rn(la, la), __fmul_rn(wa, wa)));
-  const float xg = __fadd_rn(__fmul_rn(t[0], diag), xa);
-  const float yg = __fadd_rn(__fmul_rn(t[1], diag), ya);
-  float zg = __fadd_rn(__fmul_rn(t[2], ha), za);
-  const float lg = __fmul_rn(expf(t[4]), la);
-  const float wg = __fmul_rn(expf(t[3]), wa);
-  const float hg = __fmul_rn(expf(t[5]), ha);
-  const float rgo = __fadd_rn(t[6], ra);
-  zg = __fsub_rn(zg, __fdiv_rn(hg, 2.f));
   float* box = p.boxes + ((size_t)b * p.K + slot) * 7;
-  box[0] = xg; box[1] = yg; box[2] = zg; box[3] = wg; box[4] = lg; box[5] = hg; box[6] = rgo;
+  bp_decode_box(t, an, box);
+  const float xg = box[0], yg = box[1], wg = box[3], lg = box[4], rgo = box[6];
   p.dirlab[(size_t)b * p.K + slot] = dl;
   // bev = [x, y, dx, dy, yaw]; xywhr2xyxyr, then nms_bev's way back to xywhr
   const float hw = __fdiv_rn(wg, 2.f), hh = __fdiv_rn(lg, 2.f);

@@ -28,6 +28,7 @@
 #include "resnet_kernels.cuh"
 #include "resnet101_kernels.cuh"
 #include "box_post_kernels.cuh"
+#include "anchor_loss_kernels.cuh"
 #include "image_prep_kernels.cuh"
 #include "view_cache_kernels.cuh"
 #include "kitti_eval_kernels.cuh"
@@ -1598,6 +1599,7 @@ int dfm_depth_head_forward(const float* d_cost, const float* d_depth_samples, in
 #include "liga_resnet_api.inc"
 #include "resnet101_api.inc"
 #include "box_post_api.inc"
+#include "anchor_loss_api.inc"
 #include "image_prep_api.inc"
 #include "view_cache_api.inc"
 #include "kitti_eval_api.inc"

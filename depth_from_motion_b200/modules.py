@@ -1212,13 +1212,244 @@ class _BoxPost:
         return out
 
 
+def _dist_reduce_mean(t):
+    """``dist_reduce_mean`` (models/utils/common_utils.py): the all-reduced mean over ranks when
+    ``torch.distributed`` is initialised, ``t`` itself otherwise."""
+    import torch.distributed as dist
+    if dist.is_available() and dist.is_initialized():
+        t = t / dist.get_world_size()   # a new tensor: the caller's count stays as it was
+        dist.all_reduce(t)              # sums over ranks in place
+    return t
+
+
+def _loss_config(head, liga):
+    """The loss settings both heads read from their config, with the refusals of what the shipped
+    configs never use."""
+    ex = head.extra_cfg
+    get = (lambda k, d: ex.get(k, d)) if liga else (lambda k, d: getattr(head, k, d))
+    lc, lb, ld, li = (ex.get(k) for k in ('loss_cls', 'loss_bbox', 'loss_dir', 'loss_iou'))
+    if lc is None or lc.get('type') != 'FocalLoss' or not lc.get('use_sigmoid', True):
+        raise NotImplementedError('loss: loss_cls must be a sigmoid FocalLoss (sampling samplers '
+                                  'are not implemented)')
+    if lb is None or lb.get('type') != 'SmoothL1Loss' or \
+            lb.get('reduction', 'mean') != 'mean':
+        raise NotImplementedError('loss: loss_bbox must be SmoothL1Loss with mean reduction')
+    if not head.use_direction_classifier or ld is None or \
+            ld.get('type') != 'CrossEntropyLoss' or ld.get('use_sigmoid', False):
+        raise NotImplementedError('loss: needs the direction classifier with a softmax '
+                                  'CrossEntropyLoss')
+    if li is not None and (not liga or li.get('type') != 'IOU3DLoss'):
+        raise NotImplementedError('loss: loss_iou must be LIGAAnchor3DHead\'s IOU3DLoss')
+    if get('assigner_per_size', False):
+        raise NotImplementedError('loss: assigner_per_size is not implemented')
+    cfg = head.train_cfg or {}
+    if cfg.get('code_weight'):
+        raise NotImplementedError('loss: train_cfg.code_weight is not implemented')
+    assigners = cfg.get('assigner')
+    g = dict(ex['anchor_generator'])
+    num_sizes = len(np.asarray(g.get('sizes', [[3.9, 1.6, 1.56]])).reshape(-1, 3))
+    if not isinstance(assigners, (list, tuple)) or len(assigners) != num_sizes:
+        raise NotImplementedError('loss: train_cfg.assigner must list one MaxIoUAssigner per '
+                                  'anchor size')
+    thr = []
+    for a in assigners:
+        if a.get('type') != 'MaxIoUAssigner' or \
+                a.get('iou_calculator', {}).get('type') != 'BboxOverlapsNearest3D' or \
+                a.get('iou_calculator', {}).get('coordinate', 'lidar') != 'lidar' or \
+                a.get('ignore_iof_thr', -1) > 0 or not a.get('match_low_quality', True) or \
+                not a.get('gt_max_assign_all', True) or \
+                not isinstance(a.get('neg_iou_thr'), (int, float)):
+            raise NotImplementedError(f'loss: assigner {a} is not implemented')
+        thr.append((float(a['pos_iou_thr']), float(a['neg_iou_thr']),
+                    float(a.get('min_pos_iou', 0.0))))
+    C = head.num_classes
+    return dict(
+        num_classes=C, num_sizes=num_sizes,
+        num_rots=len(g.get('rotations', [0, 1.5707963])),
+        assign_per_class=bool(get('assign_per_class', False)),
+        diff_rad_by_sin=bool(get('diff_rad_by_sin', True)), with_iou=li is not None, liga=liga,
+        thr=thr, pos_weight=float(cfg.get('pos_weight', -1)),
+        gamma=float(lc.get('gamma', 2.0)), alpha=float(lc.get('alpha', 0.25)),
+        beta=float(lb.get('beta', 1.0)),
+        loss_weight=[float(lc.get('loss_weight', 1.0)), float(lb.get('loss_weight', 1.0)),
+                     float(ld.get('loss_weight', 1.0)),
+                     float(li.get('loss_weight', 1.0)) if li is not None else 0.0],
+        dir_offset=float(get('dir_offset', -np.pi / 2)),
+        dir_limit_offset=float(get('dir_limit_offset', 0)),
+        normalizer_clamp_value=float(getattr(head, 'normalizer_clamp_value', 0)),
+        reduce_avg_factor=bool(getattr(head, 'reduce_avg_factor', False)) and liga)
+
+
+class _AnchorLossFn(torch.autograd.Function):
+    """The four loss values of one ``dfm_anchor_loss_forward`` / ``_finish``.  Forward stores the
+    gradients of the loss sums of the inputs that require grad; backward scales each by its
+    loss's normaliser, weight and ``grad_output``."""
+
+    @staticmethod
+    def forward(ctx, cls, box, dirc, loss):
+        need = ctx.needs_input_grad
+        g_cls = torch.empty_like(cls) if need[0] else None
+        g_box = torch.empty_like(box) if need[1] else None
+        g_dir = torch.empty_like(dirc) if need[2] else None
+        g_iou = torch.empty_like(box) if need[1] and loss.cfg['with_iou'] else None
+        scales = loss.forward(cls, box, dirc, g_cls, g_box, g_dir, g_iou)
+        ctx.grads = (g_cls, g_box, g_dir, g_iou)
+        ctx.save_for_backward(scales)
+        return loss.losses
+
+    @staticmethod
+    def backward(ctx, g):
+        scales, = ctx.saved_tensors
+        s = scales * g
+        g_cls, g_box, g_dir, g_iou = ctx.grads
+        gb = g_box * s[1] if g_box is not None else None
+        if g_iou is not None:
+            gb = gb + g_iou * s[3]
+        return (g_cls * s[0] if g_cls is not None else None, gb,
+                g_dir * s[2] if g_dir is not None else None, None)
+
+
+class _AnchorLoss:
+    """``loss`` of both anchor heads through ``dfm_anchor_loss_*``: one handle and anchor table per
+    (feature map size, batch, device, loss config), kept until the key changes."""
+
+    def __init__(self):
+        self.handle, self.key = None, None
+
+    def release(self):
+        if self.handle is not None:
+            capi.lib().dfm_anchor_loss_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
+
+    def run(self, head, liga, cls_scores, bbox_preds, dir_cls_preds, gt_bboxes, gt_labels,
+            input_metas, gt_bboxes_ignore):
+        cfg = _loss_config(head, liga)
+        if gt_bboxes_ignore is not None and any(g is not None and len(g) for g in
+                                                gt_bboxes_ignore):
+            raise NotImplementedError('loss: gt_bboxes_ignore is not implemented')
+        if len(cls_scores) != 1 or len(bbox_preds) != 1 or len(dir_cls_preds) != 1:
+            raise NotImplementedError('loss takes one feature level')
+        B = len(input_metas)
+        if len(gt_bboxes) != B or len(gt_labels) != B:
+            raise RuntimeError(f'loss: {B} input_metas, {len(gt_bboxes)} gt_bboxes and '
+                               f'{len(gt_labels)} gt_labels')
+        cls, box, dirc = cls_scores[0], bbox_preds[0], dir_cls_preds[0]
+        for name, t in (('cls_score', cls), ('bbox_pred', box), ('dir_cls_pred', dirc)):
+            _check_cuda(t, name)
+        dev = cls.device
+        ny, nx = cls.shape[-2:]
+        A, C = head.num_anchors, cfg['num_classes']
+        if A != cfg['num_sizes'] * cfg['num_rots'] or cls.shape != (B, A * C, ny, nx) or \
+                box.shape != (B, A * 7, ny, nx) or dirc.shape != (B, A * 2, ny, nx):
+            raise RuntimeError(f'loss: unexpected head output shapes {tuple(cls.shape)}, '
+                               f'{tuple(box.shape)}, {tuple(dirc.shape)}')
+        boxes, labels, off = [], [], [0]
+        for gb, gl in zip(gt_bboxes, gt_labels):
+            gb = gb.tensor if hasattr(gb, 'tensor') else gb
+            if gb.dim() != 2 or gb.shape[1] != 7:
+                raise NotImplementedError(f'loss: GT boxes must be [M, 7], got '
+                                          f'{tuple(gb.shape)}')
+            if gl.shape != (gb.shape[0],):
+                raise RuntimeError('loss: every sample needs one label per GT box')
+            # labels still on the host are checked here; on the device the kernels flag them
+            # and every loss comes out NaN (no host synchronisation on the CUDA path)
+            if not gl.is_cuda and gl.numel() and (int(gl.min()) < 0 or int(gl.max()) >= C):
+                raise ValueError(f'loss: GT labels must lie in 0..{C - 1}')
+            boxes.append(gb.to(dev, torch.float32))
+            labels.append(gl.to(dev, torch.int32))
+            off.append(off[-1] + gb.shape[0])
+        self.gt = torch.cat(boxes).contiguous()
+        self.gt_labels = torch.cat(labels).contiguous()
+        self.h_off = (ctypes.c_int * (B + 1))(*off)
+        self.d_off = torch.tensor(off, dtype=torch.int32).to(dev, non_blocking=True)
+        t = cfg['thr'] + [(0.0, 0.0, 0.0)] * (8 - len(cfg['thr']))
+        desc_args = (C, cfg['num_sizes'], cfg['num_rots'], ny, nx, B,
+                     int(cfg['assign_per_class']), int(cfg['diff_rad_by_sin']), 1,
+                     int(cfg['with_iou']), int(liga),
+                     (ctypes.c_float * 8)(*[x[0] for x in t]),
+                     (ctypes.c_float * 8)(*[x[1] for x in t]),
+                     (ctypes.c_float * 8)(*[x[2] for x in t]),
+                     cfg['pos_weight'], cfg['gamma'], cfg['alpha'], cfg['beta'],
+                     (ctypes.c_float * 4)(*cfg['loss_weight']), cfg['dir_offset'],
+                     cfg['dir_limit_offset'], cfg['normalizer_clamp_value'])
+        key = (repr(sorted((k, repr(v)) for k, v in cfg.items())), ny, nx, B, str(dev))
+        L = capi.lib()
+        if self.handle is None or key != self.key:
+            self.release()
+            with torch.cuda.device(dev):
+                anchors = grid_anchors(head.extra_cfg['anchor_generator'], ny, nx, dev)
+            self.anchors = anchors
+            anchors = anchors.cpu().contiguous()
+            hd = ctypes.c_void_p()
+            with torch.cuda.device(dev):
+                capi.check(L.dfm_anchor_loss_create(ctypes.byref(capi.AnchorLossDesc(*desc_args)),
+                                                    _ptr(anchors), ctypes.byref(hd)),
+                           'dfm_anchor_loss_create')
+            self.handle, self.key, self.batch, self.n = hd, key, B, ny * nx * A
+        self.cfg = cfg
+        losses = _AnchorLossFn.apply(cls.contiguous(), box.contiguous(), dirc.contiguous(), self)
+        out = dict(loss_cls=[losses[0]], loss_bbox=[losses[1]], loss_dir=[losses[2]])
+        if cfg['with_iou']:
+            out['loss_iou'] = [losses[3]]
+        return out
+
+    def forward(self, cls, box, dirc, g_cls, g_box, g_dir, g_iou):
+        """Runs the handle; sets ``self.losses`` [4] and returns the gradient scales [4]."""
+        L = capi.lib()
+        dev = cls.device
+        norm = torch.empty(1, device=dev)
+        with torch.cuda.device(dev):
+            capi.check(L.dfm_anchor_loss_forward(
+                self.handle, _ptr(cls), _ptr(box), _ptr(dirc), _ptr(self.gt),
+                _ptr(self.gt_labels), _ptr(self.d_off), ctypes.cast(self.h_off, ctypes.c_void_p),
+                _ptr(g_cls), _ptr(g_box), _ptr(g_dir), _ptr(g_iou), _ptr(norm), _stream()),
+                'dfm_anchor_loss_forward')
+            avg = _dist_reduce_mean(norm) if self.cfg['reduce_avg_factor'] else norm
+            self.losses = torch.empty(4, device=dev)
+            scales = torch.empty(4, device=dev)
+            capi.check(L.dfm_anchor_loss_finish(self.handle, _ptr(avg), _ptr(self.losses),
+                                                _ptr(scales), _stream()),
+                       'dfm_anchor_loss_finish')
+        return scales
+
+    def debug_tensor(self, name):
+        """Per-anchor target of the last call (tests only): 'assigned_gt', 'labels',
+        'dir_targets' int32 [batch, N]; 'label_weights' fp32 [batch, N]; 'bbox_targets' fp32
+        [batch, N, 7]."""
+        if self.handle is None:
+            raise RuntimeError('dfm_anchor_loss_debug_tensor: no loss call has run')
+        shape = (self.batch, self.n) + ((7,) if name == 'bbox_targets' else ())
+        dt = torch.float32 if name in ('label_weights', 'bbox_targets') else torch.int32
+        out = torch.empty(shape, device='cuda', dtype=dt)
+        capi.check(capi.lib().dfm_anchor_loss_debug_tensor(self.handle, name.encode(), _ptr(out),
+                                                           out.numel(), _stream()),
+                   f'dfm_anchor_loss_debug_tensor({name})')
+        return out
+
+
+_LOSS_DOC = """Training loss (``anchor3d_head.py:328-406`` with ``loss_single``{liga}) on CUDA
+        (``dfm_anchor_loss_*``): ``dict(loss_cls=[t], loss_bbox=[t], loss_dir=[t]{iou})`` of 0-dim
+        device tensors, differentiable with respect to the three head outputs.  ``gt_bboxes``:
+        per sample ``[M, 7]`` LiDAR boxes (tensors or objects with ``.tensor``); ``gt_labels``:
+        ``[M]`` ints in ``0..num_classes-1`` (host labels outside it raise ``ValueError``,
+        device labels make every loss NaN).  Reads ``train_cfg`` as the reference does; one feature level, sigmoid
+        FocalLoss, one MaxIoUAssigner per anchor size; refuses ``gt_bboxes_ignore`` and
+        ``code_weight``.  No host synchronisation."""
+
+
 @HEADS.register_module()
 class LIGAAnchor3DHead(_HandleMirror):
     """Forward of the reference ``LIGAAnchor3DHead`` (dense_heads/liga_anchor3d_head.py:
     12-128): ``forward(feats) -> ([cls_score], [bbox_pred], [dir_cls_preds])``, and the
-    inherited ``get_bboxes`` (anchors, decode, rotated BEV NMS) on CUDA.  Target assignment
-    and losses stay with the reference's PyTorch code; the constructor keeps their arguments
-    so the config block builds unchanged.  Debug tensors: the raw output [ny, nx, C] of
+    inherited ``get_bboxes`` (anchors, decode, rotated BEV NMS) and ``loss`` (target assignment,
+    the four losses and their gradients) on CUDA; the constructor keeps the reference's
+    arguments so the config block builds unchanged.  Debug tensors: the raw output [ny, nx, C] of
     'cls<i>' / 'reg<i>' and of the output convs 'cls_out' (cls + dir channels) / 'reg_out', at
     their widths padded to 32."""
     _family = 'anchor_head'
@@ -1299,6 +1530,25 @@ class LIGAAnchor3DHead(_HandleMirror):
                                   self.extra_cfg.get('dir_offset', -np.pi / 2),
                                   self.extra_cfg.get('dir_limit_offset', 0))
 
+    def loss(self, cls_scores, bbox_preds, dir_cls_preds, gt_bboxes, gt_labels, input_metas,
+             gt_bboxes_ignore=None):
+        if not hasattr(self, '_anchor_loss'):
+            self._anchor_loss = _AnchorLoss()
+        return self._anchor_loss.run(self, True, cls_scores, bbox_preds, dir_cls_preds, gt_bboxes,
+                                     gt_labels, input_metas, gt_bboxes_ignore)
+
+    loss.__doc__ = _LOSS_DOC.format(
+        liga=' of liga_anchor3d_head.py:130-226', iou=', loss_iou=[t] with loss_iou') + \
+        """
+
+        ``avg_factor`` is the all-reduced mean of ``num_total_samples`` under
+        ``torch.distributed`` (``reduce_avg_factor``).  Two departures from the reference's
+        ``loss_iou``: with no positive it is 0 with a zero gradient (the reference's
+        ``iou3d_loss`` asserts), and each positive is decoded against its own anchor (for
+        batch > 1 the reference indexes image 0's anchors with batch-wide indices and fails).
+        Where a decoded target value is NaN (degenerate GT) the prediction's value stands in, as
+        in ``iou3d_loss``, but the gradient does not also flow through the substituted value."""
+
 
 @HEADS.register_module()
 class Anchor3DHead(_HandleMirror):
@@ -1306,10 +1556,9 @@ class Anchor3DHead(_HandleMirror):
     ``bbox_head_3d`` of both MultiViewDfM (Waymo) configs: ``forward(feats) -> ([cls_score],
     [bbox_pred], [dir_cls_preds or None])``.  The three 1x1 convs run as one tensor-core GEMM
     that reads the BEV map once (``csrc/head1x1_tc.cuh``); ``get_bboxes`` (anchors, decode,
-    rotated BEV NMS) runs on CUDA too.  Target assignment and losses stay with the reference's
-    PyTorch code; the constructor keeps their arguments so the config block builds unchanged,
-    and the
-    ``state_dict`` (``conv_cls`` / ``conv_reg`` / ``conv_dir_cls``) is the reference's."""
+    rotated BEV NMS) and ``loss`` (target assignment, losses and their gradients) run on CUDA
+    too; the constructor keeps the reference's arguments so the config block builds unchanged,
+    and the ``state_dict`` (``conv_cls`` / ``conv_reg`` / ``conv_dir_cls``) is the reference's."""
     _family = 'anchor3d_head'
 
     def __init__(self, num_classes, in_channels, train_cfg=None, test_cfg=None,
@@ -1390,6 +1639,15 @@ class Anchor3DHead(_HandleMirror):
         return self._box_post.run(self, cls_scores, bbox_preds, dir_cls_preds, input_metas, cfg,
                                   fg, self.use_sigmoid_cls, self.dir_offset,
                                   self.dir_limit_offset)
+
+    def loss(self, cls_scores, bbox_preds, dir_cls_preds, gt_bboxes, gt_labels, input_metas,
+             gt_bboxes_ignore=None):
+        if not hasattr(self, '_anchor_loss'):
+            self._anchor_loss = _AnchorLoss()
+        return self._anchor_loss.run(self, False, cls_scores, bbox_preds, dir_cls_preds,
+                                     gt_bboxes, gt_labels, input_metas, gt_bboxes_ignore)
+
+    loss.__doc__ = _LOSS_DOC.format(liga='', iou='')
 
 
 class _ConvModuleConv(nn.Module):

@@ -151,7 +151,8 @@ def register_into_mmdet():
                              module=modules.DepthHead)
     # (the detectors DfM / MultiViewDfM are registered locally only: mmdet3d's own stay in
     # place.  LIGAAnchor3DHead and Anchor3DHead are NOT forced into mmdet's registry: the mirrors
-    # implement forward only, the detector needs the reference class's loss / get_bboxes;
+    # have forward, get_bboxes and loss, but no backward through their convs, which the
+    # detector's forward_train needs;
     # BEVHourglass's forward is the whole module)
     MM_BACKBONES.register_module(name='BEVHourglassB200', force=True,
                                  module=modules.BEVHourglass)

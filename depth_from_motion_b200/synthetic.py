@@ -594,3 +594,79 @@ BOX_POST_CASES = {
                                                            score_thr=0.05), False,
                       WAYMO_DIR_OFFSET, 304, dict(num_objects=6, ncol=4)),
 }
+
+
+def _max_iou_assigner(pos, neg):
+    return dict(type='MaxIoUAssigner', iou_calculator=dict(type='BboxOverlapsNearest3D'),
+                pos_iou_thr=pos, neg_iou_thr=neg, min_pos_iou=neg, ignore_iof_thr=-1)
+
+
+# train_cfg and loss settings of the shipped heads (configs/dfm/dfm_r34_1x8_kitti-3d-3class.py:
+# 151-225, configs/dfm/multiview-dfm_r101_dcn_2x16_waymoD5-3d-3class_camsync.py:35-92)
+KITTI_TRAIN_CFG = dict(assigner=[_max_iou_assigner(0.6, 0.45), _max_iou_assigner(0.5, 0.35),
+                                 _max_iou_assigner(0.5, 0.35)],
+                       allowed_border=0, pos_weight=-1, debug=False)
+WAYMO_TRAIN_CFG = dict(assigner=[_max_iou_assigner(0.5, 0.35), _max_iou_assigner(0.5, 0.35),
+                                 _max_iou_assigner(0.6, 0.45)],
+                       allowed_border=0, pos_weight=-1, debug=False)
+FOCAL_LOSS = dict(type='FocalLoss', use_sigmoid=True, gamma=2.0, alpha=0.25, loss_weight=1.0)
+KITTI_LOSSES = dict(loss_cls=FOCAL_LOSS,
+                    loss_bbox=dict(type='SmoothL1Loss', beta=1.0 / 9.0, loss_weight=0.5),
+                    loss_dir=dict(type='CrossEntropyLoss', use_sigmoid=False, loss_weight=0.2),
+                    loss_iou=dict(type='IOU3DLoss', loss_weight=1.0))
+WAYMO_LOSSES = dict(loss_cls=FOCAL_LOSS,
+                    loss_bbox=dict(type='SmoothL1Loss', beta=1.0 / 9.0, loss_weight=2.0),
+                    loss_dir=dict(type='CrossEntropyLoss', use_sigmoid=False, loss_weight=0.2))
+
+
+def make_anchor_loss_case(seed, anchors, ny, nx, num_sizes, num_rots, num_classes, num_gt,
+                          drop_class=None, cross_class=False, head_scale=1.0):
+    """Head outputs ([B, A * C, ny, nx], [B, A * 7, ny, nx], [B, A * 2, ny, nx]) and per-sample GT
+    (``[M, 7]`` boxes, ``[M]`` int64 labels) for ``num_gt[b]`` boxes in sample b, planted on
+    anchors of the table ``anchors`` [ny * nx * A, 7] (numpy fp32): jittered copies of random
+    anchors, labelled by the anchor's size (a random class with ``cross_class``), plus, when a
+    sample has at least 8, the edge cases: a GT equal to an anchor and its duplicate, yaws of
+    exactly +-pi / 4 and beyond +-pi, and a box too small for any anchor to reach min_pos_iou.
+    ``drop_class`` removes that class's GT (an assigner with no GT)."""
+    rng = np.random.RandomState(seed)
+    B, A, C = len(num_gt), num_sizes * num_rots, num_classes
+    cls = (-2.0 + 1.5 * rng.standard_normal((B, A * C, ny, nx))) * head_scale
+    box = 0.2 * rng.standard_normal((B, A * 7, ny, nx)) * head_scale
+    dirc = rng.standard_normal((B, A * 2, ny, nx)) * head_scale
+    gts, labels = [], []
+    for m in num_gt:
+        idx = rng.randint(0, anchors.shape[0], size=m)
+        g = anchors[idx].astype(np.float64).copy()
+        g[:, :2] += rng.uniform(-0.4, 0.4, (m, 2))
+        g[:, 2] += rng.uniform(-0.2, 0.2, m)
+        g[:, 3:6] *= rng.uniform(0.8, 1.25, (m, 3))
+        g[:, 6] += 0.4 * rng.standard_normal(m)
+        lab = (idx % A) // num_rots
+        if cross_class:
+            lab = rng.randint(0, C, size=m)
+        if m >= 8:
+            g[0] = anchors[idx[0]]
+            g[1] = g[0]
+            lab[1] = lab[0]
+            g[2, 6], g[3, 6] = np.float32(np.pi / 4), -np.float32(np.pi / 4)
+            g[4, 6], g[5, 6] = np.pi + 0.3, -np.pi - 0.4
+            g[6, 3:6] = 0.08
+        g = g.astype(np.float32)
+        keep = lab != drop_class if drop_class is not None else np.ones(m, bool)
+        gts.append(torch.from_numpy(g[keep]))
+        labels.append(torch.from_numpy(lab[keep].astype(np.int64)))
+    t = lambda a: torch.from_numpy(a.astype(np.float32))  # noqa: E731
+    return t(cls), t(box), t(dirc), gts, labels
+
+
+# name -> (head: 'liga' (KITTI config) or 'anchor3d' (Waymo config), ny, nx, GT per sample,
+# make_anchor_loss_case arguments, LIGA's loss_iou on, seed): tests/golden/anchor_loss.npz
+ANCHOR_LOSS_GOLDEN_CASES = {
+    'liga_b1': ('liga', 40, 36, [20], {}, True, 401),
+    'liga_b1_class_without_gt': ('liga', 40, 36, [16], dict(drop_class=2), True, 402),
+    'liga_zero_positives': ('liga', 40, 36, [0], {}, False, 403),
+    'liga_b2_one_empty': ('liga', 40, 36, [14, 0], {}, False, 404),
+    'anchor3d_b1_cross_class': ('anchor3d', 30, 22, [60], dict(cross_class=True), False, 405),
+    'anchor3d_b2': ('anchor3d', 30, 22, [40, 30], dict(cross_class=True), False, 406),
+    'anchor3d_b2_one_empty': ('anchor3d', 30, 22, [0, 25], {}, False, 407),
+}

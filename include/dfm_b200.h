@@ -692,6 +692,70 @@ int dfm_box_post_debug_tensor(dfm_box_post_t* h, const char* name, int* d_out, l
 int dfm_op_rotated_iou(const float* d_a, const float* d_b, int n, float* d_iou, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * Training losses of Anchor3DHead and LIGAAnchor3DHead (one feature level) for `batch` samples
+ * per call: MaxIoUAssigner on the nearest-BEV IoU (one assigner per anchor size), PseudoSampler,
+ * DeltaXYZWLHRBBoxCoder targets and direction targets, then the sigmoid focal loss, SmoothL1
+ * (with the sin difference on the yaw channel when diff_rad_by_sin), the direction softmax
+ * cross-entropy and, for LIGA with loss_iou, 1 - IoU3D of the decoded positives.  Anchor index
+ * (y * nx + x) * A + s * num_rotations + r, A = num_sizes * num_rotations; class channel
+ * j * num_classes + c, box channel j * 7 + k, direction channel j * 2 + k (NCHW).  No host
+ * synchronisation inside forward or finish; sums run in a fixed order, so repeated calls are
+ * bitwise equal.  Create fails with DFM_ERR_INVALID on more than 16 classes or 8 sizes.
+ * ---------------------------------------------------------------------------------- */
+typedef struct dfm_anchor_loss dfm_anchor_loss_t;
+typedef struct dfm_anchor_loss_desc {
+  int num_classes;              /* C sigmoid classes                                          */
+  int num_sizes;                /* anchor sizes, one assigner each                            */
+  int num_rotations;            /* rotations per size                                         */
+  int ny, nx, batch;            /* feature map and samples per call                           */
+  int assign_per_class;         /* 1: size s sees only GT of label s; 0: every GT             */
+  int diff_rad_by_sin;          /* 1: yaw channel as sin(p)cos(t) against cos(p)sin(t)        */
+  int use_direction_classifier; /* 1: direction loss                                          */
+  int with_iou;                 /* 1: 1 - IoU3D term (LIGA loss_iou)                          */
+  int liga;                     /* normalisers: 0 Anchor3DHead, 1 LIGAAnchor3DHead             */
+  float pos_iou_thr[8];         /* per assigner                                               */
+  float neg_iou_thr[8];
+  float min_pos_iou[8];
+  float pos_weight;             /* train_cfg.pos_weight (<= 0: 1)                              */
+  float gamma, alpha;           /* FocalLoss                                                  */
+  float beta;                   /* SmoothL1Loss                                               */
+  float loss_weight[4];         /* cls, bbox, dir, iou                                        */
+  float dir_offset, dir_limit_offset;
+  float normalizer_clamp_value; /* LIGA                                                       */
+} dfm_anchor_loss_desc_t;
+/* h_anchors: host [ny * nx * A][7] fp32, copied at create. */
+int dfm_anchor_loss_create(const dfm_anchor_loss_desc_t* desc, const float* h_anchors,
+                           dfm_anchor_loss_t** out);
+int dfm_anchor_loss_destroy(dfm_anchor_loss_t* h);
+/* d_cls [batch][A * C][ny][nx], d_bbox [batch][A * 7][ny][nx], d_dir [batch][A * 2][ny][nx];
+ * GT packed: d_gt_boxes [G][7] LiDAR boxes, d_gt_labels [G] int32 in 0..C-1, d_gt_off /
+ * h_gt_off [batch + 1] on the device and the host (at most 1024 boxes per sample).  Writes the
+ * gradients of the unnormalised, unweighted loss sums into each non-null d_grad_* (same layouts
+ * as the inputs; d_grad_iou is the IoU term's gradient with respect to d_bbox, only with
+ * with_iou) and d_norm [1] = sum over samples of max(positives, 1).  A GT label outside
+ * 0..C-1 is detected on the device and makes every loss of the next finish NaN.  Where a decoded
+ * target value is NaN the IoU term uses the prediction's value instead (iou3d_loss); its
+ * gradient then flows through the prediction's side of the IoU only, not also through the
+ * substituted target value as the reference's autograd does.  Such targets come only from
+ * degenerate GT (a size <= 0 or a non-finite value). */
+int dfm_anchor_loss_forward(dfm_anchor_loss_t* h, const float* d_cls, const float* d_bbox,
+                            const float* d_dir, const float* d_gt_boxes, const int* d_gt_labels,
+                            const int* d_gt_off, const int* h_gt_off, float* d_grad_cls,
+                            float* d_grad_bbox, float* d_grad_dir, float* d_grad_iou,
+                            float* d_norm, void* stream);
+/* From the last forward and d_avg [1] (the normaliser: d_norm, or its all-reduced mean for
+ * LIGA): d_losses [4] (cls, bbox, dir, iou) and d_scales [4], the factor each stored gradient
+ * takes to become that of its loss. */
+int dfm_anchor_loss_finish(dfm_anchor_loss_t* h, const float* d_avg, float* d_losses,
+                           float* d_scales, void* stream);
+/* Test hook, from the last forward, [batch][N] per anchor: "assigned_gt" int32 (-1 ignored,
+ * 0 negative, g + 1 for the sample's GT g), "labels" int32 (C for negatives and ignored),
+ * "label_weights" fp32, "dir_targets" int32, "bbox_targets" fp32 [batch][N][7].
+ * DFM_ERR_STATE before a forward, DFM_ERR_INVALID on an unknown name or wrong element count. */
+int dfm_anchor_loss_debug_tensor(dfm_anchor_loss_t* h, const char* name, void* d_out,
+                                 long long numel, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * KITTI evaluation (mmdet3d kitti_utils/eval.py: eval_class of every requested metric) of N
  * frames of ground truth and detections in CSR form.  Per box, fp64:
  *   gt [num_gt][14]: bbox[4] alpha location[3] dimensions[3] rotation_y occluded truncated
