@@ -63,6 +63,8 @@ SYMBOLS = (
     'dfm_op_let_iou', 'dfm_kitti_eval_set_overlap_limit', 'dfm_kitti_eval_workspace',
     'dfm_waymo_kitti_convert', 'dfm_anchor_loss_create', 'dfm_anchor_loss_destroy',
     'dfm_anchor_loss_forward', 'dfm_anchor_loss_finish', 'dfm_anchor_loss_debug_tensor',
+    'dfm_depth_loss_create', 'dfm_depth_loss_destroy', 'dfm_depth_loss_workspace',
+    'dfm_depth_loss_forward', 'dfm_depth_loss_debug_tensor',
 )
 
 DFM_IMAGE_PREP_CROP, DFM_IMAGE_PREP_RESCALE = 0, 1
@@ -164,6 +166,15 @@ class AnchorLossDesc(ctypes.Structure):
                [('loss_weight', c_float * 4)] + \
                [(n, c_float) for n in ('dir_offset', 'dir_limit_offset',
                                        'normalizer_clamp_value')]
+
+
+class DepthLossDesc(ctypes.Structure):
+    """``dfm_depth_loss_desc_t``."""
+    _fields_ = [(n, c_int) for n in ('num_images', 'num_planes', 'height', 'width', 'factor',
+                                     'dense')] + \
+               [(n, c_float) for n in ('min_depth', 'max_depth', 'alpha', 'gamma', 'fg_weight',
+                                       'bg_weight')] + \
+               [('balanced', c_int), ('loss_weight', c_float)]
 
 
 class ImagePrepDesc(ctypes.Structure):
@@ -297,6 +308,11 @@ def lib():
     L.dfm_anchor_loss_forward.argtypes = [vp] * 14
     L.dfm_anchor_loss_finish.argtypes = [vp] * 5
     L.dfm_anchor_loss_debug_tensor.argtypes = [vp, c_char_p, vp, c_longlong, vp]
+    L.dfm_depth_loss_create.argtypes = [POINTER(DepthLossDesc), POINTER(vp)]
+    L.dfm_depth_loss_destroy.argtypes = [vp]
+    L.dfm_depth_loss_workspace.argtypes = [vp, POINTER(c_longlong)]
+    L.dfm_depth_loss_forward.argtypes = [vp] * 10
+    L.dfm_depth_loss_debug_tensor.argtypes = [vp, c_char_p, vp, c_longlong, vp]
     L.dfm_voxel_sample.argtypes = [POINTER(VoxelSampleDesc), vp, vp, POINTER(c_double), vp, vp]
     L.dfm_kitti_eval_create.argtypes = [POINTER(KittiEvalDesc), POINTER(vp)]
     L.dfm_kitti_eval_destroy.argtypes = [vp]

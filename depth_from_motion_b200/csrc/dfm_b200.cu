@@ -29,6 +29,7 @@
 #include "resnet101_kernels.cuh"
 #include "box_post_kernels.cuh"
 #include "anchor_loss_kernels.cuh"
+#include "depth_loss_kernels.cuh"
 #include "image_prep_kernels.cuh"
 #include "view_cache_kernels.cuh"
 #include "kitti_eval_kernels.cuh"
@@ -1600,6 +1601,7 @@ int dfm_depth_head_forward(const float* d_cost, const float* d_depth_samples, in
 #include "resnet101_api.inc"
 #include "box_post_api.inc"
 #include "anchor_loss_api.inc"
+#include "depth_loss_api.inc"
 #include "image_prep_api.inc"
 #include "view_cache_api.inc"
 #include "kitti_eval_api.inc"

@@ -174,6 +174,29 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
+// ATen's trilinear align_corners arithmetic (area_pixel_compute_scale / _source_index, then the
+// truncated index and its lambda), shared by DepthHead.forward and the dense depth loss so both
+// read the same upsampled volume.  Scale of an axis of n_in samples stretched over n_out.
+__host__ __device__ inline float ac_scale(int n_in, int n_out) {
+  return n_out > 1 ? (float)(n_in - 1) / (n_out - 1) : 0.f;
+}
+// Depth bin k: low-res plane z0 and the weights of z0 and z0 + 1 (the last plane pairs with itself).
+__device__ __forceinline__ void ac_bin(float sz, int k, int D, int& z0, float& l0, float& l1) {
+  const float fz = sz * k;
+  z0 = min((int)fz, D - 1);
+  l1 = fz - z0;
+  l0 = 1.f - l1;
+}
+// Full-res row / column X: the two low-res taps (equal at the last one) and their weights.
+__device__ __forceinline__ void ac_tap(float s, int X, int n_in, int& i0, int& i1, float& w0,
+                                       float& w1) {
+  const float f = s * X;
+  i0 = (int)f;
+  i1 = i0 + (i0 < n_in - 1 ? 1 : 0);
+  w1 = f - i0;
+  w0 = 1.f - w1;
+}
+
 constexpr int DH4_PX = 128;   // output pixels along x per block
 __host__ __device__ inline int dh4_ncols(int f) { return DH4_PX / f + 3; }
 constexpr int DH4_ZS = 8;     // depth segments (warps) per block: they share the staged rows
@@ -196,26 +219,25 @@ depth_head4_kernel(const float* __restrict__ cost, const float* __restrict__ sam
   float* dh_rows = reinterpret_cast<float*>(tab_k0 + dh4_k0_ints(D));  // [D][nc]: y-blended rows
   __shared__ float red[3][DH_ZS][DH4_PX];
   const int tx = threadIdx.x, seg = threadIdx.y, tid = seg * 32 + tx;
-  const float sz = OD > 1 ? (float)(D - 1) / (OD - 1) : 0.f;
+  const float sz = ac_scale(D, OD);
   for (int z = tid; z <= D; z += 32 * DH_ZS) tab_k0[z] = OD;
   __syncthreads();
   for (int k = tid; k < OD; k += 32 * DH_ZS) {
-    const float fz = sz * k;       // ATen: area_pixel_compute_source_index, align_corners
-    const int z0 = min((int)fz, D - 1);
-    const float l1 = fz - z0;
-    tab[k] = make_float4(1.f - l1, l1, samples ? __ldg(samples + k) : 0.f, 0.f);
+    int z0;
+    float l0, l1;
+    ac_bin(sz, k, D, z0, l0, l1);
+    tab[k] = make_float4(l0, l1, samples ? __ldg(samples + k) : 0.f, 0.f);
     atomicMin(&tab_k0[z0], k);
   }
   const int Xb = blockIdx.x * DH4_PX;
   const int X0 = Xb + 4 * tx;                        // first of this thread's four pixels
   const bool live = X0 < OW;                          // OW % 4 == 0: all four or none
   const int Y = blockIdx.y;
-  const float sx = OW > 1 ? (float)(Wo - 1) / (OW - 1) : 0.f;
-  const float sy = OH > 1 ? (float)(Ho - 1) / (OH - 1) : 0.f;
-  const float fy = sy * Y;
-  const int y0 = (int)fy;
-  const int y1 = y0 + (y0 < Ho - 1 ? 1 : 0);
-  const float ly1 = fy - y0, ly0 = 1.f - ly1;
+  const float sx = ac_scale(Wo, OW);
+  const float sy = ac_scale(Ho, OH);
+  int y0, y1;
+  float ly0, ly1;
+  ac_tap(sy, Y, Ho, y0, y1, ly0, ly1);
   const long long plane = (long long)Ho * Wo;
   const long long oplane = (long long)OH * OW;
   const int nc = dh4_ncols(f);
@@ -231,11 +253,8 @@ depth_head4_kernel(const float* __restrict__ cost, const float* __restrict__ sam
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     const int X = min(X0 + j, OW - 1);
-    const float fx = sx * X;
-    const int x0 = (int)fx;
-    const int x1 = x0 + (x0 < Wo - 1 ? 1 : 0);
-    wx1[j] = fx - x0;
-    wx0[j] = 1.f - wx1[j];
+    int x0, x1;
+    ac_tap(sx, X, Wo, x0, x1, wx0[j], wx1[j]);
     c0[j] = x0 - xb;
     c1[j] = x1 - xb;
   }

@@ -465,11 +465,94 @@ def conv3d(x, weight, stride=(1, 1, 1), padding=(1, 1, 1), transposed=False,
     return y
 
 
+_DEPTH_LOSS_TYPES = ('ce', 'balanced_ce', 'focal', 'balanced_focal')
+
+
+class _DepthLossFn(torch.autograd.Function):
+    """The loss of one ``dfm_depth_loss_forward``.  Forward stores the gradient of the unweighted
+    loss sum when the volume requires grad; backward scales it by loss_weight^2 / count and
+    ``grad_output`` on the device."""
+
+    @staticmethod
+    def forward(ctx, vol, loss, samples, depth, fg, empty):
+        g = torch.empty_like(vol) if ctx.needs_input_grad[0] else None
+        out, scale = loss.forward(vol, samples, depth, fg, empty, g)
+        ctx.grad = g
+        ctx.save_for_backward(scale)
+        return out
+
+    @staticmethod
+    def backward(ctx, go):
+        scale, = ctx.saved_tensors
+        g = ctx.grad * (scale * go) if ctx.grad is not None else None
+        return g, None, None, None, None, None
+
+
+class _DepthLoss:
+    """``DepthHead.loss`` through ``dfm_depth_loss_*``: one handle per (input form, shape,
+    loss config, device), kept until the key changes."""
+
+    def __init__(self):
+        self.handle, self.key = None, None
+
+    def release(self):
+        if self.handle is not None:
+            capi.lib().dfm_depth_loss_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
+
+    def ensure(self, key, desc, dev):
+        if self.handle is None or key != self.key:
+            self.release()
+            hd = ctypes.c_void_p()
+            with torch.cuda.device(dev):
+                capi.check(capi.lib().dfm_depth_loss_create(ctypes.byref(desc), ctypes.byref(hd)),
+                           'dfm_depth_loss_create')
+            self.handle, self.key = hd, key
+            self.pixels = desc.num_images * (desc.height * desc.factor) * \
+                (desc.width * desc.factor)
+
+    def forward(self, vol, samples, depth, fg, empty, grad):
+        """Runs the handle; returns the 0-dim loss and gradient scale."""
+        dev = vol.device
+        loss = torch.empty((), device=dev)
+        scale = torch.empty((), device=dev)
+        with torch.cuda.device(dev):
+            capi.check(capi.lib().dfm_depth_loss_forward(
+                self.handle, _ptr(vol), _ptr(samples), _ptr(depth), _ptr(fg), _ptr(empty),
+                _ptr(grad), _ptr(loss), _ptr(scale), _stream()), 'dfm_depth_loss_forward')
+        return loss, scale
+
+    def workspace(self):
+        """Device bytes the handle owns."""
+        b = ctypes.c_longlong(0)
+        capi.check(capi.lib().dfm_depth_loss_workspace(self.handle, ctypes.byref(b)),
+                   'dfm_depth_loss_workspace')
+        return b.value
+
+    def debug_tensor(self, name):
+        """From the last call (tests only): 'pixel_loss' fp32 [B*N, fH, fW], the weighted
+        per-pixel term (0 outside the mask); 'count' int32 [1], the masked pixels."""
+        if self.handle is None:
+            raise RuntimeError('dfm_depth_loss_debug_tensor: no loss call has run')
+        n = 1 if name == 'count' else self.pixels
+        out = torch.empty(n, device='cuda',
+                          dtype=torch.int32 if name == 'count' else torch.float32)
+        capi.check(capi.lib().dfm_depth_loss_debug_tensor(self.handle, name.encode(), _ptr(out),
+                                                          out.numel(), _stream()),
+                   f'dfm_depth_loss_debug_tensor({name})')
+        return out
+
+
 @HEADS.register_module()
 class DepthHead(_CudaMirror):
-    """Drop-in for the reference ``DepthHead`` forward (depth_head.py:13-212).
-    ``loss`` is training-side PyTorch in the reference and is out of scope
-    (SURVEY.md section 8a row a5)."""
+    """Drop-in for the reference ``DepthHead`` (depth_head.py:13-212): ``forward`` and ``loss``
+    on CUDA."""
 
     def __init__(self, depth_cfg, in_channels=32, with_convs=True,
                  depth_loss=dict(type='ce', loss_weight=1.0),
@@ -490,6 +573,15 @@ class DepthHead(_CudaMirror):
         if self.with_convs:
             self.conv_depth = nn.Conv3d(in_channels, 1, 3, 1, 1, bias=False)
         self._samples_dev = None
+        self._depth_loss = _DepthLoss()
+
+    def _samples_on(self, dev):
+        """The injected ``depth_samples`` as fp32 on ``dev``, copied once per tensor."""
+        samples = self.depth_samples
+        if (self._samples_dev is None or self._samples_dev[0] is not samples
+                or self._samples_dev[1].device != dev):
+            self._samples_dev = (samples, samples.detach().to(dev, torch.float32).contiguous())
+        return self._samples_dev[1]
 
     def forward(self, stereo_features, return_volumes=True):
         """Returns (depth_volumes, depth_volumes_softmax, depth_preds) like
@@ -503,12 +595,7 @@ class DepthHead(_CudaMirror):
                 '(configs/dfm/dfm_r34_1x8_kitti-3d-3class.py:126 uses False)')
         b, n, d, h, w = stereo_features.shape
         f = self.downsample_factor
-        samples = self.depth_samples
-        if (self._samples_dev is None or self._samples_dev[0] is not samples
-                or self._samples_dev[1].device != stereo_features.device):
-            self._samples_dev = (samples, samples.detach().to(
-                stereo_features.device, torch.float32).contiguous())
-        sdev = self._samples_dev[1]
+        sdev = self._samples_on(stereo_features.device)
         assert sdev.numel() == f * d
         x = stereo_features.contiguous()
         dev = x.device
@@ -526,6 +613,83 @@ class DepthHead(_CudaMirror):
                 _ptr(sm[bi, ni]) if sm is not None else None,
                 _ptr(preds[bi, ni]), _stream()), 'dfm_depth_head_forward')
         return vol, sm, preds
+
+    def loss(self, depth_preds, depth_volumes, depth_img, depth_fgmask_img=None):
+        """``loss_dense_depth`` (depth_head.py:75-188) on CUDA (``dfm_depth_loss_*``): a 0-dim
+        device tensor, differentiable with respect to the volume.
+
+        ``depth_volumes`` is either a ``CostLogits`` whose ``.cost`` is DfMBackbone's
+        ``[B, N, D, H, W]`` logits -- the volume is then taken to be their x-downsample_factor
+        trilinear (align_corners) upsampling, read column by column under the masked pixels
+        without building it, and the gradient goes to ``.cost`` -- or the dense
+        ``[B*N, fD, fH, fW]`` volume the reference call site passes (its gradient is zero
+        outside the masked columns).  ``depth_img`` and ``depth_fgmask_img`` (any dtype,
+        non-zero = foreground) are ``[B*N, fH, fW]`` CUDA tensors.  Types ``ce``,
+        ``balanced_ce``, ``focal`` and ``balanced_focal``; the others raise
+        ``NotImplementedError``, a balanced type without ``depth_fgmask_img`` ``ValueError``.
+
+        Departures from the reference, all on the device with no host synchronisation:
+
+        * the loss is multiplied by ``loss_weight`` twice, as the reference does
+          (``self.loss_weight * loss_type_weight``, both ``depth_loss['loss_weight']``);
+        * with no masked pixel it is ``depth_preds.mean() * 0.0`` (NaN if ``depth_preds``
+          holds one), chosen on the device, with a zero gradient for the volume.  The
+          reference's empty branch computes that product but returns its accumulator, the
+          Python float ``0.``, and prints ``'no gt warning'``, which needs a host round trip;
+          the print is left out;
+        * the normaliser is the masked-pixel count over all ``B*N`` images, not all-reduced
+          (as in the reference);
+        * ``depth_preds`` is only checked for shape and read in the empty case; it gets no
+          gradient, as under the reference's autograd when a pixel is masked;
+        * sums over pixels run in fp64 (per-pixel softmax sums in fp32, as in the reference).
+        """
+        t = self.depth_loss_type
+        if t not in _DEPTH_LOSS_TYPES:
+            raise NotImplementedError(
+                f"DepthHead.loss: type '{t}' is not implemented on the CUDA path; it has ce, "
+                "balanced_ce, focal and balanced_focal (the shipped KITTI configs use "
+                "balanced_focal)")
+        balanced = t.startswith('balanced')
+        if balanced and depth_fgmask_img is None:
+            raise ValueError(f"DepthHead.loss: type '{t}' needs depth_fgmask_img")
+        logits = isinstance(depth_volumes, CostLogits)
+        vol = depth_volumes.cost if logits else depth_volumes
+        f = self.downsample_factor if logits else 1
+        if vol.dim() != (5 if logits else 4):
+            raise RuntimeError(f'DepthHead.loss: unexpected depth_volumes shape {tuple(vol.shape)}')
+        if logits:
+            d, h, w = vol.shape[2:]
+            n = vol.shape[0] * vol.shape[1]
+        else:
+            n, d, h, w = vol.shape
+        if len(self.depth_samples) != f * d:
+            raise RuntimeError(f'DepthHead.loss: {len(self.depth_samples)} depth_samples for '
+                               f'{f * d} depth bins')
+        full = (n, f * h, f * w)
+        for name, x in (('depth_preds', depth_preds), ('depth_img', depth_img),
+                        ('depth_fgmask_img', depth_fgmask_img)):
+            if x is not None and tuple(x.shape) != full:
+                raise RuntimeError(f'DepthHead.loss: {name} is {tuple(x.shape)}, expected {full}')
+        _check_cuda(vol, 'depth_volumes')
+        _check_cuda(depth_img, 'depth_img')
+        dev = vol.device
+        samples = self._samples_on(dev)
+        fg = None
+        if balanced:
+            if not depth_fgmask_img.is_cuda or depth_fgmask_img.device != dev:
+                raise RuntimeError('DepthHead.loss: depth_fgmask_img must be on the volume\'s '
+                                   'device')
+            fg = (depth_fgmask_img != 0).to(torch.uint8).contiguous()
+        cfg = self.depth_loss
+        focal = t.endswith('focal')
+        alpha, gamma = (float(cfg['alpha']), float(cfg['gamma'])) if focal else (1.0, 0.0)
+        fgw, bgw = (float(cfg['fg_weight']), float(cfg['bg_weight'])) if balanced else (1.0, 1.0)
+        desc = (n, d, h, w, f, int(not logits), float(self.min_depth), float(self.max_depth),
+                alpha, gamma, fgw, bgw, int(balanced), float(self.loss_weight))
+        self._depth_loss.ensure(desc + (str(dev),), capi.DepthLossDesc(*desc), dev)
+        empty = (depth_preds.detach().mean() * 0.0).to(dev, torch.float32)
+        return _DepthLossFn.apply(vol.contiguous(), self._depth_loss, samples,
+                                  depth_img.contiguous(), fg, empty)
 
 
 class _NeckBase(_HandleMirror):

@@ -670,3 +670,28 @@ ANCHOR_LOSS_GOLDEN_CASES = {
     'anchor3d_b2': ('anchor3d', 30, 22, [40, 30], dict(cross_class=True), False, 406),
     'anchor3d_b2_one_empty': ('anchor3d', 30, 22, [0, 25], {}, False, 407),
 }
+
+
+def make_depth_loss_case(seed, n, D, H, W, f=4, density=0.05, num_boxes=6):
+    """Inputs of ``DepthHead.loss`` for ``n`` images (B * N): smooth cost logits
+    ``[n, 1, D, H, W]`` in about +-20 (``smooth_field``), a sparse scan-line-like depth map
+    ``[n, fH, fW]`` and int32 foreground masks of box ids + 1 (0 = background), as the
+    training pipeline gives them.  Rows are LiDAR scan lines; about ``density`` of the pixels
+    carry a depth, drawn uniformly over [0, 65] so some fall outside the shipped [2, 59.6]
+    range.  The density is a synthetic choice, not a measured KITTI figure; 1.0 gives every
+    pixel a depth."""
+    rng = np.random.RandomState(seed)
+    fh, fw = f * H, f * W
+    cost = torch.stack([7.0 * smooth_field(rng, D, H, W, cell=4)[0] for _ in range(n)])[:, None]
+    row_p = min(1.0, 4.0 * density)
+    rows = rng.uniform(size=(n, fh, 1)) < row_p
+    cols = rng.uniform(size=(n, fh, fw)) < density / row_p
+    depth = rng.uniform(0.0, 65.0, size=(n, fh, fw)).astype(np.float32)
+    depth = np.where(rows & cols, depth, np.float32(0.0))
+    fg = np.zeros((n, fh, fw), np.int32)
+    for i in range(n):
+        for b in range(num_boxes):
+            y0, x0 = rng.randint(0, fh), rng.randint(0, fw)
+            bh, bw = rng.randint(1, max(2, fh // 3)), rng.randint(1, max(2, fw // 4))
+            fg[i, y0:y0 + bh, x0:x0 + bw] = b + 1
+    return cost.contiguous(), torch.from_numpy(depth), torch.from_numpy(fg)

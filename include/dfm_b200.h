@@ -756,6 +756,56 @@ int dfm_anchor_loss_debug_tensor(dfm_anchor_loss_t* h, const char* name, void* d
                                  long long numel, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * DepthHead.loss (dense_heads/depth_head.py:75-188) and its gradient for num_images = B * N
+ * images per call, types ce / balanced_ce / focal / balanced_focal: per masked pixel
+ *   w_pix * sum_k p_k * alpha * (1 - P_k)^gamma * (-log P_k),
+ * log P the fp32 log-softmax over the f * D bins, p_k = 1 - min(|s_k - gt| / (s_1 - s_0), 1),
+ * mask (gt > min_depth) & (gt < max_depth) in fp32 (NaN and inf excluded), w_pix fg_weight /
+ * bg_weight by the foreground mask for the balanced types and 1 otherwise.  The loss is
+ * loss_weight^2 * sum / (masked pixels of all images): the reference multiplies by its
+ * loss_weight and by a per-type weight that equals it.  The ce types are alpha = 1, gamma = 0.
+ * dense = 0: the bins are the x-factor trilinear (align_corners) upsampling of the low-res
+ * logits [num_images][num_planes][height][width], read column by column (DepthHead.forward's
+ * arithmetic); nothing of the size of the full-resolution volume is allocated.  dense = 1 (factor
+ * 1): the input is the full-resolution volume itself.  No host synchronisation inside forward;
+ * sums run in a fixed order (fp32 per pixel, fp64 across pixels), so repeated calls are bitwise
+ * equal.  Create fails with DFM_ERR_INVALID on an empty shape, fewer than two bins, factor != 1
+ * with dense, or num_images * num_planes > 65535.
+ * ---------------------------------------------------------------------------------- */
+typedef struct dfm_depth_loss dfm_depth_loss_t;
+typedef struct dfm_depth_loss_desc {
+  int num_images;               /* B * N                                                      */
+  int num_planes, height, width;/* D, H, W of the input                                       */
+  int factor;                   /* DepthHead.downsample_factor (1 with dense)                 */
+  int dense;                    /* 1: the input is the full-resolution volume                 */
+  float min_depth, max_depth;   /* depth_cfg                                                  */
+  float alpha, gamma;           /* focal factor; 1 and 0 for the ce types                     */
+  float fg_weight, bg_weight;   /* balanced types                                             */
+  int balanced;
+  float loss_weight;            /* depth_loss['loss_weight'], applied squared                 */
+} dfm_depth_loss_desc_t;
+int dfm_depth_loss_create(const dfm_depth_loss_desc_t* desc, dfm_depth_loss_t** out);
+int dfm_depth_loss_destroy(dfm_depth_loss_t* h);
+/* Device bytes the handle owns (per-pixel records and per-block partials). */
+int dfm_depth_loss_workspace(dfm_depth_loss_t* h, long long* bytes);
+/* d_volume: the logits or the dense volume; d_samples [f * D] fp32 bin depths; d_depth
+ * [num_images][f * height][f * width] fp32; d_fgmask the same shape, uint8 (non-zero =
+ * foreground), required by the balanced types and ignored by the others; d_empty [1] or NULL: the
+ * loss returned when no pixel is masked (0 when NULL).  d_grad, when not NULL, receives the
+ * gradient of the unweighted, unnormalised sum with respect to d_volume (same layout; zero
+ * outside the masked columns of a dense volume).  d_loss [1] the loss, d_scale [1] the factor the
+ * stored gradient takes to become the loss's (0 when no pixel is masked). */
+int dfm_depth_loss_forward(dfm_depth_loss_t* h, const float* d_volume, const float* d_samples,
+                           const float* d_depth, const unsigned char* d_fgmask,
+                           const float* d_empty, float* d_grad, float* d_loss, float* d_scale,
+                           void* stream);
+/* Test hook, from the last forward: "pixel_loss" fp32 [num_images][f * height][f * width], the
+ * weighted per-pixel term (0 outside the mask); "count" int32 [1], the masked pixels.
+ * DFM_ERR_STATE before a forward, DFM_ERR_INVALID on an unknown name or wrong element count. */
+int dfm_depth_loss_debug_tensor(dfm_depth_loss_t* h, const char* name, void* d_out,
+                                long long numel, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * KITTI evaluation (mmdet3d kitti_utils/eval.py: eval_class of every requested metric) of N
  * frames of ground truth and detections in CSR form.  Per box, fp64:
  *   gt [num_gt][14]: bbox[4] alpha location[3] dimensions[3] rotation_y occluded truncated
