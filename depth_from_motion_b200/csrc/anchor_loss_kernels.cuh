@@ -37,7 +37,7 @@ struct AnchorLossParams {
   int per_class, sin_diff, use_dir, with_iou;
   float pos_thr[AL_MAX_SIZES], neg_thr[AL_MAX_SIZES], min_pos[AL_MAX_SIZES];
   float pos_weight;              // train_cfg.pos_weight (<= 0: 1)
-  float gamma, alpha, beta;
+  float gamma, alpha, beta, inv_beta;
   float dir_offset, dir_limit_offset;
   // fp32 constants as PyTorch forms them from Python floats on CUDA
   float pi_f, inv_pi_f, quarter_pi_f, two_pi_f, inv_two_pi_f, inv_pi_bin_f;
@@ -416,32 +416,37 @@ __global__ void __launch_bounds__(AL_THREADS) al_loss_kernel(AnchorLossParams p)
 #pragma unroll
     for (int k = 0; k < 7; ++k) pr7[k] = pos ? __ldg(rg + (size_t)k * p.HW) : 0.f;
     const float* tg = p.targets + i * 7;
-    // SmoothL1 over the positives, channel 6 as sin(p)cos(t) against cos(p)sin(t)
+    // SmoothL1 over the positives, channel 6 as sin(p)cos(t) against cos(p)sin(t).  Forward and
+    // gradient round as mmdet's smooth_l1_loss and its autograd do in fp32 on CUDA: no FMA
+    // contraction (sin(p) cos(t) - cos(p) sin(t) is exactly 0 at p == t), / beta as
+    // * (1 / beta)_f, and the sin difference's two gradient paths summed last
     float gr[7];
 #pragma unroll
     for (int k = 0; k < 7; ++k) {
       gr[k] = 0.f;
       if (!pos) continue;
       const float t = tg[k];
-      float d, dd = 1.f;
-      if (k == 6 && p.sin_diff) {
-        float sp, cp, st, ct;
+      const bool sin6 = k == 6 && p.sin_diff;
+      float d, sp = 0.f, cp = 0.f, st = 0.f, ct = 0.f;
+      if (sin6) {
         sincosf(pr7[6], &sp, &cp);
         sincosf(t, &st, &ct);
-        d = sp * ct - cp * st;
-        dd = cp * ct + sp * st;
+        d = __fsub_rn(__fmul_rn(sp, ct), __fmul_rn(cp, st));
       } else {
-        d = pr7[k] - t;
+        d = __fsub_rn(pr7[k], t);
       }
       const float ad = fabsf(d);
       const float sg = d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f);
+      float g;
       if (ad < p.beta) {
-        acc[1] += (double)(0.5f * ad * ad / p.beta);
-        gr[k] = ad / p.beta * sg * dd;
+        acc[1] += (double)__fmul_rn(__fmul_rn(__fmul_rn(0.5f, ad), ad), p.inv_beta);
+        g = __fmul_rn(ad, p.inv_beta) * sg;
       } else {
-        acc[1] += (double)(ad - 0.5f * p.beta);
-        gr[k] = sg * dd;
+        acc[1] += (double)__fsub_rn(ad, __fmul_rn(0.5f, p.beta));
+        g = sg;
       }
+      gr[k] = sin6 ? __fadd_rn(__fmul_rn(__fmul_rn(g, ct), cp), __fmul_rn(__fmul_rn(g, st), sp))
+                   : g;
     }
     if (p.g_reg) {
       float* gp = p.g_reg + ((size_t)b * p.A * 7 + (size_t)a * 7) * p.HW + cell;

@@ -258,6 +258,19 @@ def dist_reduce_mean(t):
     return t
 
 
+def smooth_l1_terms(pb, pt, cfg):
+    """[P, 7] SmoothL1 terms of the positives' predictions ``pb`` against their targets ``pt``
+    (``add_sin_difference``, then mmdet's smooth_l1_loss before its reduction)."""
+    if cfg['diff_rad_by_sin']:
+        pe = torch.sin(pb[:, 6:7]) * torch.cos(pt[:, 6:7])
+        te = torch.cos(pb[:, 6:7]) * torch.sin(pt[:, 6:7])
+        pb = torch.cat([pb[:, :6], pe], dim=-1)
+        pt = torch.cat([pt[:, :6], te], dim=-1)
+    diff = torch.abs(pb - pt)
+    beta = cfg['beta']
+    return torch.where(diff < beta, 0.5 * diff * diff / beta, diff - 0.5 * beta)
+
+
 def losses(cls_score, bbox_pred, dir_pred, tg, anchors, cfg):
     """Loss dict of ``Anchor3DHead.loss`` (``cfg['liga']`` False) or of LIGA's ``loss_single``
     from per-sample targets ``tg``; the head outputs' dtype sets the arithmetic.  LIGA's IoU term
@@ -283,15 +296,7 @@ def losses(cls_score, bbox_pred, dir_pred, tg, anchors, cfg):
                      lw[:, None]).sum() / den_cls)
     box = bbox_pred.permute(0, 2, 3, 1).reshape(-1, 7)
     pos = torch.nonzero((labels >= 0) & (labels < C)).reshape(-1)
-    pb, pt = box[pos], btg[pos]
-    if cfg['diff_rad_by_sin']:
-        pe = torch.sin(pb[:, 6:7]) * torch.cos(pt[:, 6:7])
-        te = torch.cos(pb[:, 6:7]) * torch.sin(pt[:, 6:7])
-        pb = torch.cat([pb[:, :6], pe], dim=-1)
-        pt = torch.cat([pt[:, :6], te], dim=-1)
-    diff = torch.abs(pb - pt)
-    beta = cfg['beta']
-    sl1 = torch.where(diff < beta, 0.5 * diff * diff / beta, diff - 0.5 * beta)
+    sl1 = smooth_l1_terms(box[pos], btg[pos], cfg)
     l_bbox = w[1] * ((sl1 * torch.ones_like(sl1)).sum() / den)
     d = dir_pred.permute(0, 2, 3, 1).reshape(-1, 2)[pos]
     ce = torch.nn.functional.cross_entropy(d, dtg[pos], reduction='none')

@@ -177,15 +177,9 @@ def test_loss_matches_the_restatement(name):
     _check_against_restatement(name, *_run_case(name))
 
 
-def _check_against_restatement(name, head, liga, cfg, anchors, outs, gts, labels, metas):
-    got = head.loss([outs[0]], [outs[1]], [outs[2]], gts, labels, metas)
-    keys = ['loss_cls', 'loss_bbox', 'loss_dir'] + (['loss_iou'] if cfg['with_iou'] else [])
-    assert sorted(got) == sorted(keys)
-    total = sum(w * got[k][0] for w, k in zip(WEIGHTS, keys))
-    total.backward()
-    helper = head._anchor_loss
-    tg, ins, ref = _oracle(cfg, anchors, outs, gts, labels, torch.float64)
-    # targets: the fp32 restatement on the same device, exactly (bbox targets within 2 ulp)
+def _check_targets(helper, tg):
+    """The targets of the last call against the fp32 restatement on the same device, exactly
+    (bbox targets within 2 ulp)."""
     for k, dt in (('assigned_gt', torch.int32), ('labels', torch.int32),
                   ('label_weights', torch.float32), ('dir_targets', torch.int32)):
         want = torch.stack([t['assigned' if k == 'assigned_gt' else k] for t in tg]).to(dt)
@@ -194,6 +188,16 @@ def _check_against_restatement(name, head, liga, cfg, anchors, outs, gts, labels
     want = torch.stack([t['bbox_targets'] for t in tg])
     ulp = torch.abs(torch.nextafter(want, torch.full_like(want, np.inf)) - want)
     assert bool((torch.abs(bt - want) <= 2 * ulp).all())
+
+
+def _check_against_restatement(name, head, liga, cfg, anchors, outs, gts, labels, metas):
+    got = head.loss([outs[0]], [outs[1]], [outs[2]], gts, labels, metas)
+    keys = ['loss_cls', 'loss_bbox', 'loss_dir'] + (['loss_iou'] if cfg['with_iou'] else [])
+    assert sorted(got) == sorted(keys)
+    total = sum(w * got[k][0] for w, k in zip(WEIGHTS, keys))
+    total.backward()
+    tg, ins, ref = _oracle(cfg, anchors, outs, gts, labels, torch.float64)
+    _check_targets(head._anchor_loss, tg)
     # loss values against fp64
     for k in keys:
         assert got[k][0].item() == pytest.approx(ref[k].item(), rel=1e-6, abs=1e-12), k
