@@ -646,10 +646,8 @@ int make_warp_geom(const dfm_geometry_t* gm, int Hf, int Wf, int csf, int fsf, d
 // =====================================================================================
 struct Tower {
   ConvW dres0, dres1, c1, c2, c3, c4, c5, c6, p0;
-  DevBuf p1w;  // [27][32]
-  std::vector<float> p1w_host;  // same, host copy: kernel-parameter weights of logits_conv_kernel
+  DevBuf p1w;  // [27][32]: conv3d_c32_to_1_kernel (SIMT path)
   dfm::LogitsTcWeights p1q;     // same as a 32 x 32 (27 taps) bf16 hi/lo image: logits_tc_kernel
-  ConvW p1tc;  // the 32->1 logit conv zero-padded to 32 output channels for the tensor cores
   // z-invariance of the cur-frame half (SURVEY.md section 7): dres0 split into its cur- and
   // prev-channel halves (stereo); the cur contribution is computed on 5 replicated planes
   // and kept as 3 z-class planes (first / interior / last)
@@ -800,11 +798,6 @@ void tower_add_params(ParamTable& p, Tower& t, bool mono, int cin0, int cv) {
     std::vector<float> p((size_t)27 * cv);  // (1,cv,3,3,3) -> [tap][c]
     for (int c = 0; c < cv; ++c)
       for (int k = 0; k < 27; ++k) p[(size_t)k * cv + c] = h[(size_t)c * 27 + k];
-    std::vector<float> padded((size_t)cv * cv * 27, 0.f);  // (Cout=cv, Cin, 27), only co = 0 set
-    for (int c = 0; c < cv; ++c)
-      for (int k = 0; k < 27; ++k) padded[(size_t)c * 27 + k] = h[(size_t)c * 27 + k];
-    DFM_TRY(set_conv(t.p1tc, padded.data(), (long long)padded.size(), cv, cv, 0, dfm::TC_S1));
-    t.p1w_host = p;
     if (cv == 32 && !t.p1q.build(p.data())) return fail(DFM_ERR_CUDA, "logits weight upload failed");
     return upload(t.p1w, p.data(), p.size());
   });
@@ -951,36 +944,15 @@ int tower_forward(dfm_backbone* bb, Tower& t, bool mono, const dfm::WarpLoader& 
   // depth prediction module (dfm_backbone.py:118-128)
   g = geom_s(D, Ho, Wo, cv, cv, 1, 1, 1, 1, 1, 1);
   DFM_TRY(run_conv(src1(term(t.cur, nullptr, 0)), t.p0, t.p0b.p, g, impl, st, &t.gp0, zw_at(1)));
-  // 32 -> 1 logits conv (dfm_backbone.py:128): HBM-bound, CUDA-core kernel with the per-tap
-  // dot products staged in shared memory (tail_kernels.cuh).  DFM_LOGITS_TC=1 keeps the
-  // round-1 tensor-core variant (N = 96 MMA, 1/32 useful columns) for A/B runs; the fp32
-  // SIMT bring-up path keeps its own independent kernel.
-  // Default: logits_tc_kernel (logits_tc.cuh) -- the 27 per-tap dot products of every input
-  // position as one small wgmma GEMM, the stencil as a shared-memory gather.  DFM_LOGITS=simt
-  // selects the CUDA-core variant (tail_kernels.cuh), DFM_LOGITS=mma the round-1 N = 96 MMA.
-  static const char* logits_env = getenv("DFM_LOGITS");
-  static const bool logits_tc = getenv("DFM_LOGITS_TC") != nullptr ||
-                                (logits_env && std::string(logits_env) == "mma");
-  static const bool logits_simt = logits_env && std::string(logits_env) == "simt";
+  // 32 -> 1 logits conv (dfm_backbone.py:128), HBM-bound: logits_tc_kernel (logits_tc.cuh)
+  // computes the 27 per-tap dot products of every input position as one small wgmma GEMM and
+  // the stencil as a shared-memory gather; the fp32 SIMT path keeps its own kernel.
   const dfm::Src lsrc = src1(term(t.p0b, &t.gp0, 1));
-  if (impl != DFM_CONV_SIMT && !logits_tc && !logits_simt && cv == 32 && t.p1q.ready()) {
+  if (impl != DFM_CONV_SIMT) {
+    if (!t.p1q.ready()) return fail(DFM_ERR_STATE, "logits weights not uploaded");
     ProfScope ps(conv_class("cout1_logits_tc", g, "src"), 2.0 * V * cv * 27, st);
     if (!dfm::logits_tc_launch(lsrc, t.p1q, t.logit.p, D, Ho, Wo, st))
       return fail(DFM_ERR_CUDA, "logits_tc_kernel launch failed");
-    g_launches.fetch_add(1);
-    g_tc_launches.fetch_add(1);
-  } else if (impl != DFM_CONV_SIMT && !logits_tc && cv == 32 && t.p1w_host.size() == 27u * 32u) {
-    ProfScope ps(conv_class("cout1_logits", g, "src"), 2.0 * V * cv * 27, st);
-    if (!dfm::logits_conv_launch(lsrc, t.p1w_host.data(), t.logit.p, D, Ho, Wo, st))
-      return fail(DFM_ERR_CUDA, "logits_conv_kernel launch failed");
-    g_launches.fetch_add(1);
-  } else if (impl != DFM_CONV_SIMT && t.p1tc.tc.ready()) {
-    std::string err;
-    ProfScope ps(conv_class("conv_tc_cout1", g, "src"), 2.0 * V * cv * 27, st);
-    dfm::TcOpts o1;
-    o1.store1 = 1;
-    if (!dfm::tc_conv_src(lsrc, t.p1tc.tc, t.logit.p, nullptr, g, st, &err, o1))
-      return fail(DFM_ERR_CUDA, err);
     g_launches.fetch_add(1);
     g_tc_launches.fetch_add(1);
   } else {
@@ -1208,10 +1180,7 @@ int backbone_forward_impl(dfm_backbone_t* bb, const float* d_cur, const float* d
   const int HWo = bb->Ho * bb->Wo;
   const size_t gsm = dfm::gate_smem_bytes(bb->D);
   const size_t gsm4 = dfm::gate4_smem_bytes(bb->D);
-  static const char* gate_env = getenv("DFM_GATE");   // "v1" | "px1": A/B switches
-  const bool gate_v1 = getenv("DFM_GATE_V1") != nullptr || (gate_env && !strcmp(gate_env, "v1"));
-  if (bb->D <= 256 && HWo % 4 == 0 && gsm4 <= 220 * 1024 && !gate_v1 &&
-      !(gate_env && !strcmp(gate_env, "px1"))) {
+  if (bb->D <= 256 && HWo % 4 == 0 && gsm4 <= 220 * 1024) {
     // 4 pixels x 16 planes per thread, weights resident in shared memory, persistent blocks
     size_t& attr_sz = dfm::per_device<size_t, 11>();
     if (attr_sz < gsm4) {
@@ -1229,7 +1198,7 @@ int backbone_forward_impl(dfm_backbone_t* bb, const float* d_cur, const float* d
     dfm::gate_tile4_kernel<<<grid, 32 * ng, gsm4, st>>>(bb->st.logit.p, bb->mo.logit.p,
                                                        bb->waggT.p, bb->cost.p, bb->D, HWo,
                                                        ze_mono);
-  } else if (bb->D <= 256 && gsm <= 200 * 1024 && !gate_v1) {
+  } else if (bb->D <= 256 && gsm <= 200 * 1024) {
     // weights resident in shared memory, one persistent block per SM
     bool& attr_done = dfm::per_device<bool, 8>();
     size_t& attr_sz = dfm::per_device<size_t, 9>();
@@ -1265,14 +1234,14 @@ int backbone_forward_impl(dfm_backbone_t* bb, const float* d_cur, const float* d
 
 namespace {
 // DepthHead.forward kernel selection: four x pixels per thread (16-byte stores) whenever the
-// output width allows it, else the one-pixel-per-thread kernel
+// output width allows it, else the one-pixel-per-thread kernel (profiled as tag + "_px1")
 int launch_depth_head(const float* d_cost, const float* d_samples, int D, int Ho, int Wo,
                       int factor, float* d_volume, float* d_softmax, float* d_preds,
                       float2* d_norm, const char* tag, cudaStream_t st) {
-  ProfScope ps(tag, 0.0, st);
-  static const bool v1 = getenv("DFM_DEPTH_HEAD_V1") != nullptr;
   const size_t sm4 = dfm::dh4_smem_bytes(D, factor);
-  if ((Wo * factor) % 4 == 0 && sm4 <= 160 * 1024 && !v1) {
+  const bool four = (Wo * factor) % 4 == 0 && sm4 <= 160 * 1024;
+  ProfScope ps(four ? std::string(tag) : std::string(tag) + "_px1", 0.0, st);
+  if (four) {
     size_t& attr_sz = dfm::per_device<size_t, 10>();
     if (attr_sz < sm4) {
       CU_TRY(cudaFuncSetAttribute(dfm::depth_head4_kernel,

@@ -1,165 +1,16 @@
-// HBM-bound tail of the KITTI path, second generation (round 2):
-//   * logits_conv_kernel  -- the 32 -> 1 channel 3x3x3 conv of build_depth_pred_module
-//     (dfm_backbone.py:128) as a CUDA-core kernel.  The op reads V*32 floats and writes V
-//     (0.43 GB); on the tensor-core conv it would run as an N = 96 MMA with 1/32 useful
-//     columns.  Formulation: per INPUT voxel, the 27
-//     per-tap dot products q_t = <x, w_t> (864 FMAs whose weight operands come from the
-//     constant bank: the weights are a __grid_constant__ kernel parameter and every index is a
-//     compile-time constant), staged in shared memory; per OUTPUT voxel, out(o) = sum_t q_t(o + off_t) is 27 shared-memory reads.
-//     A block owns a 26 x 16 (x, y) output tile (28 x 18 halo = 504 positions, two per thread)
-//     and marches along z with three running accumulators per output pixel.
+// HBM-bound tail of the KITTI path, after the two logits convs:
 //   * depth_head4_kernel  -- DepthHead.forward with four consecutive x pixels per thread so the
 //     two [4D,4H,4W] volumes are written with 16-byte stores, 512 contiguous bytes per warp
-//     and depth bin.
-//   * gate_persistent_kernel -- the mono/stereo gate with the 1x1 conv weights resident in
-//     shared memory (transposed), one persistent block per SM.
+//     and depth bin.  Its align_corners helpers (ac_*) are shared with the dense depth loss.
+//   * gate_tile4_kernel, gate_persistent_kernel -- the mono/stereo gate with the 1x1 conv
+//     weights resident in shared memory (transposed), persistent blocks.  The shapes these
+//     do not fit take the one-pixel kernels of simt_kernels.cuh (depth_head_kernel,
+//     gate_kernel).
 #pragma once
 #include "conv_tc.cuh"
 #include "simt_kernels.cuh"
 
 namespace dfm {
-
-constexpr int LC_TX = 26, LC_TY = 16;                 // output tile
-constexpr int LC_PX = LC_TX + 2, LC_PY = LC_TY + 2;   // input halo
-constexpr int LC_NPOS = LC_PX * LC_PY;                // 504
-constexpr int LC_THREADS = 256;
-constexpr int LC_ZCHUNK = 8;                          // output planes per block
-
-struct LogitsConvParams {
-  float w[27 * 32];   // [tap = kz*9 + ky*3 + kx][channel]
-  Term t;             // single input term (GroupNorm affine + ReLU folded into the load)
-  int D, H, W;
-  int tiles_x, tiles_y, zchunks;
-};
-
-// Weights come from the constant bank; one position at a time.
-__global__ void __launch_bounds__(LC_THREADS)
-logits_conv_kernel(const __grid_constant__ LogitsConvParams p, float* __restrict__ out) {
-  extern __shared__ float lc_q[];   // [27][LC_NPOS]
-  float (*q)[LC_NPOS] = reinterpret_cast<float (*)[LC_NPOS]>(lc_q);
-  const int tid = threadIdx.x;
-  int b = blockIdx.x;
-  const int tx_i = b % p.tiles_x;
-  b /= p.tiles_x;
-  const int ty_i = b % p.tiles_y;
-  const int zc = b / p.tiles_y;
-  const int x0 = tx_i * LC_TX, y0 = ty_i * LC_TY;
-  const int z_lo = zc * LC_ZCHUNK, z_hi = min(p.D, z_lo + LC_ZCHUNK);
-  const long long plane = (long long)p.H * p.W;
-
-  // per-channel affine of the input term, in registers (32 + 32)
-  float sc[32], sh[32];
-#pragma unroll
-  for (int c = 0; c < 32; ++c) {
-    sc[c] = p.t.scale ? __ldg(p.t.scale + c) : 1.f;
-    sh[c] = p.t.scale ? __ldg(p.t.shift + c) : 0.f;
-  }
-  // the (up to) two output pixels of this thread: tile-linear indices tid and tid + 256
-  int oy[2], ox[2];
-  bool olive[2];
-#pragma unroll
-  for (int k = 0; k < 2; ++k) {
-    const int i = tid + k * LC_THREADS;
-    oy[k] = i / LC_TX;
-    ox[k] = i % LC_TX;
-    olive[k] = i < LC_TX * LC_TY && y0 + oy[k] < p.H && x0 + ox[k] < p.W;
-  }
-  float accA[2] = {0.f, 0.f}, accB[2] = {0.f, 0.f};  // output planes zi-1 and zi
-
-  for (int zi = max(z_lo - 1, 0); zi <= min(z_hi, p.D - 1); ++zi) {
-    // ---- phase 1: q_t of this input plane's halo positions ----
-#pragma unroll 1
-    for (int k = 0; k < 2; ++k) {
-      const int pos = tid + k * LC_THREADS;
-      if (pos >= LC_NPOS) break;
-      const int py = pos / LC_PX, px = pos % LC_PX;
-      const int gy = y0 - 1 + py, gx = x0 - 1 + px;
-      if (gy < 0 || gy >= p.H || gx < 0 || gx >= p.W) {
-#pragma unroll
-        for (int t = 0; t < 27; ++t) q[t][pos] = 0.f;
-        continue;
-      }
-      const float4* src = reinterpret_cast<const float4*>(
-          p.t.x + ((long long)term_plane(p.t, zi) * plane + (long long)gy * p.W + gx) * 32);
-      float x[32];
-#pragma unroll
-      for (int v = 0; v < 8; ++v) {
-        const float4 a = __ldg(src + v);
-        x[4 * v] = a.x; x[4 * v + 1] = a.y; x[4 * v + 2] = a.z; x[4 * v + 3] = a.w;
-      }
-#pragma unroll
-      for (int c = 0; c < 32; ++c) {
-        x[c] = fmaf(x[c], sc[c], sh[c]);
-        if (p.t.relu) x[c] = fmaxf(x[c], 0.f);
-      }
-#pragma unroll
-      for (int t = 0; t < 27; ++t) {
-        float a0 = 0.f, a1 = 0.f;   // two chains per tap
-#pragma unroll
-        for (int c = 0; c < 32; c += 2) {
-          a0 = fmaf(x[c], p.w[t * 32 + c], a0);
-          a1 = fmaf(x[c + 1], p.w[t * 32 + c + 1], a1);
-        }
-        q[t][pos] = a0 + a1;
-      }
-    }
-    __syncthreads();
-    // ---- phase 2: gather.  Input plane zi feeds output planes zi-1 (kz = 2), zi (kz = 1)
-    // and zi+1 (kz = 0); out(zi-1) is complete after this plane.
-#pragma unroll
-    for (int k = 0; k < 2; ++k) {
-      if (!olive[k]) continue;
-      float s0 = 0.f, s1 = 0.f, s2 = 0.f;
-#pragma unroll
-      for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-        for (int kx = 0; kx < 3; ++kx) {
-          const int pos = (oy[k] + ky) * LC_PX + ox[k] + kx;
-          s0 += q[0 * 9 + ky * 3 + kx][pos];
-          s1 += q[1 * 9 + ky * 3 + kx][pos];
-          s2 += q[2 * 9 + ky * 3 + kx][pos];
-        }
-      const int zo = zi - 1;
-      if (zo >= z_lo && zo < z_hi)
-        out[(long long)zo * plane + (long long)(y0 + oy[k]) * p.W + x0 + ox[k]] = accA[k] + s2;
-      accA[k] = accB[k] + s1;
-      accB[k] = s0;
-    }
-    __syncthreads();
-  }
-  // the last output plane of the chunk when it is the volume's last plane (no input plane
-  // z_hi exists to flush it)
-  if (z_hi == p.D) {
-#pragma unroll
-    for (int k = 0; k < 2; ++k)
-      if (olive[k])
-        out[(long long)(p.D - 1) * plane + (long long)(y0 + oy[k]) * p.W + x0 + ox[k]] = accA[k];
-  }
-}
-
-inline bool logits_conv_launch(const Src& s, const float* h_w /*[27][32] host*/, float* out,
-                               int D, int H, int W, cudaStream_t st) {
-  if (s.n != 1 || s.outer_relu) return false;
-  LogitsConvParams p;
-  memcpy(p.w, h_w, sizeof(p.w));
-  p.t = s.t[0];
-  p.D = D; p.H = H; p.W = W;
-  p.tiles_x = (W + LC_TX - 1) / LC_TX;
-  p.tiles_y = (H + LC_TY - 1) / LC_TY;
-  p.zchunks = (D + LC_ZCHUNK - 1) / LC_ZCHUNK;
-  const long long blocks = (long long)p.tiles_x * p.tiles_y * p.zchunks;
-  if (blocks > 0x7fffffffLL) return false;
-  constexpr size_t smem = sizeof(float) * 27 * LC_NPOS;
-  bool& attr_done = per_device<bool, 7>();
-  if (!attr_done) {
-    if (cudaFuncSetAttribute(logits_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)smem) != cudaSuccess)
-      return false;
-    attr_done = true;
-  }
-  logits_conv_kernel<<<(unsigned)blocks, LC_THREADS, smem, st>>>(p, out);
-  return cudaGetLastError() == cudaSuccess;
-}
 
 // ---------------------------------------------------------------------------------
 // DepthHead.forward, four x pixels per thread (requires (Wo * f) % 4 == 0).

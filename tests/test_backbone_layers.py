@@ -61,6 +61,10 @@ CASES = {
     # the shipped KITTI config: D % 16 == 8 in the logits chunks and the gate at full width
     'kitti_320x1280_d72': dict(seed=21, h=320, w=1280, d=72, crop=(0, 55), ori=(375, 1242, 3),
                                slabs=True),
+    # the gate's fallbacks, chosen by D alone (Ho * Wo is always a multiple of 16): at D = 120
+    # gate_tile4's shared memory no longer fits, at D = 148 gate_persistent's neither
+    'gate_persistent_48x80_d120': dict(seed=43, h=48, w=80, d=120),
+    'gate_v1_48x80_d148': dict(seed=44, h=48, w=80, d=148),
 }
 # the cases the CPU bound-separation test evaluates with the oracle (the large ones are
 # checked on the GPU, which also asserts the separation on the GPU's own layer inputs)
@@ -284,6 +288,10 @@ TC_PREFIXES = ('conv_tc', 'cout1_logits', 'gate')
 BENCH_CLASSES = ('conv_tc<32->32,s1,warp>', 'conv_tc<32->32,s1,src>', 'conv_tc_ks<32->64,s2,tma>',
                  'conv_tc_ks<64->64,s2,src>', 'conv_tck<64->64,s1,src>', 'conv_tc<64->64,T,src>',
                  'conv_tc<64->32,T,src>', 'cout1_logits_tc<32->32,s1,src>', 'gate_tile4')
+# the classes a case must have launched and compared
+CASE_CLASSES = {'bench_384x1248_d112': BENCH_CLASSES,
+                'gate_persistent_48x80_d120': ('gate_persistent',),
+                'gate_v1_48x80_d148': ('gate_v1',)}
 
 
 def _shell_mask(zidx, dz, h, w, tiles):
@@ -500,9 +508,8 @@ def run_gpu_case(name):
 def test_layers_vs_fp64(name):
     _, failures, checked = run_gpu_case(name)
     assert not failures, failures
-    if name == 'bench_384x1248_d112':
-        missing = [c for c in BENCH_CLASSES if c not in checked]
-        assert not missing, (missing, sorted(checked))
+    missing = [c for c in CASE_CLASSES.get(name, ()) if c not in checked]
+    assert not missing, (missing, sorted(checked))
 
 
 @pytest.mark.gpu
@@ -544,10 +551,6 @@ AB_ARMS = [
     # the K-outer kernel is the default for conv2 / conv4 only where D-windows x tiles fill the
     # SMs: at 64 x 112 it never runs, so this arm runs at the shipped 320 x 1280, D = 72 shape
     ({'DFM_NO_NTK': '1'}, 'kitti_320x1280_d72', 'conv_tc<64->64,s1,src>@36x40x160', 'conv_tck'),
-    ({'DFM_LOGITS': 'simt'}, 'aug_64x112_d68', 'cout1_logits<', 'cout1_logits_tc'),
-    ({'DFM_LOGITS': 'mma'}, 'aug_64x112_d68', 'conv_tc_cout1<', 'cout1_logits_tc'),
-    ({'DFM_GATE': 'px1'}, 'aug_64x112_d68', 'gate_persistent', 'gate_tile4'),
-    ({'DFM_GATE': 'v1'}, 'aug_64x112_d68', 'gate_v1', 'gate_tile4'),
 ]
 
 
@@ -573,12 +576,13 @@ def test_ab_arm_layers(arm):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('wo,factor', [(20, 4), (19, 3)])
-def test_depth_head_vs_oracle(wo, factor):
+@pytest.mark.parametrize('wo,factor,tag', [(20, 4, 'depth_head'), (19, 3, 'depth_head_px1')],
+                         ids=['20-4', '19-3'])
+def test_depth_head_vs_oracle(wo, factor, tag):
     """dfm_depth_head_forward against oracle.depth_head_forward in fp64, at the default x4
-    upsampling and at an output width (19 x 3 = 57) that is not a multiple of 4, where even the
-    default build takes the one-pixel-per-thread kernel."""
-    from depth_from_motion_b200 import modules
+    upsampling (four pixels per thread) and at an output width (19 x 3 = 57) that is not a
+    multiple of 4, which takes the one-pixel-per-thread kernel."""
+    from depth_from_motion_b200 import capi, modules
     from tests.util import rel_err
     d, ho = 12, 12
     g = torch.Generator().manual_seed(7)
@@ -589,20 +593,18 @@ def test_depth_head_vs_oracle(wo, factor):
         with_convs=False, num_views=1, depth_loss=dict(type='ce', loss_weight=1.0))
     head.depth_samples = O.depth_samples(cfg)
     head.downsample_factor = factor
-    vol, sm, preds = head(cost.cuda())
-    rvol, rsm, rpreds = O.depth_head_forward(cost.double(), O.depth_samples(cfg).double(),
+    cost = cost.cuda()
+    capi.profile_enable(True)
+    capi.profile_report()
+    try:
+        vol, sm, preds = head(cost)
+        torch.cuda.synchronize()
+        report = capi.profile_report()
+    finally:
+        capi.profile_enable(False)
+    assert [k for k in report if k.startswith('depth_head')] == [tag], report
+    rvol, rsm, rpreds = O.depth_head_forward(cost.cpu().double(), O.depth_samples(cfg).double(),
                                              factor)
     assert rel_err(vol, rvol) < 1e-5
     assert rel_err(sm, rsm) < 1e-5
     assert rel_err(preds, rpreds) < 1e-5
-
-
-@pytest.mark.gpu
-def test_depth_head_v1_arm():
-    """DFM_DEPTH_HEAD_V1 (the one-pixel-per-thread kernel) in its own interpreter."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, DFM_DEPTH_HEAD_V1='1')
-    r = subprocess.run([sys.executable, '-m', 'pytest', os.path.abspath(__file__), '-q',
-                        '-m', 'gpu', '-p', 'no:cacheprovider', '-k', 'test_depth_head_vs_oracle'],
-                       cwd=root, env=env, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, (r.stdout + r.stderr)[-4000:]
