@@ -65,6 +65,8 @@ SYMBOLS = (
     'dfm_anchor_loss_forward', 'dfm_anchor_loss_finish', 'dfm_anchor_loss_debug_tensor',
     'dfm_depth_loss_create', 'dfm_depth_loss_destroy', 'dfm_depth_loss_workspace',
     'dfm_depth_loss_forward', 'dfm_depth_loss_debug_tensor',
+    'dfm_atss_loss_create', 'dfm_atss_loss_destroy', 'dfm_atss_loss_forward',
+    'dfm_atss_loss_finish', 'dfm_atss_loss_debug_tensor',
 )
 
 DFM_IMAGE_PREP_CROP, DFM_IMAGE_PREP_RESCALE = 0, 1
@@ -175,6 +177,15 @@ class DepthLossDesc(ctypes.Structure):
                [(n, c_float) for n in ('min_depth', 'max_depth', 'alpha', 'gamma', 'fg_weight',
                                        'bg_weight')] + \
                [('balanced', c_int), ('loss_weight', c_float)]
+
+
+class AtssLossDesc(ctypes.Structure):
+    """``dfm_atss_loss_desc_t``."""
+    _fields_ = [('num_classes', c_int), ('num_levels', c_int), ('strides', c_int * 8),
+                ('feat_h', c_int * 8), ('feat_w', c_int * 8), ('batch', c_int), ('topk', c_int),
+                ('octave_base_scale', c_float), ('target_stds', c_float * 4),
+                ('wh_ratio_clip', c_float), ('giou_eps', c_float), ('gamma', c_float),
+                ('alpha', c_float), ('loss_weight', c_float * 3)]
 
 
 class ImagePrepDesc(ctypes.Structure):
@@ -313,6 +324,11 @@ def lib():
     L.dfm_depth_loss_workspace.argtypes = [vp, POINTER(c_longlong)]
     L.dfm_depth_loss_forward.argtypes = [vp] * 10
     L.dfm_depth_loss_debug_tensor.argtypes = [vp, c_char_p, vp, c_longlong, vp]
+    L.dfm_atss_loss_create.argtypes = [POINTER(AtssLossDesc), POINTER(vp)]
+    L.dfm_atss_loss_destroy.argtypes = [vp]
+    L.dfm_atss_loss_forward.argtypes = [vp] * 14
+    L.dfm_atss_loss_finish.argtypes = [vp] * 5
+    L.dfm_atss_loss_debug_tensor.argtypes = [vp, c_char_p, vp, c_longlong, vp]
     L.dfm_voxel_sample.argtypes = [POINTER(VoxelSampleDesc), vp, vp, POINTER(c_double), vp, vp]
     L.dfm_kitti_eval_create.argtypes = [POINTER(KittiEvalDesc), POINTER(vp)]
     L.dfm_kitti_eval_destroy.argtypes = [vp]

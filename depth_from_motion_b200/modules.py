@@ -1814,6 +1814,334 @@ class Anchor3DHead(_HandleMirror):
     loss.__doc__ = _LOSS_DOC.format(liga='', iou='')
 
 
+def _atss_loss_config(head):
+    """The settings ``LIGAATSSHead.loss`` reads from its config, with the refusals of what no
+    shipped config uses."""
+    g, coder, cfg = head.anchor_generator, head.bbox_coder, head.train_cfg or {}
+    asg = dict(cfg.get('assigner') or {})
+    lc, lb, lz = head.loss_cls_cfg, head.loss_bbox_cfg, head.loss_centerness_cfg
+    if head.reg_class_agnostic:
+        raise NotImplementedError('LIGAATSSHead.loss: reg_class_agnostic=True')
+    if head.num_extra_reg_channel or head.seperate_extra_reg_branch:
+        raise NotImplementedError('LIGAATSSHead.loss: extra regression channels')
+    if head.reg_avg_factor != 'default':
+        raise NotImplementedError(f'LIGAATSSHead.loss: reg_avg_factor={head.reg_avg_factor!r}')
+    if head.num_anchors != 1 or g.get('center_offset', 0.0) != 0.0 or 'scales' in g or \
+            g.get('type', 'AnchorGenerator') != 'AnchorGenerator':
+        raise NotImplementedError('LIGAATSSHead.loss: one anchor per location, from '
+                                  'octave_base_scale, centre offset 0')
+    strides = list(g['strides'])
+    if not all(isinstance(s, int) and s > 0 for s in strides) or len(strides) > 8:
+        raise NotImplementedError('LIGAATSSHead.loss: up to 8 levels of integer strides')
+    if lc.get('type') != 'FocalLoss' or not lc.get('use_sigmoid', True) or \
+            lb.get('type') != 'GIoULoss' or lz.get('type') != 'CrossEntropyLoss' or \
+            not lz.get('use_sigmoid', False):
+        raise NotImplementedError('LIGAATSSHead.loss: sigmoid FocalLoss, GIoULoss and sigmoid '
+                                  'CrossEntropyLoss only')
+    if any(lo.get('reduction', 'mean') != 'mean' for lo in (lc, lb, lz)) or \
+            lz.get('class_weight') is not None or lc.get('activated', False):
+        raise NotImplementedError('LIGAATSSHead.loss: mean reduction without class weights')
+    if asg.get('type') != 'ATSS3DCenterAssigner' or asg.get('thresh_mode', 'meanstd') != 'meanstd' \
+            or not asg.get('append_3d_centers', True) or \
+            not cfg.get('append_3d_centers', True) or asg.get('ignore_iof_thr', -1) > 0:
+        raise NotImplementedError('LIGAATSSHead.loss: ATSS3DCenterAssigner with '
+                                  "thresh_mode='meanstd' and append_3d_centers=True only")
+    if asg.get('topk') != 9 or cfg.get('allowed_border', -1) >= 0 or cfg.get('pos_weight', -1) > 0:
+        raise NotImplementedError('LIGAATSSHead.loss: topk=9, allowed_border=-1 and pos_weight=-1 '
+                                  'only')
+    means = coder.get('target_means', [0.0] * 4)
+    stds = [float(x) for x in coder.get('target_stds', [1.0] * 4)]
+    if coder.get('type', 'DeltaXYWHBBoxCoder') != 'DeltaXYWHBBoxCoder' or any(means) or \
+            stds[0] != stds[1] or stds[2] != stds[3] or coder.get('add_ctr_clamp', False):
+        raise NotImplementedError('LIGAATSSHead.loss: DeltaXYWHBBoxCoder with means 0 and equal '
+                                  'x / y and w / h stds')
+    return dict(num_classes=head.num_classes, strides=strides,
+                octave_base_scale=float(g['octave_base_scale']), target_stds=stds,
+                wh_ratio_clip=16 / 1000, giou_eps=float(lb.get('eps', 1e-6)),
+                gamma=float(lc.get('gamma', 2.0)), alpha=float(lc.get('alpha', 0.25)),
+                loss_weight=[float(lc.get('loss_weight', 1.0)), float(lb.get('loss_weight', 1.0)),
+                             float(lz.get('loss_weight', 1.0))])
+
+
+def _ptr_table(ts):
+    """A host array of device pointers (NULL for None) as a ``void *``."""
+    arr = (ctypes.c_void_p * len(ts))(*[t.data_ptr() if t is not None else None for t in ts])
+    return arr, ctypes.cast(arr, ctypes.c_void_p)
+
+
+class _ATSSLossFn(torch.autograd.Function):
+    """The 3 x L loss values of one ``dfm_atss_loss_forward`` / ``_finish``.  Forward stores the
+    gradients of the per-level loss sums of the outputs that require grad; backward scales each
+    by its loss's normaliser, weight and ``grad_output``."""
+
+    @staticmethod
+    def forward(ctx, loss, *outs):
+        grads = [torch.empty_like(o) if ctx.needs_input_grad[1 + i] else None
+                 for i, o in enumerate(outs)]
+        scales = loss.forward(outs, grads)
+        ctx.grads = grads
+        ctx.save_for_backward(scales)
+        return loss.losses
+
+    @staticmethod
+    def backward(ctx, g):
+        scales, = ctx.saved_tensors
+        s = scales * g
+        return (None,) + tuple(gr * s[i] if gr is not None else None
+                               for i, gr in enumerate(ctx.grads))
+
+
+class _ATSSLoss:
+    """``LIGAATSSHead.loss`` through ``dfm_atss_loss_*``: one handle per (feature sizes, batch,
+    device, loss config), kept until the key changes."""
+
+    def __init__(self):
+        self.handle, self.key = None, None
+
+    def release(self):
+        if self.handle is not None:
+            capi.lib().dfm_atss_loss_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
+
+    def run(self, head, cls_scores, bbox_preds, centernesses, gt_bboxes, gt_labels, img_metas,
+            gt_bboxes_ignore):
+        cfg = _atss_loss_config(head)
+        if gt_bboxes_ignore is not None and any(g is not None and len(g) for g in
+                                                gt_bboxes_ignore):
+            raise NotImplementedError('LIGAATSSHead.loss: gt_bboxes_ignore is not implemented')
+        L, C, B = len(cfg['strides']), cfg['num_classes'], len(img_metas)
+        if not (len(cls_scores) == len(bbox_preds) == len(centernesses) == L):
+            raise RuntimeError(f'LIGAATSSHead.loss: {L} levels expected, got {len(cls_scores)}, '
+                               f'{len(bbox_preds)}, {len(centernesses)}')
+        if len(gt_bboxes) != B or len(gt_labels) != B:
+            raise RuntimeError(f'LIGAATSSHead.loss: {B} img_metas, {len(gt_bboxes)} gt_bboxes and '
+                               f'{len(gt_labels)} gt_labels')
+        feat = []
+        for lv, (c, b, z) in enumerate(zip(cls_scores, bbox_preds, centernesses)):
+            for name, t in (('cls_score', c), ('bbox_pred', b), ('centerness', z)):
+                _check_cuda(t, f'{name}[{lv}]')
+            h, w = c.shape[-2:]
+            if c.shape != (B, C, h, w) or b.shape != (B, 4 * C, h, w) or \
+                    z.shape != (B, 1, h, w) or c.device != cls_scores[0].device:
+                raise RuntimeError(f'LIGAATSSHead.loss: unexpected head output shapes at level '
+                                   f'{lv}: {tuple(c.shape)}, {tuple(b.shape)}, {tuple(z.shape)}')
+            feat.append((int(h), int(w)))
+        dev = cls_scores[0].device
+        boxes, labels, off = [], [], [0]
+        for gb, gl in zip(gt_bboxes, gt_labels):
+            if gb.dim() != 2 or gb.shape[1] != 6:
+                raise RuntimeError(f'LIGAATSSHead.loss: GT must be [M, 6] (2-D box and projected '
+                                   f'3-D centre), got {tuple(gb.shape)}')
+            if gl.shape != (gb.shape[0],):
+                raise RuntimeError('LIGAATSSHead.loss: every image needs one label per GT box')
+            # labels still on the host are checked here; on the device the kernels flag them
+            # and every loss comes out NaN (no host synchronisation on the CUDA path)
+            if not gl.is_cuda and gl.numel() and (int(gl.min()) < 0 or int(gl.max()) >= C):
+                raise ValueError(f'LIGAATSSHead.loss: GT labels must lie in 0..{C - 1}')
+            boxes.append(gb.to(dev, torch.float32))
+            labels.append(gl.to(dev, torch.int32))
+            off.append(off[-1] + gb.shape[0])
+        self.gt = torch.cat(boxes).contiguous()
+        self.gt_labels = torch.cat(labels).contiguous()
+        self.h_off = (ctypes.c_int * (B + 1))(*off)
+        self.d_off = torch.tensor(off, dtype=torch.int32).to(dev, non_blocking=True)
+        pads = [int(v) for m in img_metas for v in m['pad_shape'][:2]]
+        self.h_pad = (ctypes.c_int * (2 * B))(*pads)
+        key = (repr(sorted((k, repr(v)) for k, v in cfg.items())), tuple(feat), B, str(dev))
+        if self.handle is None or key != self.key:
+            self.release()
+            z8 = lambda v: (ctypes.c_int * 8)(*v)  # noqa: E731
+            desc = capi.AtssLossDesc(
+                C, L, z8(cfg['strides']), z8([f[0] for f in feat]), z8([f[1] for f in feat]), B,
+                9, cfg['octave_base_scale'], (ctypes.c_float * 4)(*cfg['target_stds']),
+                cfg['wh_ratio_clip'], cfg['giou_eps'], cfg['gamma'], cfg['alpha'],
+                (ctypes.c_float * 3)(*cfg['loss_weight']))
+            hd = ctypes.c_void_p()
+            with torch.cuda.device(dev):
+                capi.check(capi.lib().dfm_atss_loss_create(ctypes.byref(desc), ctypes.byref(hd)),
+                           'dfm_atss_loss_create')
+            self.handle, self.key, self.batch = hd, key, B
+            self.n = sum(h * w for h, w in feat)
+        self.levels = L
+        outs = [t.contiguous() for t in (*cls_scores, *bbox_preds, *centernesses)]
+        losses = _ATSSLossFn.apply(self, *outs)
+        return dict(loss_cls=[losses[i] for i in range(L)],
+                    loss_bbox=[losses[L + i] for i in range(L)],
+                    loss_centerness=[losses[2 * L + i] for i in range(L)])
+
+    def forward(self, outs, grads):
+        """Runs the handle; sets ``self.losses`` [3 L] and returns the gradient scales [3 L]."""
+        L = self.levels
+        lib = capi.lib()
+        dev = outs[0].device
+        tabs = [_ptr_table(outs[k * L:(k + 1) * L]) for k in range(3)]
+        gtabs = [_ptr_table(grads[k * L:(k + 1) * L])
+                 if any(g is not None for g in grads[k * L:(k + 1) * L]) else (None, None)
+                 for k in range(3)]
+        norm = torch.empty(2, device=dev)
+        with torch.cuda.device(dev):
+            capi.check(lib.dfm_atss_loss_forward(
+                self.handle, tabs[0][1], tabs[1][1], tabs[2][1], _ptr(self.gt),
+                _ptr(self.gt_labels), _ptr(self.d_off), ctypes.cast(self.h_off, ctypes.c_void_p),
+                ctypes.cast(self.h_pad, ctypes.c_void_p), gtabs[0][1], gtabs[1][1], gtabs[2][1],
+                _ptr(norm), _stream()), 'dfm_atss_loss_forward')
+            # num_total_pos and the centerness sum, all-reduced in one call
+            avg = _dist_reduce_mean(norm)
+            self.losses = torch.empty(3 * L, device=dev)
+            scales = torch.empty(3 * L, device=dev)
+            capi.check(lib.dfm_atss_loss_finish(self.handle, _ptr(avg), _ptr(self.losses),
+                                                _ptr(scales), _stream()),
+                       'dfm_atss_loss_finish')
+        return scales
+
+    def debug_tensor(self, name):
+        """Per-anchor target of the last call (tests only): 'assigned_gt', 'labels' int32
+        [batch, N]; 'label_weights', 'centerness_targets' fp32 [batch, N]; 'bbox_targets' fp32
+        [batch, N, 4]; 'thresholds' fp32 [G]."""
+        if self.handle is None:
+            raise RuntimeError('dfm_atss_loss_debug_tensor: no loss call has run')
+        shape = {'bbox_targets': (self.batch, self.n, 4),
+                 'thresholds': (self.gt.shape[0],)}.get(name, (self.batch, self.n))
+        dt = torch.int32 if name in ('assigned_gt', 'labels') else torch.float32
+        out = torch.empty(shape, device=self.gt.device, dtype=dt)
+        capi.check(capi.lib().dfm_atss_loss_debug_tensor(self.handle, name.encode(), _ptr(out),
+                                                         out.numel(), _stream()),
+                   f'dfm_atss_loss_debug_tensor({name})')
+        return out
+
+
+class _Scale(nn.Module):
+    """mmcv ``Scale``: a learnable scalar factor."""
+
+    def __init__(self, scale=1.0):
+        super().__init__()
+        self.scale = nn.Parameter(torch.tensor(scale, dtype=torch.float))
+
+    def forward(self, x):
+        return x * self.scale
+
+
+@HEADS.register_module()
+class LIGAATSSHead(nn.Module):
+    """DfM's 2-D auxiliary head (dense_heads/liga_atss_head.py, an mmdet ``ATSSHead``): the
+    reference constructor and ``state_dict`` keys, a plain differentiable PyTorch ``forward``
+    (the head is trained: ConvModule = 3 x 3 conv without bias, GroupNorm, ReLU; ``Scale`` and
+    ``.float()`` on ``bbox_pred``), and ``loss`` on CUDA (``dfm_atss_loss_*``).  Registered in
+    this package's ``HEADS`` only; ``DfM`` does not build it."""
+
+    def __init__(self, num_classes, in_channels, stacked_convs=4, conv_cfg=None,
+                 norm_cfg=dict(type='GN', num_groups=32, requires_grad=True),
+                 loss_centerness=dict(type='CrossEntropyLoss', use_sigmoid=True,
+                                      loss_weight=1.0),
+                 reg_class_agnostic=True, num_extra_reg_channel=0,
+                 seperate_extra_reg_branch=False, reg_avg_factor='default', feat_channels=256,
+                 anchor_generator=dict(type='AnchorGenerator', ratios=[1.0],
+                                       octave_base_scale=8, scales_per_octave=1,
+                                       strides=[8, 16, 32, 64, 128]),
+                 bbox_coder=dict(type='DeltaXYWHBBoxCoder', target_means=[.0, .0, .0, .0],
+                                 target_stds=[0.1, 0.1, 0.2, 0.2]),
+                 loss_cls=dict(type='FocalLoss', use_sigmoid=True, gamma=2.0, alpha=0.25,
+                               loss_weight=1.0),
+                 loss_bbox=dict(type='GIoULoss', loss_weight=2.0), train_cfg=None,
+                 test_cfg=None, init_cfg=None, **kwargs):
+        super().__init__()
+        assert reg_avg_factor in ('default', 'sum_centerness')
+        assert conv_cfg is None and norm_cfg is not None and norm_cfg.get('type') == 'GN', \
+            'only the GroupNorm ConvModule is implemented'
+        self.num_classes, self.in_channels = num_classes, in_channels
+        self.feat_channels, self.stacked_convs = feat_channels, stacked_convs
+        self.reg_class_agnostic, self.reg_avg_factor = reg_class_agnostic, reg_avg_factor
+        self.num_extra_reg_channel = num_extra_reg_channel
+        self.num_reg_channel = num_extra_reg_channel + 4
+        self.seperate_extra_reg_branch = seperate_extra_reg_branch and self.num_reg_channel > 4
+        self.anchor_generator, self.bbox_coder = dict(anchor_generator), dict(bbox_coder)
+        self.loss_cls_cfg, self.loss_bbox_cfg = dict(loss_cls), dict(loss_bbox)
+        self.loss_centerness_cfg = dict(loss_centerness)
+        self.train_cfg, self.test_cfg = train_cfg, test_cfg
+        self.extra_cfg = kwargs
+        g = anchor_generator
+        self.num_anchors = len(g.get('ratios', [1.0])) * (
+            g.get('scales_per_octave', 1) if 'octave_base_scale' in g else len(g.get('scales', [1])))
+        self.cls_out_channels = num_classes      # sigmoid classification
+        ng = norm_cfg.get('num_groups', 32)
+
+        def conv_module(cin):
+            m = _ConvGN2d(cin, feat_channels)
+            m.gn = nn.GroupNorm(ng, feat_channels)
+            return m
+
+        # _init_layers (liga_atss_head.py:46-128)
+        self.cls_convs = nn.ModuleList([conv_module(in_channels if i == 0 else feat_channels)
+                                        for i in range(stacked_convs)])
+        self.reg_convs = nn.ModuleList([conv_module(in_channels if i == 0 else feat_channels)
+                                        for i in range(stacked_convs)])
+        if self.seperate_extra_reg_branch:
+            self.extra_reg_convs = nn.ModuleList(
+                [conv_module(in_channels if i == 0 else feat_channels)
+                 for i in range(stacked_convs)])
+        A, R = self.num_anchors, self.num_reg_channel
+        self.atss_cls = nn.Conv2d(feat_channels, A * num_classes, 3, padding=1)
+        per = 1 if reg_class_agnostic else num_classes
+        if not self.seperate_extra_reg_branch:
+            self.atss_reg = nn.Conv2d(feat_channels, A * R * per, 3, padding=1)
+        else:
+            self.atss_reg = nn.Conv2d(feat_channels, A * 4 * per, 3, padding=1)
+            self.atss_extra_reg = nn.Conv2d(feat_channels, A * (R - 4) * per, 3, padding=1)
+        self.atss_centerness = nn.Conv2d(feat_channels, A, 3, padding=1)
+        self.scales = nn.ModuleList([_Scale(1.0) for _ in g['strides']])
+        # ATSSHead.init_weights: normal(std 0.01), classification bias at prior 0.01
+        for m in self.modules():
+            if isinstance(m, nn.Conv2d):
+                nn.init.normal_(m.weight, 0.0, 0.01)
+                if m.bias is not None:
+                    nn.init.zeros_(m.bias)
+        nn.init.constant_(self.atss_cls.bias, float(-np.log((1 - 0.01) / 0.01)))
+
+    @staticmethod
+    def _tower(convs, x):
+        for m in convs:
+            x = torch.relu(m.gn(m.conv(x)))
+        return x
+
+    def forward(self, feats):
+        """``(cls_scores, bbox_preds, centernesses)``, one entry per level."""
+        outs = [self.forward_single(x, s) for x, s in zip(feats, self.scales)]
+        return tuple(map(list, zip(*outs)))
+
+    def forward_single(self, x, scale):
+        if self.seperate_extra_reg_branch:
+            raise NotImplementedError('LIGAATSSHead: seperate_extra_reg_branch')
+        cls_feat = self._tower(self.cls_convs, x)
+        reg_feat = self._tower(self.reg_convs, x)
+        cls_score = self.atss_cls(cls_feat)
+        bbox_pred = scale(self.atss_reg(reg_feat)).float()
+        centerness = self.atss_centerness(reg_feat)
+        return cls_score, bbox_pred, centerness
+
+    def loss(self, cls_scores, bbox_preds, centernesses, gt_bboxes, gt_labels, img_metas,
+             gt_bboxes_ignore=None):
+        """``ATSSHead.loss`` with LIGA's ``loss_single`` (liga_atss_head.py:176-270) on CUDA:
+        ``dict(loss_cls=[L], loss_bbox=[L], loss_centerness=[L])`` of 0-dim device tensors,
+        differentiable with respect to the 3 x L head outputs (fp32 CUDA tensors).
+        ``gt_bboxes``: per image ``[M, 6]``, the 2-D box then the projected 3-D centre;
+        ``gt_labels``: ``[M]`` ints in ``0..num_classes-1`` (host labels outside it raise
+        ``ValueError``, device labels make every loss NaN); ``img_metas``: ``pad_shape`` per
+        image.  Both normalisers are all-reduced means under ``torch.distributed``.  Refuses
+        ``gt_bboxes_ignore``, ``reg_class_agnostic``, extra regression channels,
+        ``reg_avg_factor='sum_centerness'``, several anchors per location, other assigner modes
+        and other loss types with ``NotImplementedError``.  No host synchronisation."""
+        if not hasattr(self, '_atss_loss'):
+            self._atss_loss = _ATSSLoss()
+        return self._atss_loss.run(self, cls_scores, bbox_preds, centernesses, gt_bboxes,
+                                   gt_labels, img_metas, gt_bboxes_ignore)
+
+
 class _ConvModuleConv(nn.Module):
     """Parameter layout of mmcv ConvModule without norm or activation: .conv only."""
 

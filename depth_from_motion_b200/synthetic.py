@@ -672,6 +672,76 @@ ANCHOR_LOSS_GOLDEN_CASES = {
 }
 
 
+# DfM's 2-D auxiliary head, bbox_head_2d of configs/dfm/dfm_r34_1x8_kitti-3d-3class.py:79-117
+# (the same block in every shipped KITTI config)
+KITTI_ATSS_HEAD = dict(
+    num_classes=3, in_channels=64, stacked_convs=4, feat_channels=64, reg_class_agnostic=False,
+    seperate_extra_reg_branch=False, num_extra_reg_channel=0,
+    anchor_generator=dict(type='AnchorGenerator', ratios=[1.0], octave_base_scale=16,
+                          scales_per_octave=1, strides=[4, 8, 16, 32, 64]),
+    bbox_coder=dict(type='DeltaXYWHBBoxCoder', target_means=[.0, .0, .0, .0],
+                    target_stds=[0.1, 0.1, 0.2, 0.2]),
+    loss_cls=FOCAL_LOSS, loss_bbox=dict(type='GIoULoss', loss_weight=2.0),
+    loss_centerness=dict(type='CrossEntropyLoss', use_sigmoid=True, loss_weight=1.0),
+    train_cfg=dict(assigner=dict(type='ATSS3DCenterAssigner', topk=9), allowed_border=-1,
+                   pos_weight=-1, append_3d_centers=True))
+ATSS_STRIDES = (4, 8, 16, 32, 64)
+
+
+def atss_feat_sizes(h, w, strides=ATSS_STRIDES):
+    """Feature sizes of the 2-D neck's five outputs for an h x w (padded) image."""
+    return [(int(np.ceil(h / s)), int(np.ceil(w / s))) for s in strides]
+
+
+def make_atss_loss_case(seed, feat_sizes, num_gt, pad_shapes, num_classes=3, head_scale=1.0,
+                        compete=False, far_centres=False):
+    """Head outputs (per level [B, C, H, W], [B, 4 * C, H, W], [B, 1, H, W]) and per-image GT
+    (``[M, 6]``: the 2-D box, then the projected 3-D centre; ``[M]`` int64 labels) for
+    ``num_gt[b]`` boxes inside image b's pad shape.  The centres sit near the box centre, a
+    quarter of them outside their box.  ``compete``: every second GT is a shifted copy of the one
+    before, so the two compete for anchors; ``far_centres``: two centres lie outside the image."""
+    rng = np.random.RandomState(seed)
+    B, C = len(num_gt), num_classes
+    cls, box, ctr = [], [], []
+    for h, w in feat_sizes:
+        cls.append((-2.0 + 1.5 * rng.standard_normal((B, C, h, w))) * head_scale)
+        box.append(0.5 * rng.standard_normal((B, 4 * C, h, w)) * head_scale)
+        ctr.append(rng.standard_normal((B, 1, h, w)) * head_scale)
+    gts, labels = [], []
+    for m, (ph, pw) in zip(num_gt, pad_shapes):
+        bw = rng.uniform(12.0, 0.8 * pw, m)
+        bh = rng.uniform(10.0, 0.9 * ph, m)
+        x1 = rng.uniform(0.0, pw - bw)
+        y1 = rng.uniform(0.0, ph - bh)
+        g = np.stack([x1, y1, x1 + bw, y1 + bh], 1)
+        if compete:
+            for i in range(1, m, 2):
+                g[i] = g[i - 1] + rng.uniform(-0.15, 0.15) * np.array([bw[i - 1], bh[i - 1]] * 2)
+        c = np.stack([(g[:, 0] + g[:, 2]) / 2, (g[:, 1] + g[:, 3]) / 2], 1)
+        c += rng.uniform(-0.3, 0.3, (m, 2)) * (g[:, 2:] - g[:, :2])
+        out = rng.uniform(size=m) < 0.25
+        c[out] = g[out, 2:] + rng.uniform(2.0, 20.0, (int(out.sum()), 2))
+        if far_centres and m >= 2:
+            c[0] = (-37.3, 0.4 * ph)
+            c[1] = (pw + 51.7, ph + 23.1)
+        gts.append(torch.from_numpy(np.concatenate([g, c], 1).astype(np.float32)))
+        labels.append(torch.from_numpy(rng.randint(0, C, size=m).astype(np.int64)))
+    t = lambda a: torch.from_numpy(a.astype(np.float32))  # noqa: E731
+    return [t(a) for a in cls], [t(a) for a in box], [t(a) for a in ctr], gts, labels
+
+
+# name -> (pad shape the features are sized for, per-image pad shapes, GT per image,
+# make_atss_loss_case arguments, seed): tests/golden/atss_loss.npz
+ATSS_LOSS_GOLDEN_CASES = {
+    'b1': ((128, 256), [(128, 256)], [6], {}, 501),
+    'b2_pad_shapes': ((64, 192), [(64, 192), (40, 120)], [5, 4], {}, 502),
+    'b2_one_empty': ((64, 192), [(64, 192), (64, 160)], [0, 7], {}, 503),
+    'b1_competing': ((96, 160), [(96, 160)], [8], dict(compete=True), 504),
+    'b1_far_centres': ((64, 192), [(64, 192)], [5], dict(far_centres=True), 505),
+    'b1_no_gt': ((64, 192), [(64, 192)], [0], {}, 506),
+}
+
+
 def make_depth_loss_case(seed, n, D, H, W, f=4, density=0.05, num_boxes=6):
     """Inputs of ``DepthHead.loss`` for ``n`` images (B * N): smooth cost logits
     ``[n, 1, D, H, W]`` in about +-20 (``smooth_field``), a sparse scan-line-like depth map

@@ -756,6 +756,69 @@ int dfm_anchor_loss_debug_tensor(dfm_anchor_loss_t* h, const char* name, void* d
                                  long long numel, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * Training loss of DfM's 2-D auxiliary LIGAATSSHead (liga_atss_head.py:176-270, 380-483 with
+ * mmdet 2.x's ATSSHead.loss) for `batch` images of num_levels levels per call, one square anchor
+ * of side octave_base_scale * stride per location (AnchorGenerator, ratios [1], one scale,
+ * centre offset 0): ATSS3DCenterAssigner (topk nearest valid anchors per level to the GT's
+ * projected 3-D centre, IoU >= mean + std of the candidates, anchor centre more than 0.01 inside
+ * the 2-D box, highest IoU wins), PseudoSampler, DeltaXYWHBBoxCoder targets (means 0) and
+ * centerness targets, then per level the sigmoid focal loss, GIoU of the decoded positives
+ * weighted by their centerness targets, and the centerness BCE.  Anchors of level l at
+ * (x * stride, y * stride), index off_l + y * feat_w + x; the valid anchors of each image come
+ * from its pad shape (min(ceil(pad / stride), feat) rows and columns).  Two orders the
+ * reference leaves to torch are fixed: equal distances at the topk-th candidate keep the lower
+ * anchor index, and an anchor positive for several GT with equal IoU goes to the first GT.  The
+ * threshold's mean and std are formed in fp64 in candidate order (level, then distance), each
+ * rounded to fp32, then added in fp32.  No host synchronisation inside forward or finish; sums
+ * run in a fixed order, so repeated calls are bitwise equal.  Create fails with DFM_ERR_INVALID
+ * on more than 16 classes, 8 levels or 32 images, or topk other than 9.
+ * ---------------------------------------------------------------------------------- */
+typedef struct dfm_atss_loss dfm_atss_loss_t;
+typedef struct dfm_atss_loss_desc {
+  int num_classes;              /* C sigmoid classes                                          */
+  int num_levels;               /* L                                                          */
+  int strides[8];               /* per level, integer                                         */
+  int feat_h[8], feat_w[8];     /* per level                                                  */
+  int batch;                    /* images per call                                            */
+  int topk;                     /* ATSS3DCenterAssigner topk (9)                              */
+  float octave_base_scale;      /* anchor side / stride                                       */
+  float target_stds[4];         /* DeltaXYWHBBoxCoder; x = y and w = h                        */
+  float wh_ratio_clip;          /* size deltas clamped to +- |log(wh_ratio_clip)|             */
+  float giou_eps;               /* GIoULoss eps                                               */
+  float gamma, alpha;           /* FocalLoss                                                  */
+  float loss_weight[3];         /* cls, bbox, centerness                                      */
+} dfm_atss_loss_desc_t;
+int dfm_atss_loss_create(const dfm_atss_loss_desc_t* desc, dfm_atss_loss_t** out);
+int dfm_atss_loss_destroy(dfm_atss_loss_t* h);
+/* d_cls / d_bbox / d_centerness: host arrays of num_levels device pointers, level l
+ * [batch][C][feat_h][feat_w], [batch][4 * C][feat_h][feat_w] (channel k * C + c: coordinate k of
+ * class c) and [batch][1][feat_h][feat_w].  GT packed: d_gt_boxes [G][6] (2-D box x1, y1, x2, y2,
+ * then the projected 3-D centre x, y), d_gt_labels [G] int32 in 0..C-1, d_gt_off / h_gt_off
+ * [batch + 1] on the device and the host; h_pad_shape [batch][2] (pad height, width) on the host.
+ * Writes the gradients of the unnormalised, unweighted per-level sums into each non-null entry of
+ * the host arrays d_grad_* (the arrays themselves may be NULL; same layouts as the inputs) and
+ * d_norm [2] = (sum over images of max(positives, 1), sum of the centerness targets).  A GT
+ * label outside 0..C-1 is detected on the device and makes every loss of the next finish NaN. */
+int dfm_atss_loss_forward(dfm_atss_loss_t* h, const float* const* d_cls,
+                          const float* const* d_bbox, const float* const* d_centerness,
+                          const float* d_gt_boxes, const int* d_gt_labels, const int* d_gt_off,
+                          const int* h_gt_off, const int* h_pad_shape, float* const* d_grad_cls,
+                          float* const* d_grad_bbox, float* const* d_grad_centerness,
+                          float* d_norm, void* stream);
+/* From the last forward and d_avg [2] (d_norm, or its mean over ranks): d_losses [3][L]
+ * (loss_cls, loss_bbox, loss_centerness of each level) and d_scales [3][L], the factor each
+ * stored gradient takes to become that of its loss. */
+int dfm_atss_loss_finish(dfm_atss_loss_t* h, const float* d_avg, float* d_losses,
+                         float* d_scales, void* stream);
+/* Test hook, from the last forward, [batch][N] per anchor (N over all levels): "assigned_gt"
+ * int32 (0 negative or invalid, g + 1 for the image's GT g), "labels" int32 (C for negatives
+ * and invalid anchors), "label_weights" fp32, "centerness_targets" fp32 (0 for non-positives),
+ * "bbox_targets" fp32 [batch][N][4]; "thresholds" fp32 [G], each GT's IoU threshold.
+ * DFM_ERR_STATE before a forward, DFM_ERR_INVALID on an unknown name or wrong element count. */
+int dfm_atss_loss_debug_tensor(dfm_atss_loss_t* h, const char* name, void* d_out,
+                               long long numel, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * DepthHead.loss (dense_heads/depth_head.py:75-188) and its gradient for num_images = B * N
  * images per call, types ce / balanced_ce / focal / balanced_focal: per masked pixel
  *   w_pix * sum_k p_k * alpha * (1 - P_k)^gamma * (-log P_k),
