@@ -14,7 +14,8 @@ DEPS = [os.path.join(HERE, 'csrc', f) for f in
          'liga_resnet_api.inc', 'resnet101_kernels.cuh', 'resnet101_api.inc',
          'box_post_kernels.cuh', 'box_post_api.inc', 'anchor_loss_kernels.cuh',
          'anchor_loss_api.inc', 'depth_loss_kernels.cuh', 'depth_loss_api.inc',
-         'atss_loss_kernels.cuh', 'atss_loss_api.inc',
+         'atss_loss_kernels.cuh', 'atss_loss_api.inc', 'imitation_loss_kernels.cuh',
+         'imitation_loss_api.inc',
          'image_prep_kernels.cuh',
          'image_prep_api.inc', 'view_cache_kernels.cuh', 'view_cache_api.inc',
          'kitti_eval_kernels.cuh', 'kitti_eval_api.inc', 'waymo_eval_kernels.cuh',

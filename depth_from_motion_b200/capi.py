@@ -67,6 +67,9 @@ SYMBOLS = (
     'dfm_depth_loss_forward', 'dfm_depth_loss_debug_tensor',
     'dfm_atss_loss_create', 'dfm_atss_loss_destroy', 'dfm_atss_loss_forward',
     'dfm_atss_loss_finish', 'dfm_atss_loss_debug_tensor',
+    'dfm_imitation_loss_create', 'dfm_imitation_loss_destroy', 'dfm_imitation_loss_workspace',
+    'dfm_imitation_loss_forward', 'dfm_imitation_loss_finish', 'dfm_imitation_loss_backward',
+    'dfm_imitation_loss_debug_tensor',
 )
 
 DFM_IMAGE_PREP_CROP, DFM_IMAGE_PREP_RESCALE = 0, 1
@@ -186,6 +189,13 @@ class AtssLossDesc(ctypes.Structure):
                 ('octave_base_scale', c_float), ('target_stds', c_float * 4),
                 ('wh_ratio_clip', c_float), ('giou_eps', c_float), ('gamma', c_float),
                 ('alpha', c_float), ('loss_weight', c_float * 3)]
+
+
+class ImitationLossDesc(ctypes.Structure):
+    """``dfm_imitation_loss_desc_t``."""
+    _fields_ = [(n, c_int) for n in ('batch', 'ny', 'nx', 'num_pairs')] + \
+               [('channels', c_int * 2), ('depth', c_int * 2), ('loss_weight', c_float * 2),
+                ('normalizer_clamp_value', c_float)]
 
 
 class ImagePrepDesc(ctypes.Structure):
@@ -329,6 +339,13 @@ def lib():
     L.dfm_atss_loss_forward.argtypes = [vp] * 14
     L.dfm_atss_loss_finish.argtypes = [vp] * 5
     L.dfm_atss_loss_debug_tensor.argtypes = [vp, c_char_p, vp, c_longlong, vp]
+    L.dfm_imitation_loss_create.argtypes = [POINTER(ImitationLossDesc), POINTER(vp)]
+    L.dfm_imitation_loss_destroy.argtypes = [vp]
+    L.dfm_imitation_loss_workspace.argtypes = [vp, POINTER(c_longlong)]
+    L.dfm_imitation_loss_forward.argtypes = [vp] * 10 + [c_int, vp, vp]
+    L.dfm_imitation_loss_finish.argtypes = [vp, vp, c_int, vp, vp, vp]
+    L.dfm_imitation_loss_backward.argtypes = [vp] * 7
+    L.dfm_imitation_loss_debug_tensor.argtypes = [vp, c_char_p, vp, c_longlong, vp]
     L.dfm_voxel_sample.argtypes = [POINTER(VoxelSampleDesc), vp, vp, POINTER(c_double), vp, vp]
     L.dfm_kitti_eval_create.argtypes = [POINTER(KittiEvalDesc), POINTER(vp)]
     L.dfm_kitti_eval_destroy.argtypes = [vp]

@@ -145,3 +145,25 @@ def load_detector(ckpt, detector, liga=None):
                        f'{" ..." if len(unknown) > 8 else ""} ({len(unknown)} in all)')
     detector.load_state_dict(keep, strict=True)
     return sorted(skipped)
+
+
+IMITATION_PREFIXES = ('conv_imitation.', 'norm_imitation.')
+
+
+def load_imitation(ckpt, module, liga=None):
+    """Strictly loads the imitation layers of a detector checkpoint into ``modules.DfMImitation``:
+    exactly its ``conv_imitation.*`` and ``norm_imitation.*`` entries, from an mmdet3d checkpoint
+    (``state_dict``), a LIGA-DfM one (``model_state``, whose ``dense_head.conv_imitation`` /
+    ``dense_head.norm_imitation`` keys the converter's table renames; ``liga=True`` applies the
+    renames to a bare state_dict too) or a bare state_dict.  A missing or extra imitation key
+    raises.  Returns what ``load_state_dict`` returns."""
+    state, liga = _unwrap(ckpt, liga)
+    keep = OrderedDict()
+    for key, value in state.items():
+        if liga:
+            if 'global_step' in key:
+                continue
+            key = convert_liga_key(key, _LIGA_RENAMES)
+        if key.startswith(IMITATION_PREFIXES):
+            keep[key] = value
+    return module.load_state_dict(keep, strict=True)

@@ -31,6 +31,7 @@
 #include "anchor_loss_kernels.cuh"
 #include "depth_loss_kernels.cuh"
 #include "atss_loss_kernels.cuh"
+#include "imitation_loss_kernels.cuh"
 #include "image_prep_kernels.cuh"
 #include "view_cache_kernels.cuh"
 #include "kitti_eval_kernels.cuh"
@@ -1573,6 +1574,7 @@ int dfm_depth_head_forward(const float* d_cost, const float* d_depth_samples, in
 #include "anchor_loss_api.inc"
 #include "depth_loss_api.inc"
 #include "atss_loss_api.inc"
+#include "imitation_loss_api.inc"
 #include "image_prep_api.inc"
 #include "view_cache_api.inc"
 #include "kitti_eval_api.inc"

@@ -2142,6 +2142,279 @@ class LIGAATSSHead(nn.Module):
                                    gt_labels, img_metas, gt_bboxes_ignore)
 
 
+class _ImitationLossFn(torch.autograd.Function):
+    """The per-pair losses of one ``dfm_imitation_loss_forward`` / ``_finish``.  When an input
+    requires grad, forward also runs ``dfm_imitation_loss_backward`` (grad_output 1) while the
+    handle's workspace still holds this call's mask; backward scales each stored gradient by its
+    loss's ``grad_output``."""
+
+    @staticmethod
+    def forward(ctx, run, *tensors):
+        P = len(run.pairs)
+        need = ctx.needs_input_grad[1:]
+        xs, ws, bs = tensors[:P], tensors[P:2 * P], tensors[2 * P:]
+        gx = [torch.empty_like(x) if need[i] else None for i, x in enumerate(xs)]
+        gw = [torch.empty_like(w) if need[P + i] else None for i, w in enumerate(ws)]
+        gb = [torch.empty_like(b) if need[2 * P + i] else None for i, b in enumerate(bs)]
+        losses, coef = run.forward(xs, ws, bs)
+        if any(need):
+            run.backward(coef, gx, gw, gb)
+        ctx.grads = gx + gw + gb
+        return losses
+
+    @staticmethod
+    def backward(ctx, go):
+        P = len(ctx.grads) // 3
+        return (None,) + tuple(g * go[i % P] if g is not None else None
+                               for i, g in enumerate(ctx.grads))
+
+
+class _ImitationLoss:
+    """``DfMImitation.loss`` through ``dfm_imitation_loss_*``: one handle per (shape, batch,
+    config, device), kept until the key changes."""
+
+    def __init__(self):
+        self.handle, self.key, self.anchors = None, None, None
+
+    def release(self):
+        if self.handle is not None:
+            capi.lib().dfm_imitation_loss_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
+
+    def anchor_xy(self, anchor_generator, ny, nx, dev):
+        """The BEV cells' anchor centres ``[nx + ny]`` (x per column, then y per row): columns 0
+        and 1 of ``grid_anchors`` rows ``(y * nx + x) * A``."""
+        key = (ny, nx, str(dev))
+        if self.anchors is None or self.anchors[0] != key:
+            with torch.cuda.device(dev):
+                a = grid_anchors(anchor_generator, ny, nx, dev)
+            A = a.shape[0] // (ny * nx)
+            xy = torch.cat((a[0:nx * A:A, 0], a[0::nx * A, 1])).contiguous()
+            self.anchors = (key, xy)
+        return self.anchors[1]
+
+    def run(self, mod, xs, ts, scales, gt_bboxes_3d):
+        B, ny, nx = xs[0].shape[0], xs[0].shape[-2], xs[0].shape[-1]
+        dev = xs[0].device
+        if len(gt_bboxes_3d) != B:
+            raise RuntimeError(f'DfMImitation.loss: {B} samples, {len(gt_bboxes_3d)} gt_bboxes_3d')
+        boxes, off = [], [0]
+        for gb in gt_bboxes_3d:
+            gb = gb.tensor if hasattr(gb, 'tensor') else gb
+            if not isinstance(gb, torch.Tensor) or gb.dim() != 2 or gb.shape[1] < 7:
+                raise RuntimeError('DfMImitation.loss: GT boxes must be [M, 7] per sample, got '
+                                   f'{tuple(gb.shape) if isinstance(gb, torch.Tensor) else gb}')
+            boxes.append(gb[:, :7].to(dev, torch.float32))
+            off.append(off[-1] + gb.shape[0])
+        self.gt = torch.cat(boxes).contiguous()
+        self.h_off = (ctypes.c_int * (B + 1))(*off)
+        self.d_off = torch.tensor(off, dtype=torch.int32).to(dev, non_blocking=True)
+        self.anchor = self.anchor_xy(mod.anchor_generator, ny, nx, dev)
+        self.pairs = [(x.shape[1], x.shape[2] if x.dim() == 5 else 1) for x in xs]
+        lw = [float(c['loss_weight']) for c in mod.imitation_cfgs]
+        P = len(self.pairs)
+        desc = (B, ny, nx, P, tuple(c for c, _ in self.pairs), tuple(z for _, z in self.pairs),
+                tuple(lw), float(mod.normalizer_clamp_value))
+        key = desc + (str(dev),)
+        if self.handle is None or key != self.key:
+            self.release()
+            pad = lambda v: v + (0,) * (2 - len(v))  # noqa: E731
+            d = capi.ImitationLossDesc(B, ny, nx, P, (ctypes.c_int * 2)(*pad(desc[4])),
+                                       (ctypes.c_int * 2)(*pad(desc[5])),
+                                       (ctypes.c_float * 2)(*pad(desc[6])), desc[7])
+            hd = ctypes.c_void_p()
+            with torch.cuda.device(dev):
+                capi.check(capi.lib().dfm_imitation_loss_create(ctypes.byref(d), ctypes.byref(hd)),
+                           'dfm_imitation_loss_create')
+            self.handle, self.key = hd, key
+        self.ts, self.scales, self.training = ts, scales, mod.training
+        ws = [c.weight for c in mod._convs()]
+        bs = [c.bias for c in mod._convs()]
+        losses = _ImitationLossFn.apply(self, *xs, *ws, *bs)
+        return [losses[i] for i in range(P)]
+
+    def forward(self, xs, ws, bs):
+        """Runs forward, the all-reduce of the packed counts and sums, and finish; returns the
+        losses [P] and the gradient coefficients [P]."""
+        import torch.distributed as dist
+        lib = capi.lib()
+        dev = xs[0].device
+        P = len(xs)
+        tabs = [_ptr_table(v) for v in (xs, self.ts, ws, bs, self.scales)]
+        packed = torch.empty(sum(2 + c for c, _ in self.pairs), device=dev)
+        ranks = dist.is_available() and dist.is_initialized()
+        world = dist.get_world_size() if ranks else 1
+        with torch.cuda.device(dev):
+            capi.check(lib.dfm_imitation_loss_forward(
+                self.handle, tabs[0][1], tabs[1][1], tabs[2][1], tabs[3][1], tabs[4][1],
+                _ptr(self.anchor), _ptr(self.gt) if self.gt.numel() else None, _ptr(self.d_off),
+                ctypes.cast(self.h_off, ctypes.c_void_p), world, _ptr(packed), _stream()),
+                'dfm_imitation_loss_forward')
+            # every pair's count / world, count and per-channel |t| sums in one all-reduce
+            if ranks:
+                dist.all_reduce(packed)
+            losses = torch.empty(P, device=dev)
+            coef = torch.empty(P, device=dev)
+            capi.check(lib.dfm_imitation_loss_finish(self.handle, _ptr(packed),
+                                                     int(self.training), _ptr(losses),
+                                                     _ptr(coef), _stream()),
+                       'dfm_imitation_loss_finish')
+        return losses, coef
+
+    def backward(self, coef, gx, gw, gb):
+        tabs = [_ptr_table(v) if any(g is not None for g in v) else (None, None)
+                for v in (gx, gw, gb)]
+        with torch.cuda.device(coef.device):
+            capi.check(capi.lib().dfm_imitation_loss_backward(
+                self.handle, _ptr(coef), None, tabs[0][1], tabs[1][1], tabs[2][1], _stream()),
+                'dfm_imitation_loss_backward')
+
+    def workspace(self):
+        """Device bytes the handle owns."""
+        b = ctypes.c_longlong(0)
+        capi.check(capi.lib().dfm_imitation_loss_workspace(self.handle, ctypes.byref(b)),
+                   'dfm_imitation_loss_workspace')
+        return b.value
+
+    def debug_tensor(self, name):
+        """From the last call (tests only): 'inbox' uint8 [B, ny, nx]; 'counts' int32 [P], this
+        rank's positives per pair; 'loss_sums' fp64 [P]."""
+        if self.handle is None:
+            raise RuntimeError('dfm_imitation_loss_debug_tensor: no loss call has run')
+        B, ny, nx = self.key[:3]
+        shape, dt = {'inbox': ((B, ny, nx), torch.uint8),
+                     'counts': ((len(self.pairs),), torch.int32),
+                     'loss_sums': ((len(self.pairs),), torch.float64)}.get(
+                         name, ((0,), torch.float32))
+        out = torch.empty(shape, device=self.gt.device, dtype=dt)
+        capi.check(capi.lib().dfm_imitation_loss_debug_tensor(self.handle, name.encode(),
+                                                              _ptr(out), out.numel(), _stream()),
+                   f'dfm_imitation_loss_debug_tensor({name})')
+        return out
+
+
+class _NormalizeLayer(nn.Module):
+    """Parameter layout of the reference's ``NormalizeLayer('cw_scale', channel)``
+    (detectors/imitation_utils.py:10-94): the running per-channel scale ``[1, C]``, which
+    ``DfMImitation.loss`` divides the teacher by and updates in training mode."""
+
+    def __init__(self, channel, momentum=0.99):
+        super().__init__()
+        self.type, self.channel, self.momentum = 'cw_scale', channel, momentum
+        self.register_buffer('scale', torch.ones(1, channel))
+
+
+class DfMImitation(nn.Module):
+    """DfM's LiDAR imitation loss (``DfM.imitation_loss``, detectors/dfm.py:455-539) with the
+    reference's imitation layers (``_init_imitation_layers``, :213-262): ``conv_imitation`` (a
+    ``ModuleList`` of 1x1 ``Conv2d`` / ``Conv3d`` with bias, or the one conv of a single config)
+    and ``norm_imitation`` (per stereo feature name, the running ``cw_scale``), with the
+    reference's ``state_dict`` keys.  Build it from the detector config's ``imitation_cfgs``,
+    ``bbox_head_3d['anchor_generator']`` and ``normalizer_clamp_value``.  The conv layers are
+    ordinary trainable parameters; the loss and its gradients run on CUDA
+    (``dfm_imitation_loss_*``).  Configurations the shipped KITTI configs do not use (mode
+    'full', kernel_size > 1, use_relu, layer 'none', a normalize type other than 'cw_scale', or
+    channel counts other than 16 / 32 / 64) raise ``NotImplementedError``."""
+
+    def __init__(self, imitation_cfgs, anchor_generator, normalizer_clamp_value=10):
+        super().__init__()
+        cfgs = list(imitation_cfgs) if isinstance(imitation_cfgs, (list, tuple)) \
+            else [imitation_cfgs]
+        if not 1 <= len(cfgs) <= 2:
+            raise NotImplementedError('DfMImitation takes one or two imitation configs')
+        for c in cfgs:
+            if c.get('mode') != 'inbox':
+                raise NotImplementedError(f"DfMImitation: mode {c.get('mode')!r} is not "
+                                          "implemented (the shipped configs use 'inbox')")
+            if c.get('layer') not in ('conv2d', 'conv3d'):
+                raise NotImplementedError(f"DfMImitation: layer {c.get('layer')!r} is not "
+                                          'implemented (conv2d and conv3d are)')
+            if c.get('kernel_size') != 1 or c.get('use_relu'):
+                raise NotImplementedError('DfMImitation: only 1x1 convs without ReLU are '
+                                          'implemented')
+            if c.get('normalize') != 'cw_scale':
+                raise NotImplementedError(f"DfMImitation: normalize {c.get('normalize')!r} is "
+                                          "not implemented (the shipped configs use 'cw_scale')")
+            if c.get('channel') not in (16, 32, 64):
+                raise NotImplementedError('DfMImitation: channel must be 16, 32 or 64')
+        self.imitation_cfgs = cfgs
+        self.anchor_generator = dict(anchor_generator)
+        self.normalizer_clamp_value = normalizer_clamp_value
+        convs = []
+        self.norm_imitation = nn.ModuleDict()
+        for c in cfgs:
+            conv = nn.Conv2d if c['layer'] == 'conv2d' else nn.Conv3d
+            convs.append(conv(c['channel'], c['channel'], kernel_size=1, padding=0, stride=1,
+                              groups=1))
+            self.norm_imitation[c['stereo_feature_layer']] = _NormalizeLayer(c['channel'])
+        self.conv_imitation = nn.ModuleList(convs) if len(convs) > 1 else convs[0]
+        self._loss = _ImitationLoss()
+
+    def _convs(self):
+        return list(self.conv_imitation) if len(self.imitation_cfgs) > 1 \
+            else [self.conv_imitation]
+
+    def loss(self, stereo_features, lidar_features, gt_bboxes_3d):
+        """The imitation losses ``[loss per config]`` (0-dim device tensors), as
+        ``losses['loss_imitation']`` holds them.  ``stereo_features`` / ``lidar_features``: dicts
+        of the stereo and teacher features by the configs' ``stereo_feature_layer`` /
+        ``lidar_feature_layer`` names (``spatial_features_2d`` ``[B, 64, ny, nx]``,
+        ``volume_features`` ``[B, 32, nz, ny, nx]``), fp32 CUDA tensors.  ``gt_bboxes_3d``: per
+        sample ``[M, 7]`` LiDAR boxes (tensors or objects with ``.tensor``).  Differentiable with
+        respect to the stereo features and the conv weights and biases; the teacher and the
+        scales get no gradient.  In training mode the scales are updated in place.  No host
+        synchronisation.
+
+        Departures from the reference, which runs only at B = 1 and only with a process group:
+        each sample is tested against its own GT (ragged lists, any B), the normaliser counts
+        the whole batch and the loss divides by B (the reference at B = 1); the counts and sums
+        are all-reduced only when ``torch.distributed`` is initialised; the update's ``n > 10``
+        gate is taken on the device; the anchor centres come from ``grid_anchors`` (the
+        reference's ``anchors[0][:, :, :, 0, 0, :3]`` indexes a list of lists and raises);
+        ``tb_dict`` is not computed."""
+        xs, ts, scales = [], [], []
+        ref = None
+        for c in self.imitation_cfgs:
+            sname, lname = c['stereo_feature_layer'], c['lidar_feature_layer']
+            if sname not in stereo_features or lname not in lidar_features:
+                raise RuntimeError(f'DfMImitation.loss: needs stereo {sname!r} and teacher '
+                                   f'{lname!r} features')
+            x, t = stereo_features[sname], lidar_features[lname]
+            scale = self.norm_imitation[sname].scale
+            for name, v in ((sname, x), (lname, t), (f'norm_imitation.{sname}.scale', scale)):
+                _check_cuda(v, name)
+            dims = 4 if c['layer'] == 'conv2d' else 5
+            if x.dim() != dims or x.shape != t.shape or x.shape[1] != c['channel'] or \
+                    (ref is not None and (x.shape[0], *x.shape[-2:]) != ref) or \
+                    x.device != t.device or scale.device != x.device:
+                raise RuntimeError(f'DfMImitation.loss: stereo {tuple(x.shape)} and teacher '
+                                   f'{tuple(t.shape)} features of {sname!r} do not match each '
+                                   f'other, the config or the other pair')
+            ref = (x.shape[0], *x.shape[-2:])
+            xs.append(x.contiguous())
+            ts.append(t.detach().contiguous())
+            scales.append(scale)
+        for conv in self._convs():
+            for v in (conv.weight, conv.bias):
+                _check_cuda(v, 'conv_imitation')
+                if v.device != xs[0].device:
+                    raise RuntimeError('DfMImitation.loss: the layers and features are on '
+                                       'different devices')
+        return self._loss.run(self, xs, ts, scales, gt_bboxes_3d)
+
+    def debug_tensor(self, name):
+        return self._loss.debug_tensor(name)
+
+    def workspace(self):
+        return self._loss.workspace()
+
+
 class _ConvModuleConv(nn.Module):
     """Parameter layout of mmcv ConvModule without norm or activation: .conv only."""
 

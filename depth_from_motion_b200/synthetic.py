@@ -765,3 +765,108 @@ def make_depth_loss_case(seed, n, D, H, W, f=4, density=0.05, num_boxes=6):
             bh, bw = rng.randint(1, max(2, fh // 3)), rng.randint(1, max(2, fw // 4))
             fg[i, y0:y0 + bh, x0:x0 + bw] = b + 1
     return cost.contiguous(), torch.from_numpy(depth), torch.from_numpy(fg)
+
+
+KITTI_IMITATION_SHAPE = (5, 304, 288)   # (nz, ny, nx) of DfM's KITTI volume and BEV features
+KITTI_IMITATION_CHANNELS = (64, 32)      # spatial_features_2d, volume_features
+
+
+def imitation_gt(seed, num_gt, ny, nx, anchor_generator=KITTI_ANCHOR_GENERATOR, yaw=True,
+                 size_scale=1.0, edge_margin=1e-4, overlap=False):
+    """``num_gt`` LiDAR boxes [M, 7] in KITTI's point-cloud range, car-sized (times
+    ``size_scale``), yaw uniform in (-pi, pi] (0 when ``yaw`` is False).  A box is redrawn until
+    no BEV anchor centre of the ny x nx grid lies within ``edge_margin`` metres of its edges, so
+    a 1-ulp difference in the in-box test cannot flip a cell.  With ``overlap`` every second box
+    is centred near the one before, so the two overlap."""
+    from .modules import grid_anchors
+    rng = np.random.RandomState(seed)
+    a = grid_anchors(anchor_generator, ny, nx, 'cpu')
+    A = a.shape[0] // (ny * nx)
+    ax, ay = a[0:nx * A:A, 0].double().numpy(), a[0::nx * A, 1].double().numpy()
+    py, px = np.meshgrid(ay, ax, indexing='ij')
+    lo, hi = KITTI_POINT_CLOUD_RANGE[:2], KITTI_POINT_CLOUD_RANGE[3:5]
+    out = []
+    while len(out) < num_gt:
+        b = np.array([rng.uniform(lo[0], hi[0]), rng.uniform(lo[1], hi[1]), rng.uniform(-2, 0),
+                      rng.uniform(3.2, 4.8) * size_scale, rng.uniform(1.4, 2.0) * size_scale,
+                      rng.uniform(1.4, 1.8), rng.uniform(-math.pi, math.pi) if yaw else 0.0])
+        if overlap and len(out) % 2 == 1:
+            b[:2] = out[-1][:2] + rng.uniform(-0.4, 0.4, 2) * b[3:5]
+        b = b.astype(np.float32).astype(np.float64)
+        c, s = math.cos(-b[6]), math.sin(-b[6])
+        lx = (px - b[0]) * c - (py - b[1]) * s
+        ly = (px - b[0]) * s + (py - b[1]) * c
+        near = (np.abs(np.abs(lx) - b[3] / 2) < edge_margin) & (np.abs(ly) <= b[4] / 2 + 1) | \
+               (np.abs(np.abs(ly) - b[4] / 2) < edge_margin) & (np.abs(lx) <= b[3] / 2 + 1)
+        if edge_margin > 0 and near.any():
+            continue
+        out.append(b)
+    return torch.tensor(np.array(out, dtype=np.float32).reshape(-1, 7))
+
+
+def make_imitation_case(seed, batch, num_gt, shape=KITTI_IMITATION_SHAPE,
+                        channels=KITTI_IMITATION_CHANNELS, occupancy=0.08, nan_rows=0, yaw=True,
+                        size_scale=1.0, edge_margin=1e-4, overlap=False):
+    """Inputs of ``DfMImitation.loss`` at ``shape`` (nz, ny, nx): stereo features (dense
+    normals), the teacher's (zero outside a sparse occupied pattern, as sparse-conv outputs are:
+    a BEV cell is occupied with probability ``occupancy``, or 0.6 near a GT centre, each z slice
+    of an occupied cell with probability 1/2, and occupied rows hold ReLU'd normals), per-sample
+    GT (``num_gt`` an int or one count per sample, see ``imitation_gt``) and the two 1x1 convs'
+    weights and biases (PyTorch's default init).  ``nan_rows`` occupied teacher rows of each
+    pair get one NaN channel.  Returns dict(stereo, teacher, gt, params) with the features keyed
+    as DfM's ``raw_features`` and params ``[W_bev, b_bev, W_vol, b_vol]``; all on the CPU."""
+    nz, ny, nx = shape
+    counts = [num_gt] * batch if isinstance(num_gt, int) else list(num_gt)
+    gt = [imitation_gt(seed * 131 + b, n, ny, nx, yaw=yaw, size_scale=size_scale,
+                       edge_margin=edge_margin, overlap=overlap) for b, n in enumerate(counts)]
+    g = torch.Generator().manual_seed(seed)
+    cb, cv = channels
+    from .modules import grid_anchors
+    a = grid_anchors(KITTI_ANCHOR_GENERATOR, ny, nx, 'cpu')
+    A = a.shape[0] // (ny * nx)
+    ax, ay = a[0:nx * A:A, 0], a[0::nx * A, 1]
+    occ = torch.rand((batch, ny, nx), generator=g) < occupancy
+    for b, boxes in enumerate(gt):
+        for box in boxes:
+            near = ((ax.view(1, nx) - box[0]) ** 2 + (ay.view(ny, 1) - box[1]) ** 2) < \
+                (0.6 * float(box[3])) ** 2
+            occ[b] |= near & (torch.rand((ny, nx), generator=g) < 0.6)
+    vocc = occ.unsqueeze(1) & (torch.rand((batch, nz, ny, nx), generator=g) < 0.5)
+    bocc = vocc.any(1)
+    t_bev = torch.relu(torch.randn((batch, cb, ny, nx), generator=g)) * bocc.unsqueeze(1)
+    t_vol = torch.relu(torch.randn((batch, cv, nz, ny, nx), generator=g)) * vocc.unsqueeze(1)
+    for t, o in ((t_bev, bocc), (t_vol, vocc)):
+        idx = torch.nonzero(o.reshape(-1)).view(-1)
+        if nan_rows and idx.numel():
+            pick = idx[torch.randperm(idx.numel(), generator=g)[:nan_rows]]
+            ch = torch.randint(0, t.shape[1], (pick.numel(),), generator=g)
+            cl = t.movedim(1, -1).contiguous()
+            cl.view(-1, t.shape[1])[pick, ch] = float('nan')
+            t.copy_(cl.movedim(-1, 1))
+    x_bev = torch.randn((batch, cb, ny, nx), generator=g) * 0.5
+    x_vol = torch.randn((batch, cv, nz, ny, nx), generator=g) * 0.5
+    params = []
+    for c in (cb, cv):
+        bound = 1.0 / math.sqrt(c)
+        params += [(torch.rand((c, c), generator=g) * 2 - 1) * bound,
+                   (torch.rand((c,), generator=g) * 2 - 1) * bound]
+    return dict(stereo=dict(spatial_features_2d=x_bev, volume_features=x_vol),
+                teacher=dict(spatial_features_2d=t_bev, volume_features=t_vol), gt=gt,
+                params=params)
+
+
+# the seeded cases of tests/golden/imitation_loss.npz at a reduced grid: (seed, num_gt, keyword
+# arguments of make_imitation_case, training mode)
+IMITATION_GOLDEN_SHAPE = (5, 48, 40)
+IMITATION_GOLDEN_CASES = {
+    'no_gt': (601, 0, dict(occupancy=0.3), True),
+    'one_gt_axis_aligned': (602, 1, dict(occupancy=0.3, yaw=False, size_scale=3.0), True),
+    'overlapping_rotated_nan': (603, 6, dict(occupancy=0.3, size_scale=2.5, overlap=True,
+                                             nan_rows=4), True),
+    'overlapping_rotated_nan_eval': (603, 6, dict(occupancy=0.3, size_scale=2.5, overlap=True,
+                                                  nan_rows=4), False),
+    'gate_10_11': (604, 3, dict(occupancy=0.3, size_scale=3.0), True),
+    'few_positives': (605, 3, dict(occupancy=0.3, size_scale=3.0), True),
+}
+# positives kept per pair (bev, volume) by zeroing every other teacher row
+IMITATION_GOLDEN_KEEP = {'gate_10_11': (10, 11), 'few_positives': (4, 7)}

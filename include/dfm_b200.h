@@ -819,6 +819,68 @@ int dfm_atss_loss_debug_tensor(dfm_atss_loss_t* h, const char* name, void* d_out
                                long long numel, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * DfM's LiDAR imitation loss (detectors/dfm.py:455-539 with imitation_utils.py's
+ * NormalizeLayer('cw_scale') and WeightedL2WithSigmaLoss, mode 'inbox', 1x1 conv, no ReLU) for
+ * `batch` samples and num_pairs (stereo x, teacher t) feature pairs per call.  Pair i has
+ * channels[i] channels (16, 32 or 64) and depth[i] z slices (1 for the BEV pair): both tensors
+ * are [batch][C][depth][ny][nx].  A row (b, z, y, x) is positive when the BEV cell (y, x)'s
+ * anchor centre (anchor_x[x], anchor_y[y], 0) lies in one of sample b's GT boxes (mmcv's
+ * points_in_boxes_part test in fp32, GT z taken as 0) and any channel of t's row is non-zero
+ * (NaN counts).  With N the positives' count (its mean over ranks), w = 1 / max(N, clamp) and
+ * s the [C] cw_scale buffer as it was at the call's start, pair i's loss is
+ *   loss_weight[i] / batch * sum_rows w * mean_c 0.5 * (W x + bias - t / s)_c^2,
+ * a NaN t / s counting as a zero difference.  In training mode, when the positives summed over
+ * ranks n exceed 10, finish updates s in place: s = s * 0.99 + (sum_rows |t| / n) * 0.01 in
+ * fp32.  Sums run in fp64 in a fixed order without atomics, so repeated calls are bitwise equal;
+ * nothing synchronises with the host.  Create fails with DFM_ERR_INVALID on a batch outside
+ * 1..64, num_pairs outside 1..2 or other channel counts.
+ * ---------------------------------------------------------------------------------- */
+typedef struct dfm_imitation_loss dfm_imitation_loss_t;
+typedef struct dfm_imitation_loss_desc {
+  int batch;                    /* B                                                          */
+  int ny, nx;                   /* BEV grid                                                   */
+  int num_pairs;                /* 1 or 2                                                     */
+  int channels[2];              /* C of each pair                                             */
+  int depth[2];                 /* z slices of each pair (1 for a BEV feature)                */
+  float loss_weight[2];         /* imitation_cfg['loss_weight'] of each pair                  */
+  float normalizer_clamp_value; /* the normaliser's lower clamp (10 in the shipped configs)    */
+} dfm_imitation_loss_desc_t;
+int dfm_imitation_loss_create(const dfm_imitation_loss_desc_t* desc, dfm_imitation_loss_t** out);
+int dfm_imitation_loss_destroy(dfm_imitation_loss_t* h);
+/* Device bytes the handle owns (the in-box mask and per-block partials). */
+int dfm_imitation_loss_workspace(dfm_imitation_loss_t* h, long long* bytes);
+/* Host arrays of num_pairs device pointers: d_stereo, d_teacher (see above), d_weight [C][C]
+ * (out, in), d_bias [C], d_scale [C] (read here, updated by finish).  d_anchor_xy [nx + ny]: the
+ * anchor centres' x per column, then y per row.  GT packed: d_gt_boxes [G][7] LiDAR boxes (x, y,
+ * z, dx, dy, dz, yaw), d_gt_off / h_gt_off [batch + 1] on the device and the host.  Writes
+ * d_packed, per pair (count / world, count, sum_rows |t_c| for each c), to be summed over ranks
+ * before finish. */
+int dfm_imitation_loss_forward(dfm_imitation_loss_t* h, const float* const* d_stereo,
+                               const float* const* d_teacher, const float* const* d_weight,
+                               const float* const* d_bias, const float* const* d_scale,
+                               const float* d_anchor_xy, const float* d_gt_boxes,
+                               const int* d_gt_off, const int* h_gt_off, int world,
+                               float* d_packed, void* stream);
+/* From the last forward and d_packed summed over ranks: d_losses [num_pairs], d_coef
+ * [num_pairs] (loss_weight * w / (batch * C), the factor from pred - t to the loss's gradient)
+ * and, when training, the scale update. */
+int dfm_imitation_loss_finish(dfm_imitation_loss_t* h, const float* d_packed, int training,
+                              float* d_losses, float* d_coef, void* stream);
+/* Gradients of the last forward's losses, times d_grad_out [num_pairs] (NULL: 1), into each
+ * non-null entry of the host arrays (the arrays may be NULL): d_grad_stereo (every element is
+ * written, zero outside the positives), d_grad_weight [C][C] and d_grad_bias [C].  Reads the
+ * workspace the last forward wrote: call it before the next forward. */
+int dfm_imitation_loss_backward(dfm_imitation_loss_t* h, const float* d_coef,
+                                const float* d_grad_out, float* const* d_grad_stereo,
+                                float* const* d_grad_weight, float* const* d_grad_bias,
+                                void* stream);
+/* Test hook, from the last forward: "inbox" uint8 [batch][ny][nx], "counts" int32 [num_pairs]
+ * (this rank's positives), "loss_sums" fp64 [num_pairs] (sum_rows sum_c 0.5 * diff^2).
+ * DFM_ERR_STATE before a forward, DFM_ERR_INVALID on an unknown name or wrong element count. */
+int dfm_imitation_loss_debug_tensor(dfm_imitation_loss_t* h, const char* name, void* d_out,
+                                    long long numel, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * DepthHead.loss (dense_heads/depth_head.py:75-188) and its gradient for num_images = B * N
  * images per call, types ce / balanced_ce / focal / balanced_focal: per masked pixel
  *   w_pix * sum_k p_k * alpha * (1 - P_k)^gamma * (-log P_k),
