@@ -12,7 +12,7 @@ DEPS = [os.path.join(HERE, 'csrc', f) for f in
          'neck_api.inc', 'frustum_api.inc', 'frustum_kernels.cuh', 'pipeline_api.inc', 'bev_api.inc', 'tail_kernels.cuh', 'voxel_sample_api.inc', 'stereo_tail_api.inc', 'logits_tc.cuh', 'wgmma.cuh', 'head1x1_tc.cuh', 'anchor3d_head_api.inc', 'spp_neck_kernels.cuh',
          'spp_neck_api.inc', 'fpn_kernels.cuh', 'fpn_api.inc', 'resnet_kernels.cuh',
          'liga_resnet_api.inc', 'resnet101_kernels.cuh', 'resnet101_api.inc',
-         'box_post_kernels.cuh', 'box_post_api.inc', 'anchor_loss_kernels.cuh',
+         'box_post_kernels.cuh', 'box_post_api.inc', 'loss_common.cuh', 'anchor_loss_kernels.cuh',
          'anchor_loss_api.inc', 'depth_loss_kernels.cuh', 'depth_loss_api.inc',
          'atss_loss_kernels.cuh', 'atss_loss_api.inc', 'imitation_loss_kernels.cuh',
          'imitation_loss_api.inc',

@@ -24,6 +24,7 @@
 #include <cstdint>
 
 #include "box_post_kernels.cuh"
+#include "loss_common.cuh"
 
 namespace dfm {
 
@@ -85,38 +86,6 @@ __device__ __forceinline__ void al_nearest_bev(const AnchorLossParams& p, const 
   o[1] = __fsub_rn(b[1], hy);
   o[2] = __fadd_rn(b[0], hx);
   o[3] = __fadd_rn(b[1], hy);
-}
-
-// mmcv sigmoid_focal_loss forward (l) and backward (g) of one logit x in fp32, as its CUDA
-// kernels compute them; is_target: the logit's class is the anchor's label
-__device__ __forceinline__ void sigmoid_focal_term(float x, bool is_target, float gamma,
-                                                   float alpha, float& l, float& g) {
-  const float pr = 1.f / (1.f + expf(-x));
-  if (is_target) {
-    const float lp = logf(fmaxf(pr, FLT_MIN));
-    l = -alpha * powf(1.f - pr, gamma) * lp;
-    g = -alpha * powf(1.f - pr, gamma) * (1.f - pr - gamma * pr * lp);
-  } else {
-    const float lq = logf(fmaxf(1.f - pr, FLT_MIN));
-    l = -(1.f - alpha) * powf(pr, gamma) * lq;
-    g = -(1.f - alpha) * powf(pr, gamma) * (gamma * (1.f - pr) * lq - pr);
-  }
-}
-
-// (x2 - x1) * (y2 - y1) of an (x1, y1, x2, y2) box
-__device__ __forceinline__ float al_area(const float* o) {
-  return __fmul_rn(__fsub_rn(o[2], o[0]), __fsub_rn(o[3], o[1]));
-}
-
-// mmdet bbox_overlaps(gt, anchor), mode 'iou', eps 1e-6, of axis-aligned (x1, y1, x2, y2) boxes
-// with areas ga and aa; symmetric in its two boxes, as every op it rounds is
-__device__ __forceinline__ float al_iou(const float* g, float ga, const float* a, float aa) {
-  const float w = fmaxf(__fsub_rn(fminf(g[2], a[2]), fmaxf(g[0], a[0])), 0.f);
-  const float h = fmaxf(__fsub_rn(fminf(g[3], a[3]), fmaxf(g[1], a[1])), 0.f);
-  const float ov = __fmul_rn(w, h);
-  if (ov == 0.f) return 0.f;
-  const float un = fmaxf(__fsub_rn(__fadd_rn(ga, aa), ov), 1e-6f);
-  return __fdiv_rn(ov, un);
 }
 
 __global__ void al_anchor_bev_kernel(AnchorLossParams p, float* bev, float* area) {
@@ -386,25 +355,6 @@ __device__ __noinline__ double al_iou3d_loss(const float* pred, const float* tgt
 
 // ---- loss-and-gradient pass ----
 
-// K fp64 sums over a block of NT threads in a fixed tree order; the totals land in red[k][0]
-template <int K, int NT>
-__device__ __forceinline__ void block_sum_fp64(const double* v, double (*red)[NT]) {
-#pragma unroll
-  for (int k = 0; k < K; ++k) red[k][threadIdx.x] = v[k];
-  __syncthreads();
-  for (int h = NT / 2; h > 0; h >>= 1) {
-    if (threadIdx.x < h) {
-#pragma unroll
-      for (int k = 0; k < K; ++k) red[k][threadIdx.x] += red[k][threadIdx.x + h];
-    }
-    __syncthreads();
-  }
-}
-
-__device__ __forceinline__ void al_block_sum4(double* v, double (*red)[AL_THREADS]) {
-  block_sum_fp64<4, AL_THREADS>(v, red);
-}
-
 __global__ void __launch_bounds__(AL_THREADS) al_loss_kernel(AnchorLossParams p) {
   __shared__ double red[4][AL_THREADS];
   const int b = blockIdx.y, n = blockIdx.x * blockDim.x + threadIdx.x;
@@ -519,7 +469,7 @@ __global__ void __launch_bounds__(AL_THREADS) al_loss_kernel(AnchorLossParams p)
       }
     }
   }
-  al_block_sum4(acc, red);
+  block_sum_fp64<4, AL_THREADS>(acc, red);
   if (threadIdx.x == 0) {
     double* o = p.partial + ((size_t)b * p.blocks + blockIdx.x) * 4;
 #pragma unroll
@@ -550,7 +500,7 @@ __global__ void __launch_bounds__(AL_THREADS) al_finish_kernel(const double* par
 #pragma unroll
     for (int k = 0; k < 4; ++k) v[k] += partial[(size_t)i * 4 + k];
   }
-  al_block_sum4(v, red);
+  block_sum_fp64<4, AL_THREADS>(v, red);
   if (threadIdx.x < 4) {
     const int k = threadIdx.x;
     const double a = *avg, eps = (double)FLT_EPSILON;

@@ -25,7 +25,7 @@
 #include <cfloat>
 #include <cstdint>
 
-#include "anchor_loss_kernels.cuh"
+#include "loss_common.cuh"
 
 namespace dfm {
 

@@ -6,6 +6,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <climits>
 #include <cmath>
 #include <cstring>
 #include <functional>
@@ -194,6 +195,49 @@ int debug_copy(const DevBuf& b, long long written, const std::string& name, floa
                          (cudaStream_t)stream));
   return DFM_OK;
 }
+
+// Test hooks of the loss and eval handles, once the name is known and a forward has run: copies
+// the `want` elements of `elem_bytes` each at `src` into a tensor of `numel` elements, which must
+// be `want` (an empty tensor copies nothing).
+int copy_debug(const std::string& k, const void* src, long long want, long long numel,
+               size_t elem_bytes, void* d_out, void* stream) {
+  if (numel != want)
+    return fail(DFM_ERR_INVALID, k + ": the tensor holds " + std::to_string(want) +
+                                     " elements, not " + std::to_string(numel));
+  if (want > 0)
+    CU_TRY(cudaMemcpyAsync(d_out, src, (size_t)want * elem_bytes, cudaMemcpyDeviceToDevice,
+                           (cudaStream_t)stream));
+  return DFM_OK;
+}
+
+// The host GT offsets [B + 1] of a loss forward: they start at 0 and ascend, give each sample at
+// most `per_sample` boxes and all samples at most `total`; *G is the total.  Any other offsets
+// fail with `msg`.
+int check_gt_offsets(const int* h_off, int B, long long per_sample, long long total,
+                     const std::string& msg, int* G) {
+  long long g = 0;
+  for (int b = 0; b < B; ++b) {
+    const long long n = (long long)h_off[b + 1] - h_off[b];
+    if (h_off[b] != g || n < 0 || n > per_sample || g + n > total)
+      return fail(DFM_ERR_INVALID, msg);
+    g += n;
+  }
+  *G = (int)g;
+  return DFM_OK;
+}
+
+// carves aligned sub-arrays out of one allocation (a first pass with base == nullptr sizes it)
+struct BpArena {
+  char* base;
+  size_t off = 0;
+  template <class T>
+  T* take(size_t count) {
+    off = (off + 255) & ~(size_t)255;
+    T* r = base ? reinterpret_cast<T*>(base + off) : nullptr;
+    off += count * sizeof(T);
+    return r;
+  }
+};
 
 struct Norm {  // GroupNorm (statistics computed per frame) or folded BatchNorm (static)
   int C = 0;

@@ -160,38 +160,27 @@ class _CudaMirror(nn.Module):
                 'is not implemented')
 
 
-class _HandleMirror(_CudaMirror):
-    """A mirror that owns one handle of include/dfm_b200.h, of the family ``_family``
-    (``dfm_<family>_create`` / ``_destroy`` / ``_set_param`` / ``_debug_tensor``).  Subclasses
-    give the key the handle is built for, the create arguments and the forward."""
+class _Handle:
+    """Owns one handle of include/dfm_b200.h, of the family ``_family`` (``dfm_<family>_create`` /
+    ``_destroy``, and where the family has them ``_workspace`` / ``_debug_tensor``), built for one
+    key and rebuilt when the key changes."""
     _family = None
     _handle = None
     _key = None
-    _batch = None
 
-    def _ensure(self, key, create_args, batch=None):
-        """``capi.lib()``, with a handle for ``key`` that holds the current parameters.  Another
-        key destroys the handle and creates a new one, ``dfm_<family>_create(*create_args(),
-        &handle)``, with a fresh ``_ParamSync``.  ``batch``, for the families with
-        ``set_num_images``: another batch size alone keeps the handle and its uploads."""
-        L = capi.lib()
-        fn = f'dfm_{self._family}'
+    def _create(self, key, create_args, device=None):
+        """Keeps the handle when it was built for ``key``.  Otherwise destroys it and creates
+        ``dfm_<family>_create(*create_args(), &handle)`` on ``device`` (None: the current device);
+        returns True then."""
         if self._handle is not None and key == self._key:
-            if batch is not None and batch != self._batch:
-                capi.check(getattr(L, fn + '_set_num_images')(self._handle, batch),
-                           fn + '_set_num_images')
-                self._batch = batch
-        else:
-            self.release()
-            hd = ctypes.c_void_p()
-            capi.check(getattr(L, fn + '_create')(*create_args(), ctypes.byref(hd)),
-                       fn + '_create')
-            self._handle, self._key, self._batch = hd, key, batch
-            self._sync = _ParamSync()
-        set_param = getattr(L, fn + '_set_param')
-        self._sync.sync(self, lambda k, p, n: capi.check(set_param(self._handle, k, p, n),
-                                                         f'{fn}_set_param({k.decode()})'))
-        return L
+            return False
+        self.release()
+        fn = f'dfm_{self._family}_create'
+        hd = ctypes.c_void_p()
+        with torch.cuda.device(device):
+            capi.check(getattr(capi.lib(), fn)(*create_args(), ctypes.byref(hd)), fn)
+        self._handle, self._key = hd, key
+        return True
 
     def release(self):
         if self._handle is not None:
@@ -204,6 +193,50 @@ class _HandleMirror(_CudaMirror):
         except Exception:
             pass
 
+    def workspace(self):
+        """Device bytes the handle owns."""
+        fn = f'dfm_{self._family}_workspace'
+        b = ctypes.c_longlong(0)
+        capi.check(getattr(capi.lib(), fn)(self._handle, ctypes.byref(b)), fn)
+        return b.value
+
+    def _debug(self, name, shape, dtype, device='cuda'):
+        """The tensor ``name`` of the handle's last forward, through the test hook
+        ``dfm_<family>_debug_tensor`` into a new ``shape`` tensor, which must hold exactly it."""
+        fn = f'dfm_{self._family}_debug_tensor'
+        if self._handle is None:
+            raise RuntimeError(f'{fn}: no forward has run')
+        out = torch.empty(shape, device=device, dtype=dtype)
+        capi.check(getattr(capi.lib(), fn)(self._handle, name.encode(), _ptr(out), out.numel(),
+                                           _stream()), f'{fn}({name})')
+        return out
+
+
+class _HandleMirror(_Handle, _CudaMirror):
+    """A mirror that owns one handle of include/dfm_b200.h (``_Handle``) and uploads its
+    parameters through ``dfm_<family>_set_param``.  Subclasses give the key the handle is built
+    for, the create arguments and the forward."""
+    _batch = None
+
+    def _ensure(self, key, create_args, batch=None):
+        """``capi.lib()``, with a handle for ``key`` that holds the current parameters.  Another
+        key creates a new handle on the current device with a fresh ``_ParamSync``.  ``batch``,
+        for the families with ``set_num_images``: another batch size alone keeps the handle and
+        its uploads."""
+        L = capi.lib()
+        fn = f'dfm_{self._family}'
+        if self._create(key, create_args):
+            self._batch = batch
+            self._sync = _ParamSync()
+        elif batch is not None and batch != self._batch:
+            capi.check(getattr(L, fn + '_set_num_images')(self._handle, batch),
+                       fn + '_set_num_images')
+            self._batch = batch
+        set_param = getattr(L, fn + '_set_param')
+        self._sync.sync(self, lambda k, p, n: capi.check(set_param(self._handle, k, p, n),
+                                                         f'{fn}_set_param({k.decode()})'))
+        return L
+
     def init_weights(self):
         pass
 
@@ -211,13 +244,7 @@ class _HandleMirror(_CudaMirror):
         """Channels-last copy of the intermediate ``name`` the handle's last forward wrote, through
         the test hook ``dfm_<family>_debug_tensor`` (shape must hold exactly that tensor; tests
         only).  The class docstring lists the names."""
-        fn = f'dfm_{self._family}_debug_tensor'
-        if self._handle is None:
-            raise RuntimeError(f'{fn}: no forward has run')
-        out = torch.empty(shape, device='cuda', dtype=torch.float32)
-        capi.check(getattr(capi.lib(), fn)(self._handle, name.encode(), _ptr(out), out.numel(),
-                                           _stream()), f'{fn}({name})')
-        return out
+        return self._debug(name, shape, torch.float32)
 
 
 class _ConvGN(nn.Module):
@@ -468,85 +495,67 @@ def conv3d(x, weight, stride=(1, 1, 1), padding=(1, 1, 1), transposed=False,
 _DEPTH_LOSS_TYPES = ('ce', 'balanced_ce', 'focal', 'balanced_focal')
 
 
-class _DepthLossFn(torch.autograd.Function):
-    """The loss of one ``dfm_depth_loss_forward``.  Forward stores the gradient of the unweighted
-    loss sum when the volume requires grad; backward scales it by loss_weight^2 / count and
-    ``grad_output`` on the device."""
+class _LossFn(torch.autograd.Function):
+    """The loss values ``[K]`` of one device pass of a loss runner over ``inputs``.
+    ``runner.terms`` lists (input, loss) pairs; forward allocates a gradient buffer for each pair
+    whose input requires grad, and ``runner.forward(*inputs, *buffers)`` fills each with the
+    gradient of that loss's sum and returns ``(losses, scales)``.  Backward gives each input the
+    sum of its buffers, each times its loss's scale and ``grad_output`` (scales None: 1)."""
 
     @staticmethod
-    def forward(ctx, vol, loss, samples, depth, fg, empty):
-        g = torch.empty_like(vol) if ctx.needs_input_grad[0] else None
-        out, scale = loss.forward(vol, samples, depth, fg, empty, g)
-        ctx.grad = g
-        ctx.save_for_backward(scale)
-        return out
+    def forward(ctx, runner, *inputs):
+        need = ctx.needs_input_grad[1:]
+        ctx.terms = runner.terms
+        ctx.grads = [torch.empty_like(inputs[i]) if need[i] else None for i, _ in ctx.terms]
+        losses, scales = runner.forward(*inputs, *ctx.grads)
+        ctx.save_for_backward(scales)
+        return losses
 
     @staticmethod
     def backward(ctx, go):
-        scale, = ctx.saved_tensors
-        g = ctx.grad * (scale * go) if ctx.grad is not None else None
-        return g, None, None, None, None, None
+        scales, = ctx.saved_tensors
+        s = go if scales is None else scales * go
+        out = [None] * len(ctx.needs_input_grad)
+        for (i, k), g in zip(ctx.terms, ctx.grads):
+            if g is not None:
+                out[1 + i] = g * s[k] if out[1 + i] is None else out[1 + i] + g * s[k]
+        return tuple(out)
 
 
-class _DepthLoss:
+class _DepthLoss(_Handle):
     """``DepthHead.loss`` through ``dfm_depth_loss_*``: one handle per (input form, shape,
-    loss config, device), kept until the key changes."""
+    loss config, device), kept until the key changes.  The gradient it stores is that of the
+    unweighted loss sum; its scale is loss_weight^2 / count."""
+    _family = 'depth_loss'
+    terms = ((0, 0),)
+    pixels = 0
 
-    def __init__(self):
-        self.handle, self.key = None, None
+    def run(self, desc, dev, vol, samples, depth, fg, empty):
+        """The 0-dim loss of ``vol`` for ``capi.DepthLossDesc(*desc)``."""
+        self._create(desc + (str(dev),), lambda: (ctypes.byref(capi.DepthLossDesc(*desc)),), dev)
+        n, _, h, w, f = desc[:5]
+        self.pixels = n * (h * f) * (w * f)
+        self.args = (samples, depth, fg, empty)
+        return _LossFn.apply(self, vol).reshape(())
 
-    def release(self):
-        if self.handle is not None:
-            capi.lib().dfm_depth_loss_destroy(self.handle)
-            self.handle = None
-
-    def __del__(self):
-        try:
-            self.release()
-        except Exception:
-            pass
-
-    def ensure(self, key, desc, dev):
-        if self.handle is None or key != self.key:
-            self.release()
-            hd = ctypes.c_void_p()
-            with torch.cuda.device(dev):
-                capi.check(capi.lib().dfm_depth_loss_create(ctypes.byref(desc), ctypes.byref(hd)),
-                           'dfm_depth_loss_create')
-            self.handle, self.key = hd, key
-            self.pixels = desc.num_images * (desc.height * desc.factor) * \
-                (desc.width * desc.factor)
-
-    def forward(self, vol, samples, depth, fg, empty, grad):
-        """Runs the handle; returns the 0-dim loss and gradient scale."""
+    def forward(self, vol, grad):
+        """Runs the handle; returns the loss [1] and its gradient scale [1]."""
         dev = vol.device
-        loss = torch.empty((), device=dev)
-        scale = torch.empty((), device=dev)
+        loss = torch.empty(1, device=dev)
+        scale = torch.empty(1, device=dev)
+        samples, depth, fg, empty = self.args
         with torch.cuda.device(dev):
             capi.check(capi.lib().dfm_depth_loss_forward(
-                self.handle, _ptr(vol), _ptr(samples), _ptr(depth), _ptr(fg), _ptr(empty),
+                self._handle, _ptr(vol), _ptr(samples), _ptr(depth), _ptr(fg), _ptr(empty),
                 _ptr(grad), _ptr(loss), _ptr(scale), _stream()), 'dfm_depth_loss_forward')
         return loss, scale
-
-    def workspace(self):
-        """Device bytes the handle owns."""
-        b = ctypes.c_longlong(0)
-        capi.check(capi.lib().dfm_depth_loss_workspace(self.handle, ctypes.byref(b)),
-                   'dfm_depth_loss_workspace')
-        return b.value
 
     def debug_tensor(self, name):
         """From the last call (tests only): 'pixel_loss' fp32 [B*N, fH, fW], the weighted
         per-pixel term (0 outside the mask); 'count' int32 [1], the masked pixels."""
-        if self.handle is None:
-            raise RuntimeError('dfm_depth_loss_debug_tensor: no loss call has run')
-        n = 1 if name == 'count' else self.pixels
-        out = torch.empty(n, device='cuda',
-                          dtype=torch.int32 if name == 'count' else torch.float32)
-        capi.check(capi.lib().dfm_depth_loss_debug_tensor(self.handle, name.encode(), _ptr(out),
-                                                          out.numel(), _stream()),
-                   f'dfm_depth_loss_debug_tensor({name})')
-        return out
+        if name == 'count':
+            return self._debug(name, 1, torch.int32)
+        return self._debug(name, self.pixels, torch.float32)
 
 
 @HEADS.register_module()
@@ -686,10 +695,9 @@ class DepthHead(_CudaMirror):
         fgw, bgw = (float(cfg['fg_weight']), float(cfg['bg_weight'])) if balanced else (1.0, 1.0)
         desc = (n, d, h, w, f, int(not logits), float(self.min_depth), float(self.max_depth),
                 alpha, gamma, fgw, bgw, int(balanced), float(self.loss_weight))
-        self._depth_loss.ensure(desc + (str(dev),), capi.DepthLossDesc(*desc), dev)
         empty = (depth_preds.detach().mean() * 0.0).to(dev, torch.float32)
-        return _DepthLossFn.apply(vol.contiguous(), self._depth_loss, samples,
-                                  depth_img.contiguous(), fg, empty)
+        return self._depth_loss.run(desc, dev, vol.contiguous(), samples, depth_img.contiguous(),
+                                    fg, empty)
 
 
 class _NeckBase(_HandleMirror):
@@ -1280,23 +1288,19 @@ def grid_anchors(anchor_generator, ny, nx, device):
     return torch.cat(per_range, dim=2).reshape(-1, 7)
 
 
-class _BoxPost:
+def _host_anchors(head, ny, nx, dev):
+    """``grid_anchors`` of the head's anchor generator, computed on ``dev``, as a host array
+    ``[N, 7]``.  Its ``.ctypes.data_as(c_void_p)`` pointer keeps it alive through a create call."""
+    with torch.cuda.device(dev):
+        anchors = grid_anchors(head.extra_cfg['anchor_generator'], ny, nx, dev)
+    return anchors.cpu().contiguous().numpy()
+
+
+class _BoxPost(_Handle):
     """``get_bboxes`` of both anchor heads through ``dfm_box_post_*``: one handle and anchor
     table per (feature map size, batch, device, test_cfg), kept until the key changes."""
-
-    def __init__(self):
-        self.handle, self.key = None, None
-
-    def release(self):
-        if self.handle is not None:
-            capi.lib().dfm_box_post_destroy(self.handle)
-            self.handle = None
-
-    def __del__(self):
-        try:
-            self.release()
-        except Exception:
-            pass
+    _family = 'box_post'
+    batch = k = 0
 
     def run(self, head, cls_scores, bbox_preds, dir_cls_preds, input_metas, cfg, num_classes,
             use_sigmoid, dir_offset, dir_limit_offset):
@@ -1328,32 +1332,27 @@ class _BoxPost:
         desc_args = (num_classes, A, ny, nx, B, int(use_sigmoid), int(cfg.get('nms_pre', -1)),
                      max_num, float(cfg.get('score_thr', 0)), float(cfg['nms_thr']),
                      float(dir_offset), float(dir_limit_offset))
-        key = desc_args + (str(cls.device),)
-        L = capi.lib()
-        if self.handle is None or key != self.key:
-            self.release()
-            with torch.cuda.device(cls.device):
-                anchors = grid_anchors(head.extra_cfg['anchor_generator'], ny, nx, cls.device)
-            anchors = anchors.cpu().contiguous()
+        dev = cls.device
+
+        def create_args():
+            anchors = _host_anchors(head, ny, nx, dev)
             if anchors.shape[0] != ny * nx * A:
                 raise RuntimeError(f'anchor generator gives {anchors.shape[0] // (ny * nx)} '
                                    f'anchors per cell, the head has {A}')
-            hd = ctypes.c_void_p()
-            capi.check(L.dfm_box_post_create(ctypes.byref(capi.BoxPostDesc(*desc_args)),
-                                             _ptr(anchors), ctypes.byref(hd)),
-                       'dfm_box_post_create')
-            self.handle, self.key = hd, key
-            n, nms_pre = ny * nx * A, desc_args[6]
-            self.batch, self.k = B, nms_pre if 0 < nms_pre < n else n
-        dev = cls.device
+            return (ctypes.byref(capi.BoxPostDesc(*desc_args)),
+                    anchors.ctypes.data_as(ctypes.c_void_p))
+
+        self._create(desc_args + (str(dev),), create_args, dev)
+        n, nms_pre = ny * nx * A, desc_args[6]
+        self.batch, self.k = B, nms_pre if 0 < nms_pre < n else n
         boxes = torch.empty((B, max_num, 7), device=dev)
         scores = torch.empty((B, max_num), device=dev)
         labels = torch.empty((B, max_num), device=dev, dtype=torch.int32)
         count = torch.empty((B,), device=dev, dtype=torch.int32)
         with torch.cuda.device(dev):
-            capi.check(L.dfm_box_post_forward(self.handle, _ptr(cls), _ptr(box), _ptr(dirc),
-                                              _ptr(boxes), _ptr(scores), _ptr(labels),
-                                              _ptr(count), _stream()), 'dfm_box_post_forward')
+            capi.check(capi.lib().dfm_box_post_forward(
+                self._handle, _ptr(cls), _ptr(box), _ptr(dirc), _ptr(boxes), _ptr(scores),
+                _ptr(labels), _ptr(count), _stream()), 'dfm_box_post_forward')
         counts = count.cpu().tolist()
         out = []
         for b, meta in enumerate(input_metas):
@@ -1367,13 +1366,34 @@ class _BoxPost:
     def debug_tensor(self, name):
         """int32 ``[batch, K]`` stage output of the last call (tests only): 'topk_index',
         'cls<c>_candidates', 'cls<c>_keep'; -1 past each sample's count."""
-        if self.handle is None:
-            raise RuntimeError('dfm_box_post_debug_tensor: no get_bboxes call has run')
-        out = torch.empty((self.batch, self.k), device='cuda', dtype=torch.int32)
-        capi.check(capi.lib().dfm_box_post_debug_tensor(self.handle, name.encode(), _ptr(out),
-                                                         out.numel(), _stream()),
-                   f'dfm_box_post_debug_tensor({name})')
-        return out
+        return self._debug(name, (self.batch, self.k), torch.int32)
+
+
+def _pack_gt(gt_bboxes, dev, boxes_of, gt_labels=None, num_classes=0, where='', each='sample'):
+    """One loss call's GT, concatenated over the samples on ``dev``: ``(gt [G, K] fp32, labels [G]
+    int32 or None, host offsets [B + 1] c_int array, device offsets [B + 1] int32)``.
+    ``boxes_of`` gives the ``[M, K]`` boxes of one sample's entry (a tensor, or an object with
+    ``.tensor``) or raises on a wrong shape.  ``where`` / ``each`` name the caller and its
+    samples in the label errors."""
+    boxes, labels, off = [], [], [0]
+    for i, gb in enumerate(gt_bboxes):
+        gb = boxes_of(gb.tensor if hasattr(gb, 'tensor') else gb)
+        if gt_labels is not None:
+            gl = gt_labels[i]
+            if gl.shape != (gb.shape[0],):
+                raise RuntimeError(f'{where}: every {each} needs one label per GT box')
+            # labels still on the host are checked here; on the device the kernels flag them
+            # and every loss comes out NaN (no host synchronisation on the CUDA path)
+            if not gl.is_cuda and gl.numel() and \
+                    (int(gl.min()) < 0 or int(gl.max()) >= num_classes):
+                raise ValueError(f'{where}: GT labels must lie in 0..{num_classes - 1}')
+            labels.append(gl.to(dev, torch.int32))
+        boxes.append(gb.to(dev, torch.float32))
+        off.append(off[-1] + gb.shape[0])
+    return (torch.cat(boxes).contiguous(),
+            torch.cat(labels).contiguous() if gt_labels is not None else None,
+            (ctypes.c_int * len(off))(*off),
+            torch.tensor(off, dtype=torch.int32).to(dev, non_blocking=True))
 
 
 def _dist_reduce_mean(t):
@@ -1444,52 +1464,13 @@ def _loss_config(head, liga):
         reduce_avg_factor=bool(getattr(head, 'reduce_avg_factor', False)) and liga)
 
 
-class _AnchorLossFn(torch.autograd.Function):
-    """The four loss values of one ``dfm_anchor_loss_forward`` / ``_finish``.  Forward stores the
-    gradients of the loss sums of the inputs that require grad; backward scales each by its
-    loss's normaliser, weight and ``grad_output``."""
-
-    @staticmethod
-    def forward(ctx, cls, box, dirc, loss):
-        need = ctx.needs_input_grad
-        g_cls = torch.empty_like(cls) if need[0] else None
-        g_box = torch.empty_like(box) if need[1] else None
-        g_dir = torch.empty_like(dirc) if need[2] else None
-        g_iou = torch.empty_like(box) if need[1] and loss.cfg['with_iou'] else None
-        scales = loss.forward(cls, box, dirc, g_cls, g_box, g_dir, g_iou)
-        ctx.grads = (g_cls, g_box, g_dir, g_iou)
-        ctx.save_for_backward(scales)
-        return loss.losses
-
-    @staticmethod
-    def backward(ctx, g):
-        scales, = ctx.saved_tensors
-        s = scales * g
-        g_cls, g_box, g_dir, g_iou = ctx.grads
-        gb = g_box * s[1] if g_box is not None else None
-        if g_iou is not None:
-            gb = gb + g_iou * s[3]
-        return (g_cls * s[0] if g_cls is not None else None, gb,
-                g_dir * s[2] if g_dir is not None else None, None)
-
-
-class _AnchorLoss:
+class _AnchorLoss(_Handle):
     """``loss`` of both anchor heads through ``dfm_anchor_loss_*``: one handle and anchor table per
-    (feature map size, batch, device, loss config), kept until the key changes."""
-
-    def __init__(self):
-        self.handle, self.key = None, None
-
-    def release(self):
-        if self.handle is not None:
-            capi.lib().dfm_anchor_loss_destroy(self.handle)
-            self.handle = None
-
-    def __del__(self):
-        try:
-            self.release()
-        except Exception:
-            pass
+    (feature map size, batch, device, loss config), kept until the key changes.  Losses and
+    scales are [cls, bbox, dir, iou]; ``bbox_pred`` stores a gradient for the bbox and, for
+    LIGA's IoU term, the IoU loss."""
+    _family = 'anchor_loss'
+    batch = n = 0
 
     def run(self, head, liga, cls_scores, bbox_preds, dir_cls_preds, gt_bboxes, gt_labels,
             input_metas, gt_bboxes_ignore):
@@ -1513,88 +1494,63 @@ class _AnchorLoss:
                 box.shape != (B, A * 7, ny, nx) or dirc.shape != (B, A * 2, ny, nx):
             raise RuntimeError(f'loss: unexpected head output shapes {tuple(cls.shape)}, '
                                f'{tuple(box.shape)}, {tuple(dirc.shape)}')
-        boxes, labels, off = [], [], [0]
-        for gb, gl in zip(gt_bboxes, gt_labels):
-            gb = gb.tensor if hasattr(gb, 'tensor') else gb
+        def boxes_of(gb):
             if gb.dim() != 2 or gb.shape[1] != 7:
                 raise NotImplementedError(f'loss: GT boxes must be [M, 7], got '
                                           f'{tuple(gb.shape)}')
-            if gl.shape != (gb.shape[0],):
-                raise RuntimeError('loss: every sample needs one label per GT box')
-            # labels still on the host are checked here; on the device the kernels flag them
-            # and every loss comes out NaN (no host synchronisation on the CUDA path)
-            if not gl.is_cuda and gl.numel() and (int(gl.min()) < 0 or int(gl.max()) >= C):
-                raise ValueError(f'loss: GT labels must lie in 0..{C - 1}')
-            boxes.append(gb.to(dev, torch.float32))
-            labels.append(gl.to(dev, torch.int32))
-            off.append(off[-1] + gb.shape[0])
-        self.gt = torch.cat(boxes).contiguous()
-        self.gt_labels = torch.cat(labels).contiguous()
-        self.h_off = (ctypes.c_int * (B + 1))(*off)
-        self.d_off = torch.tensor(off, dtype=torch.int32).to(dev, non_blocking=True)
-        t = cfg['thr'] + [(0.0, 0.0, 0.0)] * (8 - len(cfg['thr']))
-        desc_args = (C, cfg['num_sizes'], cfg['num_rots'], ny, nx, B,
-                     int(cfg['assign_per_class']), int(cfg['diff_rad_by_sin']), 1,
-                     int(cfg['with_iou']), int(liga),
-                     (ctypes.c_float * 8)(*[x[0] for x in t]),
-                     (ctypes.c_float * 8)(*[x[1] for x in t]),
-                     (ctypes.c_float * 8)(*[x[2] for x in t]),
-                     cfg['pos_weight'], cfg['gamma'], cfg['alpha'], cfg['beta'],
-                     (ctypes.c_float * 4)(*cfg['loss_weight']), cfg['dir_offset'],
-                     cfg['dir_limit_offset'], cfg['normalizer_clamp_value'])
+            return gb
+
+        self.gt, self.gt_labels, self.h_off, self.d_off = _pack_gt(
+            gt_bboxes, dev, boxes_of, gt_labels, C, 'loss')
+
+        def create_args():
+            t = cfg['thr'] + [(0.0, 0.0, 0.0)] * (8 - len(cfg['thr']))
+            desc = capi.AnchorLossDesc(
+                C, cfg['num_sizes'], cfg['num_rots'], ny, nx, B, int(cfg['assign_per_class']),
+                int(cfg['diff_rad_by_sin']), 1, int(cfg['with_iou']), int(liga),
+                (ctypes.c_float * 8)(*[x[0] for x in t]), (ctypes.c_float * 8)(*[x[1] for x in t]),
+                (ctypes.c_float * 8)(*[x[2] for x in t]), cfg['pos_weight'], cfg['gamma'],
+                cfg['alpha'], cfg['beta'], (ctypes.c_float * 4)(*cfg['loss_weight']),
+                cfg['dir_offset'], cfg['dir_limit_offset'], cfg['normalizer_clamp_value'])
+            return (ctypes.byref(desc),
+                    _host_anchors(head, ny, nx, dev).ctypes.data_as(ctypes.c_void_p))
+
         key = (repr(sorted((k, repr(v)) for k, v in cfg.items())), ny, nx, B, str(dev))
-        L = capi.lib()
-        if self.handle is None or key != self.key:
-            self.release()
-            with torch.cuda.device(dev):
-                anchors = grid_anchors(head.extra_cfg['anchor_generator'], ny, nx, dev)
-            self.anchors = anchors
-            anchors = anchors.cpu().contiguous()
-            hd = ctypes.c_void_p()
-            with torch.cuda.device(dev):
-                capi.check(L.dfm_anchor_loss_create(ctypes.byref(capi.AnchorLossDesc(*desc_args)),
-                                                    _ptr(anchors), ctypes.byref(hd)),
-                           'dfm_anchor_loss_create')
-            self.handle, self.key, self.batch, self.n = hd, key, B, ny * nx * A
-        self.cfg = cfg
-        losses = _AnchorLossFn.apply(cls.contiguous(), box.contiguous(), dirc.contiguous(), self)
+        self._create(key, create_args, dev)
+        self.batch, self.n, self.cfg = B, ny * nx * A, cfg
+        self.terms = ((0, 0), (1, 1), (2, 2)) + (((1, 3),) if cfg['with_iou'] else ())
+        losses = _LossFn.apply(self, cls.contiguous(), box.contiguous(), dirc.contiguous())
         out = dict(loss_cls=[losses[0]], loss_bbox=[losses[1]], loss_dir=[losses[2]])
         if cfg['with_iou']:
             out['loss_iou'] = [losses[3]]
         return out
 
-    def forward(self, cls, box, dirc, g_cls, g_box, g_dir, g_iou):
-        """Runs the handle; sets ``self.losses`` [4] and returns the gradient scales [4]."""
+    def forward(self, cls, box, dirc, g_cls, g_box, g_dir, g_iou=None):
+        """Runs the handle; returns the losses [4] and the gradient scales [4]."""
         L = capi.lib()
         dev = cls.device
         norm = torch.empty(1, device=dev)
         with torch.cuda.device(dev):
             capi.check(L.dfm_anchor_loss_forward(
-                self.handle, _ptr(cls), _ptr(box), _ptr(dirc), _ptr(self.gt),
+                self._handle, _ptr(cls), _ptr(box), _ptr(dirc), _ptr(self.gt),
                 _ptr(self.gt_labels), _ptr(self.d_off), ctypes.cast(self.h_off, ctypes.c_void_p),
                 _ptr(g_cls), _ptr(g_box), _ptr(g_dir), _ptr(g_iou), _ptr(norm), _stream()),
                 'dfm_anchor_loss_forward')
             avg = _dist_reduce_mean(norm) if self.cfg['reduce_avg_factor'] else norm
-            self.losses = torch.empty(4, device=dev)
+            losses = torch.empty(4, device=dev)
             scales = torch.empty(4, device=dev)
-            capi.check(L.dfm_anchor_loss_finish(self.handle, _ptr(avg), _ptr(self.losses),
+            capi.check(L.dfm_anchor_loss_finish(self._handle, _ptr(avg), _ptr(losses),
                                                 _ptr(scales), _stream()),
                        'dfm_anchor_loss_finish')
-        return scales
+        return losses, scales
 
     def debug_tensor(self, name):
         """Per-anchor target of the last call (tests only): 'assigned_gt', 'labels',
         'dir_targets' int32 [batch, N]; 'label_weights' fp32 [batch, N]; 'bbox_targets' fp32
         [batch, N, 7]."""
-        if self.handle is None:
-            raise RuntimeError('dfm_anchor_loss_debug_tensor: no loss call has run')
         shape = (self.batch, self.n) + ((7,) if name == 'bbox_targets' else ())
         dt = torch.float32 if name in ('label_weights', 'bbox_targets') else torch.int32
-        out = torch.empty(shape, device='cuda', dtype=dt)
-        capi.check(capi.lib().dfm_anchor_loss_debug_tensor(self.handle, name.encode(), _ptr(out),
-                                                           out.numel(), _stream()),
-                   f'dfm_anchor_loss_debug_tensor({name})')
-        return out
+        return self._debug(name, shape, dt)
 
 
 _LOSS_DOC = """Training loss (``anchor3d_head.py:328-406`` with ``loss_single``{liga}) on CUDA
@@ -1869,45 +1825,12 @@ def _ptr_table(ts):
     return arr, ctypes.cast(arr, ctypes.c_void_p)
 
 
-class _ATSSLossFn(torch.autograd.Function):
-    """The 3 x L loss values of one ``dfm_atss_loss_forward`` / ``_finish``.  Forward stores the
-    gradients of the per-level loss sums of the outputs that require grad; backward scales each
-    by its loss's normaliser, weight and ``grad_output``."""
-
-    @staticmethod
-    def forward(ctx, loss, *outs):
-        grads = [torch.empty_like(o) if ctx.needs_input_grad[1 + i] else None
-                 for i, o in enumerate(outs)]
-        scales = loss.forward(outs, grads)
-        ctx.grads = grads
-        ctx.save_for_backward(scales)
-        return loss.losses
-
-    @staticmethod
-    def backward(ctx, g):
-        scales, = ctx.saved_tensors
-        s = scales * g
-        return (None,) + tuple(gr * s[i] if gr is not None else None
-                               for i, gr in enumerate(ctx.grads))
-
-
-class _ATSSLoss:
+class _ATSSLoss(_Handle):
     """``LIGAATSSHead.loss`` through ``dfm_atss_loss_*``: one handle per (feature sizes, batch,
-    device, loss config), kept until the key changes."""
-
-    def __init__(self):
-        self.handle, self.key = None, None
-
-    def release(self):
-        if self.handle is not None:
-            capi.lib().dfm_atss_loss_destroy(self.handle)
-            self.handle = None
-
-    def __del__(self):
-        try:
-            self.release()
-        except Exception:
-            pass
+    device, loss config), kept until the key changes.  Losses and scales are 3 x L, in the
+    order of the head outputs (cls, bbox, centerness per level)."""
+    _family = 'atss_loss'
+    batch = n = 0
 
     def run(self, head, cls_scores, bbox_preds, centernesses, gt_bboxes, gt_labels, img_metas,
             gt_bboxes_ignore):
@@ -1933,52 +1856,41 @@ class _ATSSLoss:
                                    f'{lv}: {tuple(c.shape)}, {tuple(b.shape)}, {tuple(z.shape)}')
             feat.append((int(h), int(w)))
         dev = cls_scores[0].device
-        boxes, labels, off = [], [], [0]
-        for gb, gl in zip(gt_bboxes, gt_labels):
+        def boxes_of(gb):
             if gb.dim() != 2 or gb.shape[1] != 6:
                 raise RuntimeError(f'LIGAATSSHead.loss: GT must be [M, 6] (2-D box and projected '
                                    f'3-D centre), got {tuple(gb.shape)}')
-            if gl.shape != (gb.shape[0],):
-                raise RuntimeError('LIGAATSSHead.loss: every image needs one label per GT box')
-            # labels still on the host are checked here; on the device the kernels flag them
-            # and every loss comes out NaN (no host synchronisation on the CUDA path)
-            if not gl.is_cuda and gl.numel() and (int(gl.min()) < 0 or int(gl.max()) >= C):
-                raise ValueError(f'LIGAATSSHead.loss: GT labels must lie in 0..{C - 1}')
-            boxes.append(gb.to(dev, torch.float32))
-            labels.append(gl.to(dev, torch.int32))
-            off.append(off[-1] + gb.shape[0])
-        self.gt = torch.cat(boxes).contiguous()
-        self.gt_labels = torch.cat(labels).contiguous()
-        self.h_off = (ctypes.c_int * (B + 1))(*off)
-        self.d_off = torch.tensor(off, dtype=torch.int32).to(dev, non_blocking=True)
+            return gb
+
+        self.gt, self.gt_labels, self.h_off, self.d_off = _pack_gt(
+            gt_bboxes, dev, boxes_of, gt_labels, C, 'LIGAATSSHead.loss', 'image')
         pads = [int(v) for m in img_metas for v in m['pad_shape'][:2]]
         self.h_pad = (ctypes.c_int * (2 * B))(*pads)
-        key = (repr(sorted((k, repr(v)) for k, v in cfg.items())), tuple(feat), B, str(dev))
-        if self.handle is None or key != self.key:
-            self.release()
+
+        def create_args():
             z8 = lambda v: (ctypes.c_int * 8)(*v)  # noqa: E731
-            desc = capi.AtssLossDesc(
+            return (ctypes.byref(capi.AtssLossDesc(
                 C, L, z8(cfg['strides']), z8([f[0] for f in feat]), z8([f[1] for f in feat]), B,
                 9, cfg['octave_base_scale'], (ctypes.c_float * 4)(*cfg['target_stds']),
                 cfg['wh_ratio_clip'], cfg['giou_eps'], cfg['gamma'], cfg['alpha'],
-                (ctypes.c_float * 3)(*cfg['loss_weight']))
-            hd = ctypes.c_void_p()
-            with torch.cuda.device(dev):
-                capi.check(capi.lib().dfm_atss_loss_create(ctypes.byref(desc), ctypes.byref(hd)),
-                           'dfm_atss_loss_create')
-            self.handle, self.key, self.batch = hd, key, B
-            self.n = sum(h * w for h, w in feat)
-        self.levels = L
+                (ctypes.c_float * 3)(*cfg['loss_weight']))),)
+
+        key = (repr(sorted((k, repr(v)) for k, v in cfg.items())), tuple(feat), B, str(dev))
+        self._create(key, create_args, dev)
+        self.batch, self.n, self.levels = B, sum(h * w for h, w in feat), L
+        self.terms = tuple((i, i) for i in range(3 * L))
         outs = [t.contiguous() for t in (*cls_scores, *bbox_preds, *centernesses)]
-        losses = _ATSSLossFn.apply(self, *outs)
+        losses = _LossFn.apply(self, *outs)
         return dict(loss_cls=[losses[i] for i in range(L)],
                     loss_bbox=[losses[L + i] for i in range(L)],
                     loss_centerness=[losses[2 * L + i] for i in range(L)])
 
-    def forward(self, outs, grads):
-        """Runs the handle; sets ``self.losses`` [3 L] and returns the gradient scales [3 L]."""
+    def forward(self, *tensors):
+        """Runs the handle on the 3 L head outputs and their 3 L gradient buffers (or None);
+        returns the losses [3 L] and the gradient scales [3 L]."""
         L = self.levels
         lib = capi.lib()
+        outs, grads = tensors[:3 * L], tensors[3 * L:]
         dev = outs[0].device
         tabs = [_ptr_table(outs[k * L:(k + 1) * L]) for k in range(3)]
         gtabs = [_ptr_table(grads[k * L:(k + 1) * L])
@@ -1987,33 +1899,27 @@ class _ATSSLoss:
         norm = torch.empty(2, device=dev)
         with torch.cuda.device(dev):
             capi.check(lib.dfm_atss_loss_forward(
-                self.handle, tabs[0][1], tabs[1][1], tabs[2][1], _ptr(self.gt),
+                self._handle, tabs[0][1], tabs[1][1], tabs[2][1], _ptr(self.gt),
                 _ptr(self.gt_labels), _ptr(self.d_off), ctypes.cast(self.h_off, ctypes.c_void_p),
                 ctypes.cast(self.h_pad, ctypes.c_void_p), gtabs[0][1], gtabs[1][1], gtabs[2][1],
                 _ptr(norm), _stream()), 'dfm_atss_loss_forward')
             # num_total_pos and the centerness sum, all-reduced in one call
             avg = _dist_reduce_mean(norm)
-            self.losses = torch.empty(3 * L, device=dev)
+            losses = torch.empty(3 * L, device=dev)
             scales = torch.empty(3 * L, device=dev)
-            capi.check(lib.dfm_atss_loss_finish(self.handle, _ptr(avg), _ptr(self.losses),
+            capi.check(lib.dfm_atss_loss_finish(self._handle, _ptr(avg), _ptr(losses),
                                                 _ptr(scales), _stream()),
                        'dfm_atss_loss_finish')
-        return scales
+        return losses, scales
 
     def debug_tensor(self, name):
         """Per-anchor target of the last call (tests only): 'assigned_gt', 'labels' int32
         [batch, N]; 'label_weights', 'centerness_targets' fp32 [batch, N]; 'bbox_targets' fp32
         [batch, N, 4]; 'thresholds' fp32 [G]."""
-        if self.handle is None:
-            raise RuntimeError('dfm_atss_loss_debug_tensor: no loss call has run')
         shape = {'bbox_targets': (self.batch, self.n, 4),
                  'thresholds': (self.gt.shape[0],)}.get(name, (self.batch, self.n))
         dt = torch.int32 if name in ('assigned_gt', 'labels') else torch.float32
-        out = torch.empty(shape, device=self.gt.device, dtype=dt)
-        capi.check(capi.lib().dfm_atss_loss_debug_tensor(self.handle, name.encode(), _ptr(out),
-                                                         out.numel(), _stream()),
-                   f'dfm_atss_loss_debug_tensor({name})')
-        return out
+        return self._debug(name, shape, dt, self.gt.device)
 
 
 class _Scale(nn.Module):
@@ -2142,50 +2048,13 @@ class LIGAATSSHead(nn.Module):
                                    gt_labels, img_metas, gt_bboxes_ignore)
 
 
-class _ImitationLossFn(torch.autograd.Function):
-    """The per-pair losses of one ``dfm_imitation_loss_forward`` / ``_finish``.  When an input
-    requires grad, forward also runs ``dfm_imitation_loss_backward`` (grad_output 1) while the
-    handle's workspace still holds this call's mask; backward scales each stored gradient by its
-    loss's ``grad_output``."""
-
-    @staticmethod
-    def forward(ctx, run, *tensors):
-        P = len(run.pairs)
-        need = ctx.needs_input_grad[1:]
-        xs, ws, bs = tensors[:P], tensors[P:2 * P], tensors[2 * P:]
-        gx = [torch.empty_like(x) if need[i] else None for i, x in enumerate(xs)]
-        gw = [torch.empty_like(w) if need[P + i] else None for i, w in enumerate(ws)]
-        gb = [torch.empty_like(b) if need[2 * P + i] else None for i, b in enumerate(bs)]
-        losses, coef = run.forward(xs, ws, bs)
-        if any(need):
-            run.backward(coef, gx, gw, gb)
-        ctx.grads = gx + gw + gb
-        return losses
-
-    @staticmethod
-    def backward(ctx, go):
-        P = len(ctx.grads) // 3
-        return (None,) + tuple(g * go[i % P] if g is not None else None
-                               for i, g in enumerate(ctx.grads))
-
-
-class _ImitationLoss:
+class _ImitationLoss(_Handle):
     """``DfMImitation.loss`` through ``dfm_imitation_loss_*``: one handle per (shape, batch,
-    config, device), kept until the key changes."""
-
-    def __init__(self):
-        self.handle, self.key, self.anchors = None, None, None
-
-    def release(self):
-        if self.handle is not None:
-            capi.lib().dfm_imitation_loss_destroy(self.handle)
-            self.handle = None
-
-    def __del__(self):
-        try:
-            self.release()
-        except Exception:
-            pass
+    config, device), kept until the key changes.  When an input requires grad, the device pass
+    also runs ``dfm_imitation_loss_backward`` (grad_output 1) while the handle's workspace still
+    holds this call's mask, so each stored gradient takes only its loss's ``grad_output``."""
+    _family = 'imitation_loss'
+    anchors = None
 
     def anchor_xy(self, anchor_generator, ny, nx, dev):
         """The BEV cells' anchor centres ``[nx + ny]`` (x per column, then y per row): columns 0
@@ -2204,55 +2073,51 @@ class _ImitationLoss:
         dev = xs[0].device
         if len(gt_bboxes_3d) != B:
             raise RuntimeError(f'DfMImitation.loss: {B} samples, {len(gt_bboxes_3d)} gt_bboxes_3d')
-        boxes, off = [], [0]
-        for gb in gt_bboxes_3d:
-            gb = gb.tensor if hasattr(gb, 'tensor') else gb
+        def boxes_of(gb):
             if not isinstance(gb, torch.Tensor) or gb.dim() != 2 or gb.shape[1] < 7:
                 raise RuntimeError('DfMImitation.loss: GT boxes must be [M, 7] per sample, got '
                                    f'{tuple(gb.shape) if isinstance(gb, torch.Tensor) else gb}')
-            boxes.append(gb[:, :7].to(dev, torch.float32))
-            off.append(off[-1] + gb.shape[0])
-        self.gt = torch.cat(boxes).contiguous()
-        self.h_off = (ctypes.c_int * (B + 1))(*off)
-        self.d_off = torch.tensor(off, dtype=torch.int32).to(dev, non_blocking=True)
+            return gb[:, :7]
+
+        self.gt, _, self.h_off, self.d_off = _pack_gt(gt_bboxes_3d, dev, boxes_of)
         self.anchor = self.anchor_xy(mod.anchor_generator, ny, nx, dev)
         self.pairs = [(x.shape[1], x.shape[2] if x.dim() == 5 else 1) for x in xs]
         lw = [float(c['loss_weight']) for c in mod.imitation_cfgs]
         P = len(self.pairs)
         desc = (B, ny, nx, P, tuple(c for c, _ in self.pairs), tuple(z for _, z in self.pairs),
                 tuple(lw), float(mod.normalizer_clamp_value))
-        key = desc + (str(dev),)
-        if self.handle is None or key != self.key:
-            self.release()
+
+        def create_args():
             pad = lambda v: v + (0,) * (2 - len(v))  # noqa: E731
-            d = capi.ImitationLossDesc(B, ny, nx, P, (ctypes.c_int * 2)(*pad(desc[4])),
-                                       (ctypes.c_int * 2)(*pad(desc[5])),
-                                       (ctypes.c_float * 2)(*pad(desc[6])), desc[7])
-            hd = ctypes.c_void_p()
-            with torch.cuda.device(dev):
-                capi.check(capi.lib().dfm_imitation_loss_create(ctypes.byref(d), ctypes.byref(hd)),
-                           'dfm_imitation_loss_create')
-            self.handle, self.key = hd, key
+            return (ctypes.byref(capi.ImitationLossDesc(
+                B, ny, nx, P, (ctypes.c_int * 2)(*pad(desc[4])), (ctypes.c_int * 2)(*pad(desc[5])),
+                (ctypes.c_float * 2)(*pad(desc[6])), desc[7])),)
+
+        self._create(desc + (str(dev),), create_args, dev)
         self.ts, self.scales, self.training = ts, scales, mod.training
+        self.terms = tuple((i, i % P) for i in range(3 * P))
         ws = [c.weight for c in mod._convs()]
         bs = [c.bias for c in mod._convs()]
-        losses = _ImitationLossFn.apply(self, *xs, *ws, *bs)
+        losses = _LossFn.apply(self, *xs, *ws, *bs)
         return [losses[i] for i in range(P)]
 
-    def forward(self, xs, ws, bs):
-        """Runs forward, the all-reduce of the packed counts and sums, and finish; returns the
-        losses [P] and the gradient coefficients [P]."""
+    def forward(self, *tensors):
+        """Runs forward, the all-reduce of the packed counts and sums, and finish on the P stereo
+        features, weights and biases, then backward into their gradient buffers (or None) when
+        one is given; returns the losses [P] and None, the gradients' scale 1."""
         import torch.distributed as dist
         lib = capi.lib()
+        P = len(self.pairs)
+        xs, ws, bs = tensors[:P], tensors[P:2 * P], tensors[2 * P:3 * P]
+        grads = tensors[3 * P:]
         dev = xs[0].device
-        P = len(xs)
         tabs = [_ptr_table(v) for v in (xs, self.ts, ws, bs, self.scales)]
         packed = torch.empty(sum(2 + c for c, _ in self.pairs), device=dev)
         ranks = dist.is_available() and dist.is_initialized()
         world = dist.get_world_size() if ranks else 1
         with torch.cuda.device(dev):
             capi.check(lib.dfm_imitation_loss_forward(
-                self.handle, tabs[0][1], tabs[1][1], tabs[2][1], tabs[3][1], tabs[4][1],
+                self._handle, tabs[0][1], tabs[1][1], tabs[2][1], tabs[3][1], tabs[4][1],
                 _ptr(self.anchor), _ptr(self.gt) if self.gt.numel() else None, _ptr(self.d_off),
                 ctypes.cast(self.h_off, ctypes.c_void_p), world, _ptr(packed), _stream()),
                 'dfm_imitation_loss_forward')
@@ -2261,42 +2126,27 @@ class _ImitationLoss:
                 dist.all_reduce(packed)
             losses = torch.empty(P, device=dev)
             coef = torch.empty(P, device=dev)
-            capi.check(lib.dfm_imitation_loss_finish(self.handle, _ptr(packed),
+            capi.check(lib.dfm_imitation_loss_finish(self._handle, _ptr(packed),
                                                      int(self.training), _ptr(losses),
                                                      _ptr(coef), _stream()),
                        'dfm_imitation_loss_finish')
-        return losses, coef
-
-    def backward(self, coef, gx, gw, gb):
-        tabs = [_ptr_table(v) if any(g is not None for g in v) else (None, None)
-                for v in (gx, gw, gb)]
-        with torch.cuda.device(coef.device):
-            capi.check(capi.lib().dfm_imitation_loss_backward(
-                self.handle, _ptr(coef), None, tabs[0][1], tabs[1][1], tabs[2][1], _stream()),
-                'dfm_imitation_loss_backward')
-
-    def workspace(self):
-        """Device bytes the handle owns."""
-        b = ctypes.c_longlong(0)
-        capi.check(capi.lib().dfm_imitation_loss_workspace(self.handle, ctypes.byref(b)),
-                   'dfm_imitation_loss_workspace')
-        return b.value
+            if any(g is not None for g in grads):
+                gtabs = [_ptr_table(v) if any(g is not None for g in v) else (None, None)
+                         for v in (grads[:P], grads[P:2 * P], grads[2 * P:])]
+                capi.check(lib.dfm_imitation_loss_backward(
+                    self._handle, _ptr(coef), None, gtabs[0][1], gtabs[1][1], gtabs[2][1],
+                    _stream()), 'dfm_imitation_loss_backward')
+        return losses, None
 
     def debug_tensor(self, name):
         """From the last call (tests only): 'inbox' uint8 [B, ny, nx]; 'counts' int32 [P], this
         rank's positives per pair; 'loss_sums' fp64 [P]."""
-        if self.handle is None:
-            raise RuntimeError('dfm_imitation_loss_debug_tensor: no loss call has run')
-        B, ny, nx = self.key[:3]
+        B, ny, nx = self._key[:3]
         shape, dt = {'inbox': ((B, ny, nx), torch.uint8),
                      'counts': ((len(self.pairs),), torch.int32),
                      'loss_sums': ((len(self.pairs),), torch.float64)}.get(
                          name, ((0,), torch.float32))
-        out = torch.empty(shape, device=self.gt.device, dtype=dt)
-        capi.check(capi.lib().dfm_imitation_loss_debug_tensor(self.handle, name.encode(),
-                                                              _ptr(out), out.numel(), _stream()),
-                   f'dfm_imitation_loss_debug_tensor({name})')
-        return out
+        return self._debug(name, shape, dt, self.gt.device)
 
 
 class _NormalizeLayer(nn.Module):

@@ -683,7 +683,9 @@ int dfm_box_post_forward(dfm_box_post_t* h, const float* d_cls, const float* d_b
  * "topk_index" (selected anchors by score descending, anchor index ascending; DFM_ERR_STATE
  * when the grid skipped the top-k), "cls<c>_candidates" (anchors passing score_thr for class c,
  * in NMS processing order), "cls<c>_keep" (anchors kept by class c's NMS, in order); -1 past
- * each sample's count.  DFM_ERR_INVALID on a wrong element count. */
+ * each sample's count.  An unknown name fails with DFM_ERR_INVALID, before a forward too; a
+ * known one with DFM_ERR_STATE before a forward, then a wrong element count with
+ * DFM_ERR_INVALID. */
 int dfm_box_post_debug_tensor(dfm_box_post_t* h, const char* name, int* d_out, long long numel,
                               void* stream);
 /* Test hook: the fp32 rotated IoU the NMS of dfm_box_post_forward decides with, pair by pair.
@@ -751,7 +753,8 @@ int dfm_anchor_loss_finish(dfm_anchor_loss_t* h, const float* d_avg, float* d_lo
 /* Test hook, from the last forward, [batch][N] per anchor: "assigned_gt" int32 (-1 ignored,
  * 0 negative, g + 1 for the sample's GT g), "labels" int32 (C for negatives and ignored),
  * "label_weights" fp32, "dir_targets" int32, "bbox_targets" fp32 [batch][N][7].
- * DFM_ERR_STATE before a forward, DFM_ERR_INVALID on an unknown name or wrong element count. */
+ * An unknown name fails with DFM_ERR_INVALID, before a forward too; a known one with
+ * DFM_ERR_STATE before a forward, then a wrong element count with DFM_ERR_INVALID. */
 int dfm_anchor_loss_debug_tensor(dfm_anchor_loss_t* h, const char* name, void* d_out,
                                  long long numel, void* stream);
 
@@ -814,7 +817,8 @@ int dfm_atss_loss_finish(dfm_atss_loss_t* h, const float* d_avg, float* d_losses
  * int32 (0 negative or invalid, g + 1 for the image's GT g), "labels" int32 (C for negatives
  * and invalid anchors), "label_weights" fp32, "centerness_targets" fp32 (0 for non-positives),
  * "bbox_targets" fp32 [batch][N][4]; "thresholds" fp32 [G], each GT's IoU threshold.
- * DFM_ERR_STATE before a forward, DFM_ERR_INVALID on an unknown name or wrong element count. */
+ * An unknown name fails with DFM_ERR_INVALID, before a forward too; a known one with
+ * DFM_ERR_STATE before a forward, then a wrong element count with DFM_ERR_INVALID. */
 int dfm_atss_loss_debug_tensor(dfm_atss_loss_t* h, const char* name, void* d_out,
                                long long numel, void* stream);
 
@@ -876,7 +880,8 @@ int dfm_imitation_loss_backward(dfm_imitation_loss_t* h, const float* d_coef,
                                 void* stream);
 /* Test hook, from the last forward: "inbox" uint8 [batch][ny][nx], "counts" int32 [num_pairs]
  * (this rank's positives), "loss_sums" fp64 [num_pairs] (sum_rows sum_c 0.5 * diff^2).
- * DFM_ERR_STATE before a forward, DFM_ERR_INVALID on an unknown name or wrong element count. */
+ * An unknown name fails with DFM_ERR_INVALID, before a forward too; a known one with
+ * DFM_ERR_STATE before a forward, then a wrong element count with DFM_ERR_INVALID. */
 int dfm_imitation_loss_debug_tensor(dfm_imitation_loss_t* h, const char* name, void* d_out,
                                     long long numel, void* stream);
 
@@ -926,7 +931,8 @@ int dfm_depth_loss_forward(dfm_depth_loss_t* h, const float* d_volume, const flo
                            void* stream);
 /* Test hook, from the last forward: "pixel_loss" fp32 [num_images][f * height][f * width], the
  * weighted per-pixel term (0 outside the mask); "count" int32 [1], the masked pixels.
- * DFM_ERR_STATE before a forward, DFM_ERR_INVALID on an unknown name or wrong element count. */
+ * An unknown name fails with DFM_ERR_INVALID, before a forward too; a known one with
+ * DFM_ERR_STATE before a forward, then a wrong element count with DFM_ERR_INVALID. */
 int dfm_depth_loss_debug_tensor(dfm_depth_loss_t* h, const char* name, void* d_out,
                                 long long numel, void* stream);
 

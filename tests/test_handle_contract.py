@@ -9,7 +9,10 @@ eleven at a small valid size against the state_dict its Python mirror uploads:
 - after the whole state_dict is uploaded nothing is missing, and a key can be uploaded again;
 - the debug hook refuses an unknown name and a tensor no forward has written, and after a
   forward a size other than what it wrote;
-- destroy(NULL) returns DFM_OK."""
+- destroy(NULL) returns DFM_OK.
+
+The handles without parameters (the losses, box_post, kitti_eval) keep the debug-hook and
+destroy parts."""
 import ctypes
 
 import pytest
@@ -166,6 +169,56 @@ def test_handle_contract():
     for family in FAMILIES + ('box_post',):
         assert getattr(L, f'dfm_{family}_destroy')(None) == capi.DFM_OK, family
     assert L.dfm_neck_missing_params(None) == -1
+
+
+def _unparameterised(L):
+    """(family, handle at a small valid size, (a tensor a forward writes, an unknown name)) of
+    the handles without parameters."""
+    f8 = ctypes.c_float * 8
+    ci8 = ctypes.c_int * 8
+    anchors = (ctypes.c_float * (4 * 4 * 2 * 7))()   # ny = nx = 4, 2 anchors per cell
+    half = f8(*[0.5] * 8)
+    al = capi.AnchorLossDesc(1, 1, 2, 4, 4, 1, 0, 1, 1, 0, 0, f8(*[0.6] * 8), f8(*[0.45] * 8),
+                             half, -1.0, 2.0, 0.25, 1.0 / 9, (ctypes.c_float * 4)(1, 2, 0.2, 0),
+                             -1.5707963, 0.0, 0.0)
+    at = capi.AtssLossDesc(1, 1, ci8(8), ci8(4), ci8(4), 1, 9, 8.0,
+                           (ctypes.c_float * 4)(0.1, 0.1, 0.2, 0.2), 0.016, 1e-7, 2.0, 0.25,
+                           (ctypes.c_float * 3)(1, 1, 1))
+    ci2, cf2 = ctypes.c_int * 2, ctypes.c_float * 2
+    ke = capi.KittiEvalDesc(1, (ctypes.c_int * 3)(0), 1, (ctypes.c_int * 3)(0), 0, 0,
+                            (ctypes.c_double * 18)(*[0.7] * 18))
+    return [
+        ('anchor_loss', _create(L, 'anchor_loss', ctypes.byref(al), anchors), ('labels', 'nope')),
+        ('atss_loss', _create(L, 'atss_loss', ctypes.byref(at)), ('labels', 'nope')),
+        ('depth_loss', _create(L, 'depth_loss', ctypes.byref(capi.DepthLossDesc(
+            1, 4, 4, 4, 1, 0, 2.0, 59.6, 1.0, 0.0, 1.0, 1.0, 0, 1.0))), ('count', 'nope')),
+        ('imitation_loss', _create(L, 'imitation_loss', ctypes.byref(capi.ImitationLossDesc(
+            1, 4, 4, 1, ci2(64), ci2(1), cf2(1.0), 10.0))), ('counts', 'nope')),
+        ('box_post', _create(L, 'box_post', ctypes.byref(capi.BoxPostDesc(
+            1, 2, 4, 4, 1, 1, -1, 10, 0.1, 0.01, -1.5707963, 0.0)), anchors),
+         ('cls0_keep', 'cls1_keep')),
+        ('kitti_eval', _create(L, 'kitti_eval', ctypes.byref(ke)), ('tp_scores', 'nope')),
+    ]
+
+
+@pytest.mark.gpu
+def test_unparameterised_debug_hooks():
+    """The handles without parameters keep the debug-hook part of the contract: an unknown name
+    is DFM_ERR_INVALID before any forward too, a known one DFM_ERR_STATE until a forward ran;
+    destroy(NULL) returns DFM_OK."""
+    import torch
+    L = capi.lib()
+    buf = torch.zeros(1 << 16, device='cuda')
+    p = vp(buf.data_ptr())
+    for family, h, (known, unknown) in _unparameterised(L):
+        try:
+            assert _debug(L, family, h, unknown, p, 1) == ERR_INVALID, family
+            assert 'unknown tensor' in _error(), (family, _error())
+            assert _debug(L, family, h, known, p, 1) == ERR_STATE, family
+            assert 'not written' in _error(), (family, _error())
+        finally:
+            assert getattr(L, f'dfm_{family}_destroy')(h) == capi.DFM_OK, family
+        assert getattr(L, f'dfm_{family}_destroy')(None) == capi.DFM_OK, family
 
 
 @pytest.mark.gpu

@@ -58,7 +58,7 @@ def main():
             p, s = modules._ptr, modules._stream()
 
             def c_call():
-                capi.check(L.dfm_box_post_forward(bp.handle, p(cls), p(box), p(dirc), p(ob),
+                capi.check(L.dfm_box_post_forward(bp._handle, p(cls), p(box), p(dirc), p(ob),
                                                   p(osc), p(ol), p(oc), s), 'forward')
             for _ in range(5):
                 c_call()
