@@ -31,7 +31,6 @@
 //     DFM_TC_DEBUG=<bits> disables loader work (1 everything, 8 proxy fence, 16 the
 //     loaders' global loads, 32 the loaders' shared-memory stores).
 #pragma once
-#include <cuda.h>
 #include <cuda_bf16.h>
 
 #include <algorithm>
@@ -248,8 +247,8 @@ struct TcWeights {
   void release() { dev.release(); }
   // packed: [27][Cin][Cout] fp32 (tap = kz*9 + ky*3 + kx; transposed weights are
   // already in "o = 2i - 1 + k" orientation)
-  // kslice: the CTA groups split the *input* channels (16 per group) and each covers all
-  // output channels; partial sums meet in global memory (see conv_tc_kernel, KSLICE).
+  // ks (stride 2 only): the CTA groups split the *input* channels (16 per group) and each covers
+  // all output channels; partial sums meet in global memory (see conv_tc_kernel, KSLICE).
   template <int MODE>
   bool build_mode(const float* packed, int cin, int cout, std::string* err, bool ks = false) {
     release();
@@ -296,18 +295,8 @@ struct TcWeights {
     }
     return true;
   }
-  // share_bricks = false: a 32 -> 64 stride-2 layer takes the input-channel slices instead of
-  // the cluster-shared bricks (see below)
-  bool build(const float* packed, int cin, int cout, int m, std::string* err,
-             bool share_bricks = true) {
-    static const bool no_ks1 = getenv("DFM_NO_KSLICE") != nullptr;
-    // stride 1, 64 -> 64: four output-channel groups each re-load the input and issue N = 48
-    // MMAs; four input-channel slices would issue N = 192 MMAs on a quarter of the input each
-    // (opt-in: not measured on H100; the 64 -> 64 stride-1 layers of the backbone run on the
-    // K-outer kernel of conv_tc_neck.cuh)
-    static const bool ks1 = getenv("DFM_KSLICE_S1") != nullptr;
-    if (m == TC_S1) return build_mode<TC_S1>(packed, cin, cout, err,
-                                             cin == 64 && cout == 64 && !no_ks1 && ks1);
+  bool build(const float* packed, int cin, int cout, int m, std::string* err) {
+    if (m == TC_S1) return build_mode<TC_S1>(packed, cin, cout, err);
     if (m == TC_S2) {
       // stride-2 layers are loader-bound: with independent output-channel groups every group
       // re-loads and re-transforms the whole input (2x for 32->64, 4x for 64->64).
@@ -317,14 +306,10 @@ struct TcWeights {
       // Four clustered groups of 16 outputs issue N = 16 / 32 MMAs that each re-read the whole
       // 64-channel brick from shared memory: H100 SXM, KITTI D = 112 stereo conv3, 0.570 ms
       // clustered vs 0.220 ms sliced.
-      // A/B switches: DFM_S2_KSLICE=1 (read whenever weights are set) slices 32 -> 64 too -- the
-      // route DFM_NO_TMA / DFM_TMA_CONV3 refine --, DFM_NO_KSLICE=1 independent output groups.
-      static const bool no_ks = getenv("DFM_NO_KSLICE") != nullptr;
-      static const bool tma_ab = getenv("DFM_NO_TMA") != nullptr || getenv("DFM_TMA_CONV3") != nullptr;
-      const bool ks = cout == 64 && !no_ks &&
-                      (cin == 64 || !share_bricks || tma_ab || getenv("DFM_S2_KSLICE") != nullptr);
+      // Other shapes keep independent output-channel groups.
+      const bool ks = cin == 64 && cout == 64;
       if (!build_mode<TC_S2>(packed, cin, cout, err, ks)) return false;
-      if (cin == 32 && cout == 64 && !ks && !no_ks) cluster = nsplit;  // 2
+      if (cin == 32 && cout == 64) cluster = nsplit;  // 2
       return true;
     }
     return build_mode<TC_T>(packed, cin, cout, err);
@@ -471,7 +456,6 @@ __device__ __forceinline__ float4 ld_act(const float4* p) {
 
 template <int NT>  // number of input terms (compile-time: sizes the in-flight registers)
 struct SrcLoader8 {
-  static constexpr bool kTma = false;
   Src s;
   int C, H, W;
   // items of a thread in flight at once: at most 12 float4 (48 registers) of raw loads
@@ -522,7 +506,6 @@ struct SrcLoader8 {
 };
 
 struct WarpLoader8 {
-  static constexpr bool kTma = false;
   WarpLoader w;
   static constexpr int BATCH = 1;
   struct Raw {
@@ -567,141 +550,6 @@ struct WarpLoader8 {
     }
   }
 };
-
-// ----------------------------------------------------------------------------------
-// TMA loader (stride-2 convs): the input was written once by presplit_kernel as bf16 hi / lo
-// pairs in the parity-planar "pre-split" layout (see presplit_kernel; 16 bytes per (chunk,
-// voxel), the same 4 bytes per value as fp32), viewed by a rank-4 tensor map
-// {8, W/2, H/2, planes*2*4*chunks}.  One elected thread then stages a whole brick with
-// cp.async.bulk.tensor: per (hi|lo, x/y parity class) ONE dense box of 9 x 17 positions x 2
-// chunks, and out-of-range halo positions arrive as zeros.  No loader warp touches the data: the fused GroupNorm /
-// ReLU / residual transform and the bf16 split happened once, in the producer pass.
-// (The box / zero-fill / byte-count semantics are pinned by the GPU parity tests of the backbone,
-// whose stride-2 hourglass.conv1 runs on this loader at full size and on ragged fixtures.)
-// ----------------------------------------------------------------------------------
-struct TmaLoader8 {
-  static constexpr bool kTma = true;
-  static constexpr int BATCH = 1;
-  CUtensorMap map;
-  int nch_total;  // channels / 8 of the pre-split tensor
-  struct Raw {};
-  __device__ __forceinline__ void issue(int, int, int, int, Raw&) const {}
-  __device__ __forceinline__ void finish(const Raw&, int, float v[8]) const {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = 0.f;
-  }
-};
-constexpr int TMA_S2_CLS = 17 * 9;                         // rows of one parity class, one chunk
-constexpr int TMA_S2_CLSR = (2 * TMA_S2_CLS + 7) / 8 * 8;  // two chunks, padded to 128 bytes
-
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, int c1, int c2,
-                                            int c3, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%2, %3, %4, %5}], [%6];" ::"r"(dst),
-      "l"(map), "r"(0), "r"(c1), "r"(c2), "r"(c3), "r"(bar)
-      : "memory");
-}
-
-// producer pass: value = the fused input transform of `ld` (<= 3 terms), split to bf16 hi / lo,
-// written in the pre-split layout of a stride-2 consumer: x / y PARITY-PLANAR,
-//   [plane z][hi|lo][y parity][x parity][8-channel chunk][H/2][W/2] x 16 bytes,
-// so every parity class of a stride-2 brick is a DENSE 2-D box for TMA (a strided box --
-// elementStrides 2 -- moves one 16-byte element per request).
-// A warp transforms a run of 64 consecutive x of one row (coalesced 32-byte reads), stages the
-// split values in shared memory and writes 512-byte runs per (hi|lo, x parity, chunk).
-constexpr int PS_XRUN = 64, PS_WARPS = 4, PS_SEG = 33;  // 33: shared-memory segment pitch
-inline size_t presplit_smem_bytes(int C) { return (size_t)PS_WARPS * 4 * (C / 8) * PS_SEG * 16; }
-template <int NT>
-__global__ void __launch_bounds__(32 * PS_WARPS)
-presplit_kernel(const SrcLoader8<NT> ld, int Z, uint4* __restrict__ out) {
-  extern __shared__ uint4 ps_sm[];
-  const int nch = ld.C >> 3, W = ld.W, H = ld.H, W2 = W >> 1, H2 = H >> 1;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint4* sm = ps_sm + (size_t)warp * 4 * nch * PS_SEG;   // [hi|lo][x parity][chunk][33]
-  const int runs_per_row = (W + PS_XRUN - 1) / PS_XRUN;
-  const long long nruns = (long long)Z * H * runs_per_row;
-  for (long long r = (long long)blockIdx.x * PS_WARPS + warp; r < nruns;
-       r += (long long)gridDim.x * PS_WARPS) {
-    const int run = (int)(r % runs_per_row);
-    const long long zy = r / runs_per_row;
-    const int y = (int)(zy % H), z = (int)(zy / H);
-    const int xb = run * PS_XRUN;
-#pragma unroll 4
-    for (int i = lane; i < PS_XRUN * nch; i += 32) {
-      const int xl = i / nch, chunk = i - xl * nch, x = xb + xl;
-      if (x < W) {
-        typename SrcLoader8<NT>::Raw raw;
-        ld.issue(z, y, x, chunk * 8, raw);
-        float val[8];
-        ld.finish(raw, chunk * 8, val);
-        uint4* hi = sm + ((xl & 1) * nch + chunk) * PS_SEG + (xl >> 1);
-        split_store(val, reinterpret_cast<uint8_t*>(hi),
-                    reinterpret_cast<uint8_t*>(hi + 2 * nch * PS_SEG));
-      }
-    }
-    __syncwarp();
-    const int py = y & 1, y2 = y >> 1, x2 = (xb >> 1) + lane;
-    for (int seg = 0; seg < 4 * nch; ++seg) {
-      const int chunk = seg % nch, px = (seg / nch) & 1, hl = seg / (2 * nch);
-      if (2 * x2 + px < W)
-        out[((((long long)(z * 2 + hl) * 4 + py * 2 + px) * nch + chunk) * H2 + y2) * W2 + x2] =
-            sm[seg * PS_SEG + lane];
-    }
-    __syncwarp();
-  }
-}
-inline bool presplit_launch(const Src& s, int C, int Z, int H, int W, uint4* out, cudaStream_t st) {
-  if ((H | W) & 1) return false;
-  const size_t smem = presplit_smem_bytes(C);
-  const long long nruns = (long long)Z * H * ((W + PS_XRUN - 1) / PS_XRUN);
-  const int blocks = (int)std::min<long long>((nruns + PS_WARPS - 1) / PS_WARPS, 12LL * tc_sm_count());
-  auto go = [&](auto kern, auto ld) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) !=
-        cudaSuccess)
-      return false;
-    kern<<<blocks, 32 * PS_WARPS, smem, st>>>(ld, Z, out);
-    return cudaGetLastError() == cudaSuccess;
-  };
-  if (s.n == 1) return go(presplit_kernel<1>, SrcLoader8<1>{s, C, H, W});
-  if (s.n == 2) return go(presplit_kernel<2>, SrcLoader8<2>{s, C, H, W});
-  return go(presplit_kernel<3>, SrcLoader8<3>{s, C, H, W});
-}
-
-// host: tensor map over a pre-split buffer: rank 4 {8 bf16, W/2, H/2, planes*2*4*chunks}, box =
-// one parity class of a stride-2 brick (9 x 17 positions) for two adjacent chunks
-inline bool make_presplit_map_s2(CUtensorMap* map, const void* base, int W, int H,
-                                 long long slabs, std::string* err) {
-  typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                               const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                               const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  static EncodeFn encode = nullptr;
-  if (!encode) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) !=
-            cudaSuccess || !fn || qres != cudaDriverEntryPointSuccess) {
-      if (err) *err = "cuTensorMapEncodeTiled is not available from this driver";
-      return false;
-    }
-    encode = (EncodeFn)fn;
-  }
-  const int W2 = W / 2, H2 = H / 2;
-  const cuuint64_t dims[4] = {8, (cuuint64_t)W2, (cuuint64_t)H2, (cuuint64_t)slabs};
-  const cuuint64_t strides[3] = {16, (cuuint64_t)W2 * 16, (cuuint64_t)H2 * W2 * 16};
-  const cuuint32_t box[4] = {8, 9, 17, 2};
-  const cuuint32_t estr[4] = {1, 1, 1, 1};
-  const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_UINT16, 4, const_cast<void*>(base), dims,
-                            strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    if (err) *err = "cuTensorMapEncodeTiled failed with code " + std::to_string((int)r);
-    return false;
-  }
-  return true;
-}
 
 struct TcParams {
   const uint8_t* wimg;
@@ -802,25 +650,21 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                                                                  const __grid_constant__ Loader ld) {
   using M = TcMode<MODE>;
   using Win = TcWin<MODE>;
-  constexpr bool TMA = Loader::kTma;
   constexpr bool CLU = CL > 1;
-  static_assert(!TMA || MODE == TC_S2, "the TMA loader serves the stride-2 brick only");
-  static_assert(!CLU || (MODE == TC_S2 && !TMA && CIN != 16),
-                "cluster-shared bricks serve the stride-2 output-channel split with register loaders");
+  static_assert(!CLU || (MODE == TC_S2 && CIN != 16),
+                "cluster-shared bricks serve the stride-2 output-channel split");
   constexpr int CG = M::CG < CIN ? M::CG : CIN;  // channels per stage
   constexpr int NCH = CG / 8;                    // 16-byte channel chunks per stage
   constexpr int NCG = CIN / CG;                  // pipeline stages per input plane
-  static_assert(!TMA || NCH == 2, "TMA stride-2 stages hold two 8-channel chunks");
-  // stage layout.  Register loaders: [hi|lo][chunk][ROWS rows] with the four x/y parity classes
-  // of a stride-2 brick inside a chunk's rows.  TMA loader: [hi|lo][class][chunk][153 rows], one
-  // TMA box per (hi|lo, class), each block padded to 128 bytes.
-  constexpr uint32_t S2_CLS16 = TMA ? TMA_S2_CLSR : TMA_S2_CLS;  // class stride, 16-byte rows
-  constexpr uint32_t A_LBO = TMA ? TMA_S2_CLS * 16 : M::ROWS * 16;
+  // stage layout: [hi|lo][chunk][ROWS rows] with the four x/y parity classes of a stride-2
+  // brick inside a chunk's rows
+  constexpr uint32_t S2_CLS16 = 17 * M::PITCH;  // stride-2 class stride, 16-byte rows
+  constexpr uint32_t A_LBO = M::ROWS * 16;
   constexpr uint32_t A_SBO = M::PITCH * 16;
-  constexpr uint32_t A_HL = TMA ? 4 * TMA_S2_CLSR * 16 : NCH * M::ROWS * 16;  // hi -> lo offset
+  constexpr uint32_t A_HL = NCH * M::ROWS * 16;  // hi -> lo offset
   constexpr uint32_t STAGE_BYTES = 2 * A_HL;
   constexpr uint32_t B_SBO = 128;
-  // K-slice variant (stride 1 / 2, instantiated with CIN = 16 = the channels this CTA group loads,
+  // K-slice variant (stride 2, instantiated with CIN = 16 = the channels this CTA group loads,
   // NCTA = all output channels): every slice stores its partial sums; kslice_reduce_kernel adds
   // them in slice order (deterministic) and takes the GroupNorm statistics on the way
   constexpr bool KSLICE = CIN == 16;
@@ -853,9 +697,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
 
   if (tid == 0) {
     for (int s = 0; s < M::NSTAGE; ++s) {
-      // one arrival per loader warp of the group (of every CTA of the cluster); TMA: the issuing
-      // thread's expect_tx arrival
-      mbar_init(full_a(s), TMA ? 1 : CL * LG_THREADS / 32);
+      // one arrival per loader warp of the group (of every CTA of the cluster)
+      mbar_init(full_a(s), CL * LG_THREADS / 32);
       mbar_init(empty_a(s), CL * TC_MMA_THREADS / 32);  // one arrival per consumer warp
     }
     mbar_init(w_bar, 1);
@@ -882,48 +725,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   if constexpr (CLU) cluster_sync_all();
   else __syncthreads();
 
-  if constexpr (TMA) {
-    if (warp == LOAD_WARP0 && lane == 0) {
-      // ============================ TMA producer (one thread) ============================
-      constexpr uint32_t STAGE_TX = 8u * 2u * TMA_S2_CLS * 16u;  // 8 boxes of 2 x 153 x 16 bytes
-      uint32_t stage_ctr = 0;
-      TcWalk walk = tc_walk_begin(p);
-      TcItem it;
-      while (tc_walk_next(p, walk, it)) {
-        const int zi0 = max(M::zi_first(it.z_lo), 0);
-        const int zi1 = min(M::zi_last(it.z_hi - 1), p.Di - 1);
-        const int chunk0 = CIN == 16 ? it.split * 2 : 0;
-        for (int zi = zi0; zi <= zi1; ++zi) {
-#pragma unroll 1
-          for (int cg = 0; cg < NCG; ++cg, ++stage_ctr) {
-            const int s = stage_ctr % M::NSTAGE;
-            mbar_wait(empty_a(s), ((stage_ctr / M::NSTAGE) & 1) ^ 1, p.err);
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(full_a(s)),
-                         "r"(STAGE_TX)
-                         : "memory");
-            const uint32_t st_addr = smem_u32(a_s + s * STAGE_BYTES);
-#pragma unroll
-            for (int hl = 0; hl < 2; ++hl) {
-#pragma unroll
-              for (int cls = 0; cls < 4; ++cls) {
-                // brick class = (brick x parity) * 2 + (brick y parity).  Brick position bx
-                // is input x = 2*x0 - 1 + bx: brick parity 0 holds the ODD input columns
-                // x0-1, x0, ... (half index), brick parity 1 the EVEN ones x0, x0+1, ...
-                const int bxp = cls >> 1, byp = cls & 1;
-                const int cls_in = (1 - byp) * 2 + (1 - bxp);
-                const int slab = ((zi * 2 + hl) * 4 + cls_in) * ld.nch_total + chunk0 + cg * NCH;
-                tma_load_4d(st_addr + hl * A_HL + cls * (TMA_S2_CLSR * 16), &ld.map,
-                            it.x0 - 1 + bxp, it.y0 - 1 + byp, slab, full_a(s));
-              }
-            }
-          }
-        }
-      }
-    }
-  }
-  if (TMA && warp >= LOAD_WARP0) {
-    // (the loader warps have nothing to do: the first loader warp's lane 0 issued the TMA boxes)
-  } else if (warp >= LOAD_WARP0) {
+  if (warp >= LOAD_WARP0) {
     // ============================ loaders ============================
     const int lw = warp - LOAD_WARP0;
     const int lgrp = lw & (LGROUPS - 1);
@@ -1414,8 +1216,7 @@ bool tc_launch(const Loader& ld, const TcWeights& w, float* out, double* stats,
                const ConvGeom& g, cudaStream_t st, std::string* err, TcOpts opt = TcOpts()) {
   using M = TcMode<MODE>;
   constexpr int CG = M::CG < CIN ? M::CG : CIN;
-  constexpr size_t STAGE_BYTES = Loader::kTma ? (size_t)2 * 4 * TMA_S2_CLSR * 16
-                                              : (size_t)2 * (CG / 8) * M::ROWS * 16;
+  constexpr size_t STAGE_BYTES = (size_t)2 * (CG / 8) * M::ROWS * 16;
   const size_t smem = w.image_bytes + M::NSTAGE * STAGE_BYTES + (2 * M::NSTAGE + 1) * 8;
   auto kern = conv_tc_kernel<MODE, CIN, NCTA, Loader, CL>;
   if (w.cluster != CL || (CL > 1 && w.nsplit != CL)) {
@@ -1537,8 +1338,8 @@ bool tc_dispatch(const Loader& ld, const TcWeights& w, float* out, double* stats
   if (w.kslice) {
     // the input-channel slices store partial outputs into a scratch; a second kernel adds them
     // in slice order into `out` and accumulates the GroupNorm statistics
-    if ((mode != TC_S2 && mode != TC_S1) || g.Cout != 64 || opt.addend || opt.store1) {
-      if (err) *err = "conv_tc: K-slice weights are for plain convs with 64 outputs";
+    if (mode != TC_S2 || g.Cout != 64 || opt.addend || opt.store1) {
+      if (err) *err = "conv_tc: K-slice weights are for plain stride-2 convs with 64 outputs";
       return false;
     }
     const long long V = (long long)g.Do * g.Ho * g.Wo;
@@ -1549,16 +1350,7 @@ bool tc_dispatch(const Loader& ld, const TcWeights& w, float* out, double* stats
     }
     TcOpts o2 = opt;
     o2.slice_stride = V * 64;
-    bool launched = false;
-    if constexpr (Loader::kTma) {
-      if (mode == TC_S2) launched = tc_launch<TC_S2, 16, 64, Loader>(ld, w, part, nullptr, g, st, err, o2);
-      else if (err) *err = "conv_tc: the TMA loader serves stride-2 convs only";
-    } else {
-      launched = mode == TC_S2
-                     ? tc_launch<TC_S2, 16, 64, Loader>(ld, w, part, nullptr, g, st, err, o2)
-                     : tc_launch<TC_S1, 16, 64, Loader>(ld, w, part, nullptr, g, st, err, o2);
-    }
-    if (!launched) return false;
+    if (!tc_launch<TC_S2, 16, 64, Loader>(ld, w, part, nullptr, g, st, err, o2)) return false;
     const int blocks = (int)std::min<long long>(8LL * tc_sm_count(), (V + 15) / 16);
     kslice_reduce_kernel<<<blocks, 256, 0, st>>>(part, w.nsplit, V, (long long)g.Ho * g.Wo, out,
                                                  stats, opt.zw_lo, opt.zw_hi, opt.zw);
@@ -1568,16 +1360,12 @@ bool tc_dispatch(const Loader& ld, const TcWeights& w, float* out, double* stats
     }
     return true;
   }
-  if constexpr (Loader::kTma) {
-    if (err) *err = "conv_tc: the TMA loader serves the K-slice stride-2 convs only";
+  if (mode == TC_S2 && w.cluster > 1) {
+    if (g.Cin == 32 && w.cluster == 2)
+      return tc_launch<TC_S2, 32, 32, Loader, 2>(ld, w, out, stats, g, st, err, opt);
+    if (err) *err = "conv_tc: unsupported (Cin, cluster size)";
     return false;
-  } else {
-    if (mode == TC_S2 && w.cluster > 1) {
-      if (g.Cin == 32 && w.cluster == 2)
-        return tc_launch<TC_S2, 32, 32, Loader, 2>(ld, w, out, stats, g, st, err, opt);
-      if (err) *err = "conv_tc: unsupported (Cin, cluster size)";
-      return false;
-    }
+  }
 #define TC_CASE(MD, CI, NC) \
   if (mode == MD && g.Cin == CI) \
     return tc_launch<MD, CI, NC, Loader>(ld, w, out, stats, g, st, err, opt)
@@ -1589,7 +1377,6 @@ bool tc_dispatch(const Loader& ld, const TcWeights& w, float* out, double* stats
 #undef TC_CASE
   if (err) *err = "conv_tc: unsupported (mode, Cin)";
   return false;
-  }
 }
 
 inline bool tc_conv_src(const Src& s, const TcWeights& w, float* out, double* stats,
@@ -1604,20 +1391,6 @@ inline bool tc_conv_src(const Src& s, const TcWeights& w, float* out, double* st
     return tc_dispatch(ld, w, out, stats, g, st, err, opt);
   }
   SrcLoader8<3> ld{s, g.Cin, g.Hi, g.Wi};
-  return tc_dispatch(ld, w, out, stats, g, st, err, opt);
-}
-// stride-2 conv whose input is a pre-split tensor (presplit_kernel): bricks staged by TMA
-inline bool tc_conv_presplit(const uint4* ps, int channels, const TcWeights& w, float* out,
-                             double* stats, const ConvGeom& g, cudaStream_t st, std::string* err,
-                             TcOpts opt = TcOpts()) {
-  if (tc_mode_of(g) != TC_S2 || !w.kslice || channels != g.Cin) {
-    if (err) *err = "conv_tc: the TMA loader serves the K-slice stride-2 convs only";
-    return false;
-  }
-  TmaLoader8 ld;
-  ld.nch_total = channels / 8;
-  if (!make_presplit_map_s2(&ld.map, ps, g.Wi, g.Hi, (long long)g.Di * 2 * 4 * ld.nch_total, err))
-    return false;
   return tc_dispatch(ld, w, out, stats, g, st, err, opt);
 }
 inline bool tc_conv_warp(const WarpLoader& wl, const TcWeights& w, float* out, double* stats,

@@ -328,10 +328,9 @@ int upload(DevBuf& b, const float* h, size_t n) {
   return DFM_OK;
 }
 
-// tc_mode: dfm::TC_S1 / TC_S2 / TC_T, or -1 for "no tensor-core kernel for this layer";
-// share_bricks: see dfm::TcWeights::build
+// tc_mode: dfm::TC_S1 / TC_S2 / TC_T, or -1 for "no tensor-core kernel for this layer"
 int set_conv(ConvW& cw, const float* h, long long numel, int Cin, int Cout, int transposed,
-             int tc_mode, bool share_bricks = true) {
+             int tc_mode) {
   if (numel != (long long)27 * Cin * Cout)
     return fail(DFM_ERR_INVALID, "conv weight has wrong element count");
   cw.Cin = Cin;
@@ -342,7 +341,7 @@ int set_conv(ConvW& cw, const float* h, long long numel, int Cin, int Cout, int 
   cw.tc.release();
   if (tc_mode >= 0 && dfm::tc_supported(Cin, Cout, transposed)) {
     std::string err;
-    if (!cw.tc.build(p.data(), Cin, Cout, tc_mode, &err, share_bricks))
+    if (!cw.tc.build(p.data(), Cin, Cout, tc_mode, &err))
       return fail(DFM_ERR_CUDA, err);
   }
   cw.ntk.release();
@@ -542,38 +541,6 @@ int run_conv(const dfm::Src& s, const ConvW& w, float* out, const dfm::ConvGeom&
       }, "src", w, out, g, impl, gn, st, zw);
 }
 
-// Stride-2 conv fed by TMA: one producer pass applies the fused input transform of `s` and
-// writes it pre-split (bf16 hi / lo, brick-friendly layout) into `ps`, then the conv stages its
-// bricks with cp.async.bulk.tensor instead of eight loader warps (conv_tc.cuh, TmaLoader8).
-int run_conv_presplit(const dfm::Src& s, DevBuf& ps, const ConvW& w, float* out,
-                      const dfm::ConvGeom& g, cudaStream_t st, Norm* gn, const ZW& zw) {
-  const long long Vin = (long long)g.Di * g.Hi * g.Wi;
-  DFM_TRY(ps.alloc((size_t)Vin * g.Cin));
-  {
-    ProfScope ps_scope("presplit<" + std::to_string(g.Cin) + ">@" + std::to_string(g.Di) + "x" +
-                           std::to_string(g.Hi) + "x" + std::to_string(g.Wi), 0.0, st);
-    if (!dfm::presplit_launch(s, g.Cin, g.Di, g.Hi, g.Wi, reinterpret_cast<uint4*>(ps.p), st))
-      return fail(DFM_ERR_CUDA, "presplit_kernel launch failed");
-    g_launches.fetch_add(1);
-  }
-  const long long V = (long long)(zw.count_planes ? zw.count_planes : g.Do) * g.Ho * g.Wo;
-  if (gn) DFM_TRY(gn->begin_stats(st));
-  {
-    std::string err;
-    ProfScope pc(conv_class(w.tc.kslice ? "conv_tc_ks" : "conv_tc", g, "tma"), conv_flops(g), st);
-    dfm::TcOpts o;
-    o.zw_lo = zw.lo;
-    o.zw_hi = zw.hi;
-    o.zw = zw.w;
-    if (!dfm::tc_conv_presplit(reinterpret_cast<const uint4*>(ps.p), g.Cin, w.tc, out,
-                               gn ? gn->sums.p : nullptr, g, st, &err, o))
-      return fail(DFM_ERR_CUDA, err);
-  }
-  g_launches.fetch_add(2);  // conv + slice reduce
-  g_tc_launches.fetch_add(1);
-  return gn ? gn_finalize(*gn, V, 32, st) : DFM_OK;
-}
-
 int run_conv_warp(const dfm::WarpLoader& ld, const ConvW& w, float* out, const dfm::ConvGeom& g,
                   int impl, cudaStream_t st, Norm* gn = nullptr, const float* addend = nullptr) {
   if (addend && (impl == DFM_CONV_SIMT || !w.tc.ready()))
@@ -701,7 +668,6 @@ struct Tower {
   DevBuf cls5, cls3;
   Norm g0, g1, gc1, gc2, gc3, gc4, gc5, gc6, gp0;
   DevBuf raw0, raw1, b1, b2, b3, b4, b5, b6, cur, p0b, logit;
-  DevBuf ps0, ps2;  // pre-split (bf16 hi / lo) inputs of the two stride-2 convs, read by TMA
   // what the last forward wrote (dfm_backbone_debug_tensor refuses the rest): the z-class
   // path keeps dres0_mono's output in cls3 only, and only that path writes cls3
   bool raw0_written = false, cls3_written = false;
@@ -818,11 +784,6 @@ void tower_add_params(ParamTable& p, Tower& t, bool mono, int cin0, int cv) {
   add_norm(p, "dres0" + sfx + ".gn", t.g0);
   add_norm(p, "dres1" + sfx + ".gn", t.g1);
   struct HG { const char* key; ConvW* w; Norm* n; int ci, co, tr, mode; };
-  // conv1: the stereo tower shares bricks in a CTA cluster; the mono tower keeps the TMA-fed
-  // input-channel slices, so the shipped forward keeps running (and the per-layer test of the
-  // benchmarked shape keeps checking) the presplit producer and the TMA loader.  At KITTI D = 112
-  // that costs 0.107 ms (H100 SXM: 0.432 vs 0.325 ms), the stereo tower carries 83 % of conv1's
-  // bytes.
   const HG hgs[] = {{"conv1.0", &t.c1, &t.gc1, cv, 2 * cv, 0, dfm::TC_S2},
                     {"conv2", &t.c2, &t.gc2, 2 * cv, 2 * cv, 0, dfm::TC_S1},
                     {"conv3.0", &t.c3, &t.gc3, 2 * cv, 2 * cv, 0, dfm::TC_S2},
@@ -832,9 +793,8 @@ void tower_add_params(ParamTable& p, Tower& t, bool mono, int cin0, int cv) {
   for (const HG& e : hgs) {
     const std::string base = hg + "." + e.key;
     const long long n = 27LL * e.ci * e.co;
-    p.add(base + ".0.weight", n, [e, n, mono](const float* h) {
-      return set_conv(*e.w, h, n, e.ci, e.co, e.tr, e.mode, !mono);
-    });
+    p.add(base + ".0.weight", n,
+          [e, n](const float* h) { return set_conv(*e.w, h, n, e.ci, e.co, e.tr, e.mode); });
     add_norm(p, base + ".1", *e.n);
   }
   p.add(pr + ".0.conv.weight", n1,
@@ -936,32 +896,15 @@ int tower_forward(dfm_backbone* bb, Tower& t, bool mono, const dfm::WarpLoader& 
   // cost0 = gn1(raw1) + relu(gn0(raw0)) is never stored: consumers re-evaluate it
   const dfm::Term T1 = term(t.raw1, &t.g1, 0);
   // hourglass (conv_modules.py:129-149)
-  // stereo conv1 runs as a cluster of two output-channel groups that share every input brick,
-  // mono conv1 and conv3 as input-channel slices (conv_tc.cuh, TcWeights::build; tower_add_params).
-  // On the K-slice route conv1 is fed by TMA from a pre-split copy of its input (DFM_NO_TMA=1:
-  // register loaders; DFM_S2_KSLICE=1 puts the stereo conv1 there too, for A/B runs)
-  static const bool no_tma = getenv("DFM_NO_TMA") != nullptr;
-  auto tma_ok = [&](const ConvW& w) {
-    return impl != DFM_CONV_SIMT && !no_tma && w.tc.ready() && w.tc.kslice &&
-           w.tc.mode == dfm::TC_S2;
-  };
+  // conv1 runs as a cluster of two output-channel groups that share every input brick, conv3 as
+  // input-channel slices (conv_tc.cuh, TcWeights::build)
   g = geom_s(D, Ho, Wo, cv, 2 * cv, 2, 2, 2, 1, 1, 1);
-  if (tma_ok(t.c1) && dfm::tc_mode_of(g) == dfm::TC_S2)
-    DFM_TRY(run_conv_presplit(src2(T1, T0), t.ps0, t.c1, t.b1.p, g, st, &t.gc1, zw_at(2)));
-  else
-    DFM_TRY(run_conv(src2(T1, T0), t.c1, t.b1.p, g, impl, st, &t.gc1, zw_at(2)));
+  DFM_TRY(run_conv(src2(T1, T0), t.c1, t.b1.p, g, impl, st, &t.gc1, zw_at(2)));
   const int D2 = g.Do, H2 = g.Ho, W2 = g.Wo;
   g = geom_s(D2, H2, W2, 2 * cv, 2 * cv, 1, 1, 1, 1, 1, 1);
   DFM_TRY(run_conv(src1(term(t.b1, &t.gc1, 1)), t.c2, t.b2.p, g, impl, st, &t.gc2, zw_at(2)));
   g = geom_s(D2, H2, W2, 2 * cv, 2 * cv, 2, 2, 2, 1, 1, 1);
-  // (conv3, half resolution: TMA is opt-in.  H100 SXM, KITTI D=112: register loaders 0.220 + 0.103
-  // ms (stereo + mono); TMA 0.231 + 0.099 ms plus 0.123 + 0.047 ms of producer passes)
-  static const bool tma_c3 = getenv("DFM_TMA_CONV3") != nullptr;
-  if (tma_c3 && tma_ok(t.c3) && dfm::tc_mode_of(g) == dfm::TC_S2)
-    DFM_TRY(run_conv_presplit(src1(term(t.b2, &t.gc2, 1)), t.ps2, t.c3, t.b3.p, g, st, &t.gc3,
-                              zw_at(4)));
-  else
-    DFM_TRY(run_conv(src1(term(t.b2, &t.gc2, 1)), t.c3, t.b3.p, g, impl, st, &t.gc3, zw_at(4)));
+  DFM_TRY(run_conv(src1(term(t.b2, &t.gc2, 1)), t.c3, t.b3.p, g, impl, st, &t.gc3, zw_at(4)));
   const int D4 = g.Do, H4 = g.Ho, W4 = g.Wo;
   g = geom_s(D4, H4, W4, 2 * cv, 2 * cv, 1, 1, 1, 1, 1, 1);
   DFM_TRY(run_conv(src1(term(t.b3, &t.gc3, 1)), t.c4, t.b4.p, g, impl, st, &t.gc4, zw_at(4)));

@@ -56,7 +56,7 @@ CASES = {
     # with (D - 32) % 8 == 4, i.e. interior statistics weight 4.5
     'aug_64x112_d68': dict(seed=42, h=64, w=112, d=68, flip=True, crop=(10, 40), scale=1.03,
                            ori=(375, 1242, 3)),
-    # the benchmarked shape: conv2 / conv4 on the K-outer kernel, full TMA brick grid
+    # the benchmarked shape: conv2 / conv4 on the K-outer kernel, full-size tile grids
     'bench_384x1248_d112': dict(seed=3, h=384, w=1248, d=112, ori=(370, 1224, 3), slabs=True),
     # the shipped KITTI config: D % 16 == 8 in the logits chunks and the gate at full width
     'kitti_320x1280_d72': dict(seed=21, h=320, w=1280, d=72, crop=(0, 55), ori=(375, 1242, 3),
@@ -174,7 +174,7 @@ def fp64_params(params, dev):
 # ---------------------------------------------------------------------------------------------
 # CPU: the bounds keep a lost product term out, at the test shapes
 # ---------------------------------------------------------------------------------------------
-LAYER_CLASS = {'raw0': 'dres0 (warp loader)', 'raw1': 'dres1', 'c1': 'conv1 s2 (TMA, K-slice)',
+LAYER_CLASS = {'raw0': 'dres0 (warp loader)', 'raw1': 'dres1', 'c1': 'conv1 s2 (cluster)',
                'c2': 'conv2', 'c3': 'conv3 s2 (K-slice)', 'c4': 'conv4',
                'c5': 'conv5 T', 'c6': 'conv6 T (2 terms)', 'p0': 'pred.0',
                'logit': 'pred.1 (logits)'}
@@ -285,7 +285,7 @@ LEVEL = {'raw0': 1, 'cls3': 1, 'raw1': 1, 'c1': 2, 'c2': 2, 'c3': 4, 'c4': 4, 'c
 # kernel classes of the profile report (names without the shape) that compute a compared layer
 TC_PREFIXES = ('conv_tc', 'cout1_logits', 'gate')
 # every class the issue of this test names must be among them at the benchmarked shape
-BENCH_CLASSES = ('conv_tc<32->32,s1,warp>', 'conv_tc<32->32,s1,src>', 'conv_tc_ks<32->64,s2,tma>',
+BENCH_CLASSES = ('conv_tc<32->32,s1,warp>', 'conv_tc<32->32,s1,src>', 'conv_tc_cl<32->64,s2,src>',
                  'conv_tc_ks<64->64,s2,src>', 'conv_tck<64->64,s1,src>', 'conv_tc<64->64,T,src>',
                  'conv_tc<64->32,T,src>', 'cout1_logits_tc<32->32,s1,src>', 'gate_tile4')
 # the classes a case must have launched and compared
@@ -542,12 +542,6 @@ def test_debug_hook_refuses_unwritten_tensor():
 AB_ARMS = [
     # (env, case, a class the arm must launch, a default-path class it must not launch).  The
     # default path launches the "avoid" class at that case, so each arm demonstrably switched.
-    ({'DFM_NO_TMA': '1'}, 'aug_64x112_d68', 'conv_tc_ks<32->64,s2,src>', ',tma>'),
-    ({'DFM_TMA_CONV3': '1'}, 'aug_64x112_d68', 'conv_tc_ks<64->64,s2,tma>',
-     'conv_tc_ks<64->64,s2,src>'),
-    ({'DFM_NO_KSLICE': '1'}, 'aug_64x112_d68', 'conv_tc<64->64,s2,src>', 'conv_tc_ks'),
-    ({'DFM_KSLICE_S1': '1'}, 'aug_64x112_d68', 'conv_tc_ks<64->64,s1,src>',
-     'conv_tc<64->64,s1,src>'),
     # the K-outer kernel is the default for conv2 / conv4 only where D-windows x tiles fill the
     # SMs: at 64 x 112 it never runs, so this arm runs at the shipped 320 x 1280, D = 72 shape
     ({'DFM_NO_NTK': '1'}, 'kitti_320x1280_d72', 'conv_tc<64->64,s1,src>@36x40x160', 'conv_tck'),

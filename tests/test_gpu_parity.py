@@ -71,6 +71,9 @@ CONV_CASES = [
     (32, 32, (6, 9, 21), (1, 1, 1), (1, 1, 1), False),
     (64, 32, (4, 8, 16), (1, 1, 1), (1, 1, 1), False),
     (32, 64, (8, 12, 20), (2, 2, 2), (1, 1, 1), False),
+    # stride 2 on independent output-channel groups (conv_tc.cuh, TcWeights::build)
+    (32, 32, (8, 10, 18), (2, 2, 2), (1, 1, 1), False),
+    (64, 32, (6, 8, 14), (2, 2, 2), (1, 1, 1), False),
     (64, 64, (4, 6, 10), (1, 1, 1), (1, 1, 1), False),
     (64, 64, (8, 8, 12), (2, 2, 2), (1, 1, 1), False),
     (64, 64, (3, 4, 5), (2, 2, 2), (1, 1, 1), True),
@@ -338,9 +341,9 @@ def full_size():
 def test_full_size_matches_oracle(full_size):
     """THE benchmarked configuration (BASELINE.json configs[1]: 370x1224 padded to 384x1248,
     D=112): DfMBackbone + DepthHead on the tensor-core path with every shortcut on (z-class
-    first layer, shortened mono tower, K-slice stride-2 convs) against one whole frame of the
-    CPU oracle (dfm_backbone.py:143-214, depth_head.py:190-212), all three backbone outputs
-    and depth_preds, max-norm and element-wise."""
+    first layer, shortened mono tower, cluster and K-slice stride-2 convs) against one whole
+    frame of the CPU oracle (dfm_backbone.py:143-214, depth_head.py:190-212), all three
+    backbone outputs and depth_preds, max-norm and element-wise."""
     torch.set_num_threads(max(1, (os.cpu_count() or 8)))
     cfg = full_size['cfg']
     with torch.no_grad():

@@ -1,10 +1,7 @@
 #!/usr/bin/env python
-"""Times the stride-2 hourglass convs (conv1 32->64, conv3 64->64) of both towers at the
-benchmarked KITTI shape (D = 112, 384 x 1248 features) on the two routes of conv1, alternately in
-one process: the cluster-shared bricks (default for the stereo tower) and the input-channel
-slices (DFM_S2_KSLICE=1, fed by TMA from a pre-split copy of the input).  The mono tower's conv1
-and conv3 run as input-channel slices on both and are a control for run-to-run drift.  Per layer
-it prints ms per step (CUDA events around every launch, presplit and slice-reduce passes
+"""Times the stride-2 hourglass convs of both towers at the benchmarked KITTI shape (D = 112,
+384 x 1248 features): conv1 (32->64) on cluster-shared bricks and conv3 (64->64) on input-channel
+slices.  Per layer it prints ms per step (CUDA events around every launch, the slice-reduce pass
 included), GB/s of the algorithmic bytes (inputs read once, output written once) and their share
 of the 3.35 TB/s data-sheet HBM bandwidth, next to the card name and power limit.  Run on an
 H100."""
@@ -38,12 +35,9 @@ def layer_of(key):
     """('conv1' | 'conv3', tower) of a profile row, or None."""
     cls, _, shape = key.partition('@')
     dz = int(shape.split('x')[0]) if shape else 0
-    # presplit rows carry the input depth, conv rows the output depth
-    if cls.startswith('presplit<32>'):
-        return 'conv1', 'stereo' if dz == D else 'mono'
-    if cls.startswith(('conv_tc_ks<32->64,s2', 'conv_tc_cl<32->64,s2')):
+    if cls.startswith('conv_tc_cl<32->64,s2'):
         return 'conv1', 'stereo' if dz == D // 2 else 'mono'
-    if cls.startswith(('conv_tc_ks<64->64,s2', 'conv_tc_cl<64->64,s2')):
+    if cls.startswith('conv_tc_ks<64->64,s2'):
         return 'conv3', 'stereo' if dz == D // 4 else 'mono'
     return None
 
@@ -65,53 +59,36 @@ def main():
     metas[0]['cam2img'] = syn.KITTI_P2.astype('float32').tolist()
     cur, prev = cur.cuda(), prev.cuda()
     cfg = syn.depth_cfg_for(D)
-    models = {}
-    for route in ('kslice', 'cluster'):
-        if route == 'kslice':
-            os.environ['DFM_S2_KSLICE'] = '1'
-        else:
-            os.environ.pop('DFM_S2_KSLICE', None)
-        m = modules.DfMBackbone(in_channels=C, depth_cfg=cfg).cuda().eval()
-        m.load_state_dict(params, strict=True)
-        with torch.no_grad():
-            m(cur, prev, copy.deepcopy(metas))     # weights are built (route fixed) on first use
-        models[route] = m
-    os.environ.pop('DFM_S2_KSLICE', None)
-    torch.cuda.synchronize()
-    ms = {r: {} for r in models}
-    rows = {r: {} for r in models}
+    m = modules.DfMBackbone(in_channels=C, depth_cfg=cfg).cuda().eval()
+    m.load_state_dict(params, strict=True)
+    ms, rows = {}, {}
     with torch.no_grad():
         for _ in range(ROUNDS):
-            for route, m in models.items():
-                m(cur, prev, copy.deepcopy(metas))
-                torch.cuda.synchronize()
-                capi.profile_enable(True)
-                capi.profile_report()
-                for _ in range(STEPS):
-                    m(cur, prev, metas)
-                torch.cuda.synchronize()
-                rep = capi.profile_report()
-                capi.profile_enable(False)
-                for k, v in rep.items():
-                    lt = layer_of(k)
-                    if lt is None:
-                        continue
-                    ms[route].setdefault(lt, []).append(v['ms'] / STEPS)
-                    rows[route].setdefault(lt, set()).add(k)
+            m(cur, prev, copy.deepcopy(metas))
+            torch.cuda.synchronize()
+            capi.profile_enable(True)
+            capi.profile_report()
+            for _ in range(STEPS):
+                m(cur, prev, metas)
+            torch.cuda.synchronize()
+            rep = capi.profile_report()
+            capi.profile_enable(False)
+            for k, v in rep.items():
+                lt = layer_of(k)
+                if lt is None:
+                    continue
+                ms.setdefault(lt, []).append(v['ms'] / STEPS)
+                rows.setdefault(lt, set()).add(k)
     out = dict(card=card(), shape=dict(D=D, feature_hw=[H, W]), rounds=ROUNDS,
                steps_per_round=STEPS, layers={})
-    for route in models:
-        for (layer, tower), per_round in sorted(ms[route].items()):
-            # rows of one layer are summed per round (conv + presplit / slice reduce)
-            n = len(rows[route][(layer, tower)])
-            sums = [sum(per_round[i:i + n]) for i in range(0, len(per_round), n)]
-            t = sorted(sums)[len(sums) // 2]
-            nbytes = algorithmic_bytes(layer, tower)
-            out['layers'][f'{layer}.{tower}.{route}'] = dict(
-                ms=round(t, 4), ms_rounds=[round(s, 4) for s in sums],
-                rows=sorted(rows[route][(layer, tower)]),
-                algorithmic_gb=round(nbytes / 1e9, 3), gbs=round(nbytes / t / 1e6, 1),
-                share_of_hbm=round(nbytes / t / 1e6 / (HBM_TBS * 1e3), 3))
+    for (layer, tower), per_round in sorted(ms.items()):
+        t = sorted(per_round)[len(per_round) // 2]
+        nbytes = algorithmic_bytes(layer, tower)
+        out['layers'][f'{layer}.{tower}'] = dict(
+            ms=round(t, 4), ms_rounds=[round(s, 4) for s in per_round],
+            rows=sorted(rows[(layer, tower)]),
+            algorithmic_gb=round(nbytes / 1e9, 3), gbs=round(nbytes / t / 1e6, 1),
+            share_of_hbm=round(nbytes / t / 1e6 / (HBM_TBS * 1e3), 3))
     print(json.dumps(out, indent=1))
 
 
